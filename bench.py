@@ -7,7 +7,7 @@
     python bench.py --scaling strong --frames F                    # ONE fixed job through the L2 seam, pairs sharded p mod world
 
 Workloads (config.workload):
-  vga_lightglue   (default; the driver's line) steady state of BASELINE.json configs[3] with the deep_front_end.yaml matcher: synthetic
+  vga_lightglue   (default) steady state of BASELINE.json configs[3] with the deep_front_end.yaml matcher: synthetic
                   640x480 sequence, Sequential(max_frame_lookahead=20), SuperPoint (<= 5000 keypoints) -> LightGlue (9 layers) ->
                   RANSAC-5pt.  One STEP = 2 new frames: 2 detections + 40 matches + 40 verifications.
   mp1_lightglue   configs[2]: 1024x1024 frames, SuperPoint -> LightGlue over all earlier frames.  STEP = 1 detection + 16 pairs.
@@ -66,18 +66,6 @@ WORKLOADS = {
         text="SuperPoint (1024 keypoints)+LightGlue+RANSAC-5pt, 640x480 sequence, lookahead 20: the launch-/sync-bound regime (early exit + pruning fire)",
         matcher_text="LightGlue 'stop' weights: early exit around layer 4-5, pruning at every layer (reference CPU semantics)"),
 }
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed `ncu --set full` captures
-# (profiles/): per workload, or None where no capture of that workload's launch shape exists
-DOMINANT_DRAM_BYTES = {
-    # profiles/r02_flash_ps.txt: the 16-problem launch (self- or cross-attention of a lock-step batch of 8 pairs at 5000 keypoints;
-    # 2 of every 3 k_flash_ps launches of this workload have that shape): 2.726 GB read + 0.086 GB written, against 0.33 GB of
-    # operands - the 64 heads of a batch do not fit L2 together, K / V tiles are re-read per 256-query block
-    "vga_lightglue": 2725897000 + 86424320,
-    # profiles/r02_conv_ps_1b.txt: conv1b, the largest of the nine k_conv_ps launch shapes (43 % of the network's FLOPs): input planes once
-    "superpoint_only": 78848256 + 5455104,
-}
-
-
 def config_of(name: str) -> dict:
     w = WORKLOADS[name]
     pairs = w["lookahead"] * w["new_frames"]
@@ -97,12 +85,12 @@ def measured_peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
-        return d.get("bf16_tflops_sustained", 1409.2), d.get("hbm_gbs", 6569.0), "measured"
-    return 1400.0, 6650.0, "fallback"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "measured"
+    return 989.0, 3350.0, "H100 SXM data sheet, dense"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
 
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -305,6 +293,55 @@ def _broadcast_weights(sds, world, dev):
             off += n
 
 
+DUMP_DESC_BYTES = 32 << 20  # descriptor share of the --dump-outputs budget (64 MB in all)
+
+
+def dump_outputs(out_dir: Path, step: dict) -> None:
+    """Write what the last timed step returned as float32 / float64 .npy files: per new frame the keypoints, scores and
+    descriptors (when all descriptors of the step exceed DUMP_DESC_BYTES, a fixed seeded sample of 1024 rows per frame, with
+    their row indices), per pair (ordered by (new frame, earlier frame)) the match index pairs and the verification result
+    (E, R, t, inlier count, inlier mask; NaN where a pair had too few matches)."""
+    import torch
+
+    out_dir.mkdir(parents=True, exist_ok=True)
+    frames = step["frames"]
+    arrays = {}
+    kp = [f.kp.float().cpu().numpy() for f in frames]
+    arrays["keypoints"] = np.concatenate(kp) if kp else np.zeros((0, 2), np.float32)
+    arrays["keypoint_counts"] = np.array([len(k) for k in kp], np.float64)
+    arrays["scores"] = np.concatenate([f.score.float().cpu().numpy() for f in frames]) if frames else np.zeros(0, np.float32)
+    full = sum(len(k) for k in kp) * 256 * 4 <= DUMP_DESC_BYTES
+    desc, rows = [], []
+    for i, f in enumerate(frames):
+        n = len(f.kp)
+        idx = np.arange(n) if full else np.sort(np.random.default_rng(1000 + i).choice(n, size=min(n, 1024), replace=False))
+        desc.append(f.desc[torch.as_tensor(idx, device=f.desc.device, dtype=torch.long)].float().cpu().numpy())
+        rows.append(np.stack([np.full(len(idx), i), idx], 1).astype(np.float64))
+    arrays["descriptors"] = np.concatenate(desc) if desc else np.zeros((0, 256), np.float32)
+    arrays["descriptor_rows"] = np.concatenate(rows) if rows else np.zeros((0, 2), np.float64)
+    keys = sorted(step["pairs"])
+    if keys:
+        ms, counts, E, R, t, ninl, masks = [], [], [], [], [], [], []
+        for k in keys:
+            m, fut = step["pairs"][k]
+            e, r, tt, n_in, mask = fut.result()
+            ms.append(m.cpu().numpy().astype(np.float64).reshape(-1, 2))
+            counts.append(len(ms[-1]))
+            E.append(np.full(9, np.nan) if e is None else np.asarray(e, np.float64).reshape(9))
+            R.append(np.full(9, np.nan) if r is None else np.asarray(r, np.float64).reshape(9))
+            t.append(np.full(3, np.nan) if tt is None else np.asarray(tt, np.float64).reshape(3))
+            ninl.append(float(n_in))
+            masks.append(mask.cpu().numpy().astype(np.float64).reshape(-1))
+        arrays["pair_index"] = np.array(keys, np.float64)
+        arrays["matches"] = np.concatenate(ms)
+        arrays["match_counts"] = np.array(counts, np.float64)
+        arrays["E"], arrays["R"], arrays["t"] = np.stack(E), np.stack(R), np.stack(t)
+        arrays["inlier_counts"] = np.array(ninl, np.float64)
+        arrays["inlier_mask"] = np.concatenate(masks)
+    for name, a in arrays.items():
+        np.save(out_dir / f"{name}.npy", a)
+
+
 def run_cuda(args):
     import torch
     import torch.distributed as dist
@@ -346,37 +383,47 @@ def run_cuda(args):
     stats = {"matches": 0, "inliers": 0, "pairs": 0, "stops": 0, "keypoints": 0, "frames": 0}
 
     stats_lock = threading.Lock()
+    # --dump-outputs: references to what the latest step returned (device tensors and verification results; no copies in the step)
+    last_step = {"frames": [], "pairs": {}}
 
     def step_device(c):
         pending = []
+        out_frames, out_pairs = [], {}
+        last_step["frames"], last_step["pairs"] = out_frames, out_pairs
         if not w["matcher"]:  # detect-describe only: every frame of the step enqueued before the first count is read
             for f in fe.detect_many([frames_dev[(c + j) % len(frames_dev)] for j in range(NEW_FRAMES)]):
                 stats["keypoints"] += len(f)
                 stats["frames"] += 1
+                out_frames.append(f)
             return
         for j in range(NEW_FRAMES):
             f = fe.detect(frames_dev[(c + j) % len(frames_dev)])
             stats["keypoints"] += len(f)
             stats["frames"] += 1
+            out_frames.append(f)
             if not w["matcher"]:
                 continue
             prevs = list(window)
             if w["matcher"] == "lightglue":
                 # lock-step batches of 8 pairs (b2_lightglue_match_batched_dev) over MATCH_LANES concurrent LightGlue instances;
                 # a batch's verifications are queued the moment it completes and overlap the other batches' matcher kernels
-                def on_chunk(c0, res, prevs=prevs, f=f):
+                def on_chunk(c0, res, prevs=prevs, f=f, j=j):
                     with stats_lock:
-                        for prev, (m, stop) in zip(prevs[c0:c0 + len(res)], res):
-                            pending.append(fe.verify_async(prev, f, m, cal, cal, THR_PX))
+                        for i, (prev, (m, stop)) in enumerate(zip(prevs[c0:c0 + len(res)], res)):
+                            fut = fe.verify_async(prev, f, m, cal, cal, THR_PX)
+                            pending.append(fut)
+                            out_pairs[(j, c0 + i)] = (m, fut)
                             stats["matches"] += int(m.shape[0])
                             stats["stops"] += stop
                             stats["pairs"] += 1
 
                 fe.match_many([(prev, f) for prev in prevs], on_chunk=on_chunk)
             else:
-                def on_pair(i, m, prevs=prevs, f=f):  # a pair's verification is queued the moment its matches exist
+                def on_pair(i, m, prevs=prevs, f=f, j=j):  # a pair's verification is queued the moment its matches exist
                     with stats_lock:
-                        pending.append(fe.verify_async(prevs[i], f, m, cal, cal, THR_PX))
+                        fut = fe.verify_async(prevs[i], f, m, cal, cal, THR_PX)
+                        pending.append(fut)
+                        out_pairs[(j, i)] = (m, fut)
                         stats["matches"] += int(m.shape[0])
                         stats["pairs"] += 1
 
@@ -424,6 +471,8 @@ def run_cuda(args):
     if not in_graph:
         fe.profile_start(w["dominant"])
     total_ms, cursor = timed_pass(cursor)
+    if args.dump_outputs and rank == 0:  # rank 0's stretch of the sequence (each rank has its own seeded frames)
+        dump_outputs(Path(args.dump_outputs), last_step)
     if not in_graph:
         k_ms, k_launches, k_work = fe.profile_stop()
         prof_total_ms = total_ms
@@ -580,8 +629,7 @@ def run_cuda(args):
             "warmup": args.warmup, "ms_per_step": max_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
             "data": "synthetic", "config": config_of(wname), "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches),
             "roofline": {"bound": "tensor", "kernel": w["dominant"], "achieved": achieved, "peak": tf_peak, "unit": "TFLOP/s",
-                         "frac": achieved / tf_peak, "traffic": DOMINANT_DRAM_BYTES.get(wname),
-                         "traffic_unit": "dram__bytes_read.sum + dram__bytes_write.sum of one launch (ncu --set full capture under profiles/, the launch shape named in bench.py DOMINANT_DRAM_BYTES); null = no capture of this workload's launch shape",
+                         "frac": achieved / tf_peak, "traffic": None, "traffic_unit": "not measured",
                          "peak_source": f"bf16_tflops_sustained ({peak_src})",
                          "kernel_ms_per_step": k_ms / args.steps, "kernel_launches_per_step": k_launches / args.steps,
                          "kernel_share_of_step": k_ms / prof_total_ms if prof_total_ms else None,
@@ -589,10 +637,10 @@ def run_cuda(args):
                                            f"which per-launch events cannot see); that pass took {prof_total_ms / args.steps:.2f} ms per step") if in_graph
                          else ("CUDA events around every launch inside the timed pass" +
                                (f"; {DETECT_LANES} SuperPoint lanes run concurrently, so a launch shares the SMs with other lanes' kernels and "
-                                "the summed kernel time exceeds the step time (the kernel alone: profiles/r02_conv_ps_*.txt)"
+                                "the summed kernel time exceeds the step time"
                                 if not w["matcher"] and DETECT_LANES > 1 else
                                 "; 3 SuperGlue instances match pairs concurrently (match_superglue_many), so a launch shares the SMs with the other "
-                                "lanes' kernels: per-launch time, and with it this fraction, is inflated by the contention (one lane: 0.24)"
+                                "lanes' kernels: per-launch time, and with it this fraction, is inflated by the contention"
                                 if w["matcher"] == "superglue" else "")),
                          "note": "split-fp16 x3 products: tensor-pipe FLOPs are 3x the algorithmic FLOPs counted here (ceiling of frac = 0.33)"},
             "work": {"matches_per_pair": stats["matches"] / max(1, stats["pairs"]), "inliers_per_pair": stats["inliers"] / max(1, stats["pairs"]),
@@ -690,7 +738,12 @@ def main():
                     help="opt-in mode: the reference's CUDA numerics for attention (fp16 flash SDPA, one MMA per product); NOT the "
                          "parity-pinned default - the line says so in config.matcher")
     ap.add_argument("--lg-batch", type=int, default=0, help="experiments: pairs per lock-step LightGlue batch inside the library (0 = default)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what rank 0's last timed step returned to DIR/<name>.npy (float32 / float64, <= 64 MB); "
+                         "weak-scaling CUDA path only")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "cuda" or args.scaling != "weak"):
+        ap.error("--dump-outputs is only supported with --impl cuda --scaling weak")
     global FP16_ATTN
     FP16_ATTN = bool(args.fp16_attention)
     if args.impl == "reference":

@@ -113,7 +113,7 @@ class Context:
         rc = self._lib.b2_create(int(device), C.byref(h))
         if rc != 0 or not h:
             raise B200Error(
-                f"b2_create(device={device}) failed with {rc}: an sm_100 (B200) GPU is required; there is no CPU fallback")
+                f"b2_create(device={device}) failed with {rc}: an sm_90 (H100) GPU is required; there is no CPU fallback")
         self.handle = h
         self.device = device
 

@@ -1,4 +1,4 @@
-"""In-tree build of libgtsfm_b200.so (nvcc, sm_100a only).  `python -m gtsfm_b200.build` or __graft_entry__.build()."""
+"""In-tree build of libgtsfm_b200.so (nvcc, sm_90a only).  `python -m gtsfm_b200.build` or __graft_entry__.build()."""
 from __future__ import annotations
 
 import os
@@ -14,12 +14,12 @@ OBJ = PKG / "csrc" / "_obj"
 LIB = PKG / "libgtsfm_b200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
     # 5-point solver: null space by five Householder reflections (static indexing, registers) instead of Jacobi sweeps on the
-    # 9 x 9 Gram matrix (run-time indexed local memory: 1.1 ms per hypothesis batch on B200); tests/cpp/test_ransac_math.cpp
+    # 9 x 9 Gram matrix (run-time indexed local memory); tests/cpp/test_ransac_math.cpp
     # builds both variants on the host
     "-DB2_FIVEPT_QR",
 ]
@@ -64,7 +64,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
             list(ex.map(compile_one, jobs))
     objs = [OBJ / (s.stem + ".o") for s in srcs]
     if jobs or not LIB.exists() or force:
-        cmd = [nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(LIB), *map(str, objs)]
+        cmd = [nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(LIB), *map(str, objs)]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -12,7 +12,7 @@ extern "C" int b2_create(int device, b2_context** out) {
   if (cudaGetDeviceCount(&count) != cudaSuccess || device < 0 || device >= count) return B2_ERR_CUDA;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return B2_ERR_CUDA;
-  if (prop.major != 10) return B2_ERR_STATE;  // sm_100a cubins only: fail loudly on anything else
+  if (prop.major != 9 || prop.minor != 0) return B2_ERR_STATE;  // sm_90a cubins only: fail loudly on anything else
   if (cudaSetDevice(device) != cudaSuccess) return B2_ERR_CUDA;
   b2_context* ctx = new b2_context();
   ctx->device = device;

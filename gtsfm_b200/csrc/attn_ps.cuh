@@ -1,43 +1,23 @@
-// Persistent warp-specialised tcgen05 + TMA flash attention over a BATCH of problems, A operands in TMEM ("TS" MMAs),
-// split-fp16 operands (~fp32 accuracy).
+// Persistent warp-specialised wgmma + TMA flash attention over a BATCH of problems, split-fp16 operands (~fp32 accuracy).
 //
 //   O[Nq][256] = softmax(scale * Q K^T) V per head; q / k / v arrive as fp16 hi / lo planes with UNSCALED lo
 //   (x ~= hi + lo, lo = fp16(x - hi)), the output leaves as hi / lo planes with the usual 2^11-scaled lo.
 //
-// Why TMEM operands: a 128 x 64 x 16 SS-mode MMA reads 4 KB of A and 2 KB of B from shared memory per 32 tensor cycles
-// (192 B/clk > the 128 B/clk the SM's shared memory delivers).  Here Q lives in TMEM for a whole segment and P is written
-// back over its own logits in TMEM, so shared memory only carries the K / V tiles (B operands).
-//
-// One CTA (352 threads, one per SM) owns TWO 128-query tiles of one head at a time and streams 64-key tiles.
-// TMEM (512 columns; per query tile q at q * 256):
-//     [  0, 64) logits buffer 0: S (128 x 64 fp32), overwritten in place by P: hi = columns [0, 32), lo = [32, 64)
-//     [ 64,128) logits buffer 1                                                 (column c = keys 2c, 2c + 1 as half2)
-//     [128,192) O accumulator (128 x 64 fp32), accumulated by the tensor core across ALL key tiles of a segment
-//     [192,224) Q hi, [224,256) Q lo  (column c = dims 2c, 2c + 1)
+// One CTA (288 threads, one per SM) owns TWO 128-query tiles of one head at a time and streams 64-key tiles.
 //   warp 8 lane 0 : TMA producer - K and V tiles through one 4-entry ring (128-byte swizzled, zero OOB fill)
-//   warps 9, 10   : MMA issuers of query tile 0 / 1 (warp-uniform issue, one elected lane; warp 9 also owns the TMEM
-//                   allocation).  Two issuers because a barrier wait costs the issuing warp 150-250 cycles and the
-//                   tcgen05 queue is shallow: while one warp waits for its P tile the other's MMAs keep the pipe busy.
-//                   Per key tile i, issuer q:
-//                     PV_q(i): O_q += Ph Vh + Ph Vl + Pl Vh   (A = P from TMEM, B = V MN-major)      12 tcgen05.mma
-//                     S_q(i+2) = Qh Kh^T + Qh Kl^T + Ql Kh^T  (A = Q from TMEM) into buffer i & 1    12 tcgen05.mma
-//                   the logits run two key tiles ahead of the softmax.
-//   warps 0-3 / 4-7: softmax warpgroup of query tile 0 / 1, one thread per query row (= TMEM lane): tcgen05.ld S, base-2
-//                   online softmax with a LAZY reference maximum (O and l are only rescaled when the row maximum grew by
-//                   more than 2^8 - P then stays <= 256, exact in the hi / lo split - so O normally never leaves TMEM),
-//                   P = 2^(s - m) split to fp16 hi / lo and stored over S with tcgen05.st.
-// Hand-offs are mbarriers: TMA complete_tx (kv_full), tcgen05.commit (s_full, o_full, kv_empty) and 128-thread arrivals
-// (q_ready, p_full).
+//   warps 0-3 / 4-7: consumer warpgroup of query tile 0 / 1, Q hi / lo in shared memory.  Per key tile and 64-row slab:
+//                   S = Qh Kh^T + Qh Kl^T + Ql Kh^T (wgmma from shared memory); base-2 online softmax on the fragment with a
+//                   LAZY reference maximum (rescale only when the row maximum grew by more than 2^8: P <= 256 stays exact
+//                   in the hi / lo split); O += Ph Vh + Ph Vl + Pl Vh (P from registers, V MN-major), O kept in registers.
 //
 // Schedule ("stream-K" over the key dimension): the whole launch - every problem of the batch, i.e. the self- or
 // cross-attention of all images of up to 8 pairs - is ONE linear space of (item, key tile) units, item = (problem, head,
 // 256-query block), cut into equal contiguous ranges, one per SM.  A CTA therefore runs a few SEGMENTS (item, key-tile
-// range) back to back: TMEM stays allocated, the barriers keep running phase counters, the TMA producer streams the next
-// segment's K / V tiles while the current one drains, and the next segment's Q is stored and its first logits issued
-// before the softmax warps write the current segment's result.  A segment that covers its item completely writes the
-// normalised output planes; otherwise it writes an un-normalised partial (O, m, l), and the LAST segment of an item to
-// arrive (device-scope counter, stream-K "fix-up") combines the partials in the same kernel.  All barrier parities are
-// functions of running counters (ring entry `ge`, tile `gt`, segment `seg`) that every role advances identically.
+// range) back to back: the barriers keep running phase counters and the TMA producer streams the next segment's K / V
+// tiles while the current one drains.  A segment that covers its item completely writes the normalised output planes;
+// otherwise it writes an un-normalised partial (O, m, l), and the LAST segment of an item to arrive (device-scope counter,
+// stream-K "fix-up") combines the partials in the same kernel.  All barrier parities are functions of the running ring
+// counter `ge` that every role advances identically.
 #pragma once
 #include "tma.cuh"
 
@@ -47,9 +27,10 @@ constexpr int AS_NS = 4;                     // ring depth; entry e holds K tile
 constexpr int AS_HALF = 2 * AW_KV_BYTES;     // hi + lo plane of one 64 x 64 tile = 16 KB
 constexpr int AS_STAGE = 2 * AS_HALF;        // K part at +0, V part at +AS_HALF
 constexpr int AS_TILE_BYTES = AS_NS * AS_STAGE;
-constexpr size_t AS_SMEM = AS_TILE_BYTES + 1024 + 512;
-constexpr uint32_t AS_COL_O = 128, AS_COL_Q = 192;
-constexpr int AS_THREADS = 352;     // 8 softmax warps + TMA producer warp + 2 MMA issuer warps
+constexpr int AS_Q_PLANE = AW_Q * AW_D * 2;  // 16 KB: one plane of a 128-query tile
+constexpr int AS_Q_BYTES = 2 * 2 * AS_Q_PLANE;  // hi + lo planes of both query tiles
+constexpr size_t AS_SMEM = AS_TILE_BYTES + AS_Q_BYTES + 1024 + 512;
+constexpr int AS_THREADS = 256 + 32;  // 2 consumer warpgroups + TMA producer warp
 constexpr float AS_RESCALE = 8.0f;  // log2 of the largest P allowed before the reference maximum is refreshed
 constexpr int AP_MAXP = 16;         // problems per launch (2 images x 8 pairs)
 
@@ -103,7 +84,7 @@ __device__ __forceinline__ AttnPsSeg attn_ps_decode(const AttnPsArgs& a, int w, 
 }
 
 // SINGLE = the reference's CUDA numerics (lightglue.py:116-121: q, k, v cast to half, fp16 flash SDPA, result cast back):
-// only the hi planes take part - ONE tcgen05.mma per product instead of three - and the output is rounded to fp16.  Opt-in
+// only the hi planes take part - ONE wgmma per product instead of three - and the output is rounded to fp16.  Opt-in
 // (b2_lightglue_params.fp16_attention); the default exact path reproduces the fp32 CPU front-end.
 template <bool SINGLE>
 static __global__ void __launch_bounds__(AS_THREADS, 1) k_flash_ps(const __grid_constant__ AttnPsMaps maps, const __grid_constant__ AttnPsArgs args) {
@@ -111,31 +92,20 @@ static __global__ void __launch_bounds__(AS_THREADS, 1) k_flash_ps(const __grid_
   const uint32_t raw = tc::smem_u32(ap_raw);
   const uint32_t smem0 = (raw + 1023u) & ~1023u;
   unsigned char* sm = ap_raw + (smem0 - raw);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + AS_TILE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + AS_TILE_BYTES + AS_Q_BYTES);
   uint64_t* kv_full = bars;                 // [AS_NS]
-  uint64_t* kv_empty = kv_full + AS_NS;     // [AS_NS]
-  uint64_t* s_full = kv_empty + AS_NS;      // [4] query tile x logits buffer
-  uint64_t* p_full = s_full + 4;            // [2]
-  uint64_t* o_full = p_full + 2;            // [2]
-  uint64_t* q_ready = o_full + 2;           // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(q_ready + 2);
-  volatile int* last_flag = reinterpret_cast<volatile int*>(tmem_slot + 2);  // [2] per softmax warpgroup
+  uint64_t* kv_empty = kv_full + AS_NS;     // [AS_NS] one arrival per consumer warp
+  volatile int* last_flag = reinterpret_cast<volatile int*>(kv_empty + AS_NS);  // [2] per consumer warpgroup
 
   const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
   const int w_begin = blockIdx.x * args.quota;
   const int w_end = min(args.W, w_begin + args.quota);
 
   if (t == 0) {
-    for (int i = 0; i < AS_NS; ++i) tc::mbar_init(&kv_full[i], 1), tc::mbar_init(&kv_empty[i], 2);  // released by both issuers
-    for (int i = 0; i < 4; ++i) tc::mbar_init(&s_full[i], 1);
-    for (int i = 0; i < 2; ++i) tc::mbar_init(&p_full[i], 128), tc::mbar_init(&o_full[i], 1), tc::mbar_init(&q_ready[i], 128);
+    for (int i = 0; i < AS_NS; ++i) tc::mbar_init(&kv_full[i], 1), tc::mbar_init(&kv_empty[i], 8);
     tc::fence_mbar_init();
   }
-  if (warp == 9) tc::tmem_alloc(tmem_slot, 512);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
   bool ok = true;
 
   if (warp == 8) {
@@ -167,223 +137,182 @@ static __global__ void __launch_bounds__(AS_THREADS, 1) k_flash_ps(const __grid_
         w += sg.T;
       }
     }
-  } else if (warp >= 9) {
-    // ===== MMA issuer of query tile q (whole warp, one elected lane issues) =====
-    const int q = warp - 9;
-    const uint32_t idS = tc::idesc_f16(AW_Q, AW_KV);                        // Q K^T: A (TMEM) and B K-major
-    const uint32_t idO = tc::idesc_f16(AW_Q, AW_D) | tc::IDESC_B_MN_MAJOR;  // P V: V as stored = MN-major
-    const uint32_t tQh = tmem + q * 256 + AS_COL_Q, tQl = tQh + 32;
-    const uint32_t tO = tmem + q * 256 + AS_COL_O;
-    int ge = 0, gt = 0, seg = 0;
-    for (int w = w_begin; w < w_end; ++seg) {
-      const AttnPsSeg sg = attn_ps_decode(args, w, w_end);
-      const int T = sg.T;
-      auto issue_S = [&](int j) {  // logits of the segment's key tile j: ring entry ge + j, logits buffer (gt + j) & 1
-        const int s = (ge + j) % AS_NS, buf = (gt + j) & 1;
-        const uint64_t dKh = tc::smem_desc_sw128(smem0 + s * AS_STAGE);
-        const uint64_t dKl = tc::smem_desc_sw128(smem0 + s * AS_STAGE + AW_KV_BYTES);
-        const uint32_t tS = tmem + q * 256 + buf * 64;
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          const uint64_t adv = (uint64_t)(ks * 2);
-          const uint32_t ac = (uint32_t)(ks * 8);
-          tc::umma_f16_ts_w(tS, tQh + ac, dKh + adv, idS, ks ? 1u : 0u);
-          if (!SINGLE) {
-            tc::umma_f16_ts_w(tS, tQh + ac, dKl + adv, idS, 1u);
-            tc::umma_f16_ts_w(tS, tQl + ac, dKh + adv, idS, 1u);
-          }
-        }
-        tc::umma_commit_w(&s_full[q * 2 + buf]);
-      };
-      auto issue_PV = [&](int j) {  // V tile j sits in ring entry ge + j + 2; P in logits buffer (gt + j) & 1
-        const int s = (ge + j + 2) % AS_NS, buf = (gt + j) & 1;
-        const uint64_t dVh = tc::smem_desc_sw128_mn(smem0 + s * AS_STAGE + AS_HALF);
-        const uint64_t dVl = tc::smem_desc_sw128_mn(smem0 + s * AS_STAGE + AS_HALF + AW_KV_BYTES);
-        const uint32_t tPh = tmem + q * 256 + buf * 64, tPl = tPh + 32;
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          const uint32_t ac = (uint32_t)(ks * 8);
-          const uint64_t advV = (uint64_t)(ks * 128);
-          tc::umma_f16_ts_w(tO, tPh + ac, dVh + advV, idO, (j | ks) ? 1u : 0u);
-          if (!SINGLE) {
-            tc::umma_f16_ts_w(tO, tPh + ac, dVl + advV, idO, 1u);
-            tc::umma_f16_ts_w(tO, tPl + ac, dVh + advV, idO, 1u);
-          }
-        }
-        tc::umma_commit_w(&o_full[q]);
-      };
-      ok = tc::mbar_wait(&q_ready[q], seg & 1) && ok;  // this segment's Q rows are in TMEM
-      for (int j = 0; j < 2 && j < T; ++j) {
-        const int g = ge + j;
-        ok = tc::mbar_wait(&kv_full[g % AS_NS], (g / AS_NS) & 1) && ok;
-        __syncwarp();
-        tc::fence_after_sync();
-        issue_S(j);
-        tc::umma_commit_w(&kv_empty[g % AS_NS]);
-      }
-      if (T == 1) {  // ring entry 1 of a one-tile segment is empty but still cycles through the ring
-        const int g = ge + 1;
-        ok = tc::mbar_wait(&kv_full[g % AS_NS], (g / AS_NS) & 1) && ok;
-        __syncwarp();
-        tc::umma_commit_w(&kv_empty[g % AS_NS]);
-      }
-      bool h_kv = false;
-      for (int i = 0; i < T; ++i) {
-        const int g = ge + i + 2;  // ring entry: V tile i and (if any) K tile i + 2
-        const bool more = i + 2 < T;
-        if (!h_kv) ok = tc::mbar_wait(&kv_full[g % AS_NS], (g / AS_NS) & 1) && ok;
-        ok = tc::mbar_wait(&p_full[q], (gt + i) & 1) && ok;  // P_q(i) stored over S_q(i); O_q rescaled if it had to be
-        __syncwarp();
-        tc::fence_after_sync();
-        h_kv = (i + 1 < T) && tc::mbar_test(&kv_full[(g + 1) % AS_NS], ((g + 1) / AS_NS) & 1);
-        issue_PV(i);
-        if (more) issue_S(i + 2);  // overwrites buffer (gt + i) & 1 = P_q(i): in issue order after PV_q(i) has read it
-        tc::umma_commit_w(&kv_empty[g % AS_NS]);
-      }
-      ge += T + 2, gt += T;
-      w += T;
-    }
   } else {
-    // ===== softmax warpgroups: q = 0 (warps 0-3), q = 1 (warps 4-7); thread = query row = TMEM lane =====
+    // ===== consumer warpgroup q: query rows q * 128 + slab * 64 + rq (+ 8) =====
     const int q = warp >> 2;
     const int r = t & 127;
-    const uint32_t lane_off = (uint32_t)((warp & 3) * 32) << 16;
-    const uint32_t tB = tmem + q * 256 + lane_off, tO = tB + AS_COL_O;
-    const float c2 = args.scale * 1.4426950408889634f;
+    const int rq = (warp & 3) * 16 + (lane >> 2);  // fragment rows rq, rq + 8 of a slab
+    const int c2 = (lane & 3) * 2;                 // fragment columns 8j + c2, + 1
+    const uint32_t sQ = smem0 + AS_TILE_BYTES + q * 2 * AS_Q_PLANE;
+    const float c2s = args.scale * 1.4426950408889634f;
+    auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + q) : "memory"); };
+    auto release = [&](int g) { if (lane == 0) tc::mbar_arrive(&kv_empty[g % AS_NS]); };
 
-    auto store_q = [&](const AttnPsSeg& sg) {  // this thread's query row of segment sg -> TMEM (zero rows past the end)
-      const AttnPsProblem& pr = args.p[sg.z];
-      const int qrow = sg.q0 + q * AW_Q + r;
-      uint32_t wv[32];
-#pragma unroll
-      for (int pl = 0; pl < (SINGLE ? 1 : 2); ++pl) {
-        const __half* src = (pl ? pr.Ql : pr.Qh) + ((size_t)sg.h * pr.Nq + qrow) * 64;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          uint4 v = make_uint4(0u, 0u, 0u, 0u);
-          if (qrow < pr.Nq) v = __ldg(reinterpret_cast<const uint4*>(src) + c);
-          wv[4 * c] = v.x, wv[4 * c + 1] = v.y, wv[4 * c + 2] = v.z, wv[4 * c + 3] = v.w;
-        }
-        tc::tmem_st32(tB + AS_COL_Q + pl * 32, wv);
-      }
-      tc::tmem_st_wait();
-      tc::fence_before_sync();
-      tc::mbar_arrive(&q_ready[q]);
-    };
-
-    int gt = 0;
-    if (w_begin < w_end) store_q(attn_ps_decode(args, w_begin, w_end));
+    int ge = 0;
     for (int w = w_begin; w < w_end;) {
       const AttnPsSeg sg = attn_ps_decode(args, w, w_end);
       const AttnPsProblem& pr = args.p[sg.z];
       const int T = sg.T, Nk = pr.Nk;
-      float m_ref = -INFINITY, l_i = 0.f;
-      bool h_s = false;  // pre-polled: logits of the next tile already complete
-      for (int i = 0; i < T; ++i) {
-        const int gi = gt + i;
-        if (!h_s) ok = tc::mbar_wait(&s_full[q * 2 + (gi & 1)], (gi >> 1) & 1) && ok;
-        tc::fence_after_sync();
-        const uint32_t tS = tB + (gi & 1) * 64;
-        const int k0 = (sg.tile0 + i) * AW_KV;
-        float a[64];
-        tc::tmem_ld64(tS, a);
-        if (k0 + AW_KV > Nk) {
+      {  // this thread's query row -> shared memory, 128-byte swizzled (zero rows past the end)
+        const int qrow = sg.q0 + q * AW_Q + r;
+        wg_bar();  // the previous segment's MMAs of every warp of the group have read Q
 #pragma unroll
-          for (int j = 0; j < 64; ++j)
-            if (k0 + j >= Nk) a[j] = -INFINITY;  // 2^(-inf) = 0
-        }
-        float mx = a[0];
-#pragma unroll
-        for (int j = 1; j < 64; ++j) mx = fmaxf(mx, a[j]);
-        const float m_new = fmaxf(m_ref, mx * c2);
-        // PV_q(i-1) landed?  (pre-poll, consumed below; the previous segment's last phase was consumed by its epilogue)
-        bool waited = i == 0 || tc::mbar_test(&o_full[q], (gi - 1) & 1);
-        if (__any_sync(0xffffffffu, m_new - m_ref > AS_RESCALE)) {  // also true on the first tile (m_ref = -inf)
-          const float corr = tc::ex2(m_ref - m_new);
-          l_i *= corr;
-          if (i > 0) {  // bring O (in TMEM) to the new reference
-            if (!waited) ok = tc::mbar_wait(&o_full[q], (gi - 1) & 1) && ok;
-            tc::fence_after_sync();
-            waited = true;
-            float o[64];
-            tc::tmem_ld64(tO, o);
-            uint32_t ow[64];
-#pragma unroll
-            for (int j = 0; j < 64; ++j) ow[j] = __float_as_uint(o[j] * corr);
-            tc::tmem_st32(tO, ow);
-            tc::tmem_st32(tO + 32, ow + 32);
-          }
-          m_ref = m_new;
-        }
-        uint32_t ph[32], pl[32];
-        float2 rs2 = make_float2(0.f, 0.f);
-        const float2 c22 = make_float2(c2, c2), nm2 = make_float2(-m_ref, -m_ref), neg1 = make_float2(-1.f, -1.f);
-#pragma unroll
-        for (int jj = 0; jj < 32; ++jj) {  // packed fp32 pairs: the softmax warps are issue-slot bound
-          const float2 e = tc::ffma2(make_float2(a[2 * jj], a[2 * jj + 1]), c22, nm2);
-          const float2 p2 = make_float2(tc::ex2(e.x), tc::ex2(e.y));
-          rs2 = tc::fadd2(rs2, p2);
-          const __half2 hh = __floats2half2_rn(p2.x, p2.y);
-          ph[jj] = *reinterpret_cast<const uint32_t*>(&hh);
-          if (!SINGLE) {
-            const float2 d = tc::ffma2(__half22float2(hh), neg1, p2);  // p - hi, exact
-            const __half2 ll = __floats2half2_rn(d.x, d.y);
-            pl[jj] = *reinterpret_cast<const uint32_t*>(&ll);
-          }
-        }
-        l_i += rs2.x + rs2.y;
-        h_s = (i + 1 < T) && tc::mbar_test(&s_full[q * 2 + ((gi + 1) & 1)], ((gi + 1) >> 1) & 1);
-        tc::tmem_st32(tS, ph);  // P_i over S_i (this thread's own row; every column of it is already in registers)
-        if (!SINGLE) tc::tmem_st32(tS + 32, pl);
-        tc::tmem_st_wait();
-        if (!waited) ok = tc::mbar_wait(&o_full[q], (gi - 1) & 1) && ok;  // every phase is observed once
-        tc::fence_before_sync();
-        tc::mbar_arrive(&p_full[q]);
-      }
-      gt += T;
-      w += T;
-      // next segment's Q goes in now (all logits of this segment have completed), so its first MMAs overlap our epilogue
-      if (w < w_end) store_q(attn_ps_decode(args, w, w_end));
-      // ---- this segment's result ----
-      float o[64];
-      ok = tc::mbar_wait(&o_full[q], (gt - 1) & 1) && ok;
-      tc::fence_after_sync();
-      tc::tmem_ld64(tO, o);
-      tc::fence_before_sync();  // our read of O is ordered before the next segment's first PV (gated by our p_full arrival)
-      const int qrow = sg.q0 + q * AW_Q + r;
-      if (sg.nsplits == 1) {
-        if (qrow < pr.Nq) {
-          const float inv = 1.0f / l_i;
-          uint4* dh = reinterpret_cast<uint4*>(pr.Oh + (size_t)qrow * 256 + sg.h * 64);
-          uint4* dl = reinterpret_cast<uint4*>(pr.Ol + (size_t)qrow * 256 + sg.h * 64);
+        for (int pl = 0; pl < (SINGLE ? 1 : 2); ++pl) {
+          const __half* src = (pl ? pr.Ql : pr.Qh) + ((size_t)sg.h * pr.Nq + qrow) * 64;
+          unsigned char* dst = sm + AS_TILE_BYTES + q * 2 * AS_Q_PLANE + pl * AS_Q_PLANE + r * 128;
 #pragma unroll
           for (int c = 0; c < 8; ++c) {
-            uint32_t hi[4], lo[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              if (SINGLE) {  // SDPA returns half: the message is the fp16 rounding of the fp32 accumulator
-                const __half2 hh = __floats2half2_rn(tc::clamp_h(o[8 * c + 2 * i] * inv), tc::clamp_h(o[8 * c + 2 * i + 1] * inv));
-                hi[i] = *reinterpret_cast<const uint32_t*>(&hh), lo[i] = 0u;
-              } else {
-                tc::split2(o[8 * c + 2 * i] * inv, o[8 * c + 2 * i + 1] * inv, hi[i], lo[i]);
-              }
-            }
-            dh[c] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            dl[c] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+            uint4 v = make_uint4(0u, 0u, 0u, 0u);
+            if (qrow < pr.Nq) v = __ldg(reinterpret_cast<const uint4*>(src) + c);
+            *reinterpret_cast<uint4*>(dst + ((c ^ (r & 7)) << 4)) = v;
           }
         }
+        tc::fence_proxy_async();  // generic-proxy stores -> visible to the tensor core
+        wg_bar();
+      }
+      float o[2][32];
+      float m_ref[2][2], l_i[2][2];
+#pragma unroll
+      for (int sl = 0; sl < 2; ++sl)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) m_ref[sl][h] = -INFINITY, l_i[sl][h] = 0.f;
+      for (int j = 0; j < 2; ++j) ok = tc::mbar_wait(&kv_full[(ge + j) % AS_NS], ((ge + j) / AS_NS) & 1) && ok;
+      if (T == 1) release(ge + 1);  // ring entry 1 of a one-tile segment is empty but still cycles through the ring
+      for (int i = 0; i < T; ++i) {
+        const int gv = ge + i + 2;  // ring entry: V tile i and (if any) K tile i + 2
+        ok = tc::mbar_wait(&kv_full[gv % AS_NS], (gv / AS_NS) & 1) && ok;
+        const uint32_t sK = smem0 + ((ge + i) % AS_NS) * AS_STAGE, sV = smem0 + (gv % AS_NS) * AS_STAGE + AS_HALF;
+        const uint64_t dKh = tc::wg_desc_sw128(sK), dKl = tc::wg_desc_sw128(sK + AW_KV_BYTES);
+        const uint64_t dVh = tc::wg_desc_sw128(sV), dVl = tc::wg_desc_sw128(sV + AW_KV_BYTES);
+        const int k0 = (sg.tile0 + i) * AW_KV;
+#pragma unroll
+        for (int sl = 0; sl < 2; ++sl) {
+          const uint64_t dQh = tc::wg_desc_sw128(sQ + sl * (64 * 128)), dQl = tc::wg_desc_sw128(sQ + AS_Q_PLANE + sl * (64 * 128));
+          float a[32];
+          tc::wg_fence();
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) {
+            const uint64_t adv = (uint64_t)(ks * 2);
+            tc::wg_ss_n64(a, dQh + adv, dKh + adv, ks ? 1u : 0u);
+            if (!SINGLE) {
+              tc::wg_ss_n64(a, dQh + adv, dKl + adv, 1u);
+              tc::wg_ss_n64(a, dQl + adv, dKh + adv, 1u);
+            }
+          }
+          tc::wg_commit();
+          tc::wg_wait<0>();
+          if (k0 + AW_KV > Nk) {
+#pragma unroll
+            for (int jj = 0; jj < 32; ++jj)
+              if (k0 + 8 * (jj >> 2) + c2 + (jj & 1) >= Nk) a[jj] = -INFINITY;  // 2^(-inf) = 0
+          }
+          uint32_t ph[16], pl[16];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {  // fragment row rq + 8h: a[4j + 2h + e]
+            float mx = a[2 * h];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) mx = fmaxf(mx, fmaxf(a[4 * j + 2 * h], a[4 * j + 2 * h + 1]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            const float m_new = fmaxf(m_ref[sl][h], mx * c2s);
+            if (m_new - m_ref[sl][h] > AS_RESCALE) {  // also true on the first tile (m_ref = -inf); uniform over the quad
+              const float corr = tc::ex2(m_ref[sl][h] - m_new);
+              l_i[sl][h] *= corr;
+              if (i > 0) {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) o[sl][4 * j + 2 * h] *= corr, o[sl][4 * j + 2 * h + 1] *= corr;
+              }
+              m_ref[sl][h] = m_new;
+            }
+            float rs = 0.f;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const float p0 = tc::ex2(fmaf(a[4 * j + 2 * h], c2s, -m_ref[sl][h]));
+              const float p1 = tc::ex2(fmaf(a[4 * j + 2 * h + 1], c2s, -m_ref[sl][h]));
+              rs += p0 + p1;
+              const __half2 hh = __floats2half2_rn(p0, p1);
+              // A fragment of k step j / 2: registers (row rq, k 2c), (row rq + 8, k 2c), (row rq, k 2c + 8), (row rq + 8, ...)
+              const int ri = 4 * (j >> 1) + 2 * (j & 1) + h;
+              ph[ri] = *reinterpret_cast<const uint32_t*>(&hh);
+              if (!SINGLE) {
+                const float2 hf = __half22float2(hh);
+                const __half2 ll = __floats2half2_rn(p0 - hf.x, p1 - hf.y);  // p - hi, exact
+                pl[ri] = *reinterpret_cast<const uint32_t*>(&ll);
+              }
+            }
+            l_i[sl][h] += rs;
+          }
+          tc::wg_fence();
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) {
+            const uint64_t advV = (uint64_t)(ks * 128);  // 16 key rows of 128 bytes
+            tc::wg_rs_n64_bt(o[sl], ph + 4 * ks, dVh + advV, (i | ks) ? 1u : 0u);
+            if (!SINGLE) {
+              tc::wg_rs_n64_bt(o[sl], ph + 4 * ks, dVl + advV, 1u);
+              tc::wg_rs_n64_bt(o[sl], pl + 4 * ks, dVh + advV, 1u);
+            }
+          }
+          tc::wg_commit();
+          tc::wg_wait<0>();
+        }
+        release(ge + i);                // K tile i (and V tile i - 2)
+        if (i + 2 >= T) release(gv);   // an entry without a K tile: V tile i was its only content
+      }
+      ge += T + 2;
+      w += T;
+      // ---- this segment's result: row sums over the quad ----
+#pragma unroll
+      for (int sl = 0; sl < 2; ++sl)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          l_i[sl][h] += __shfl_xor_sync(0xffffffffu, l_i[sl][h], 1);
+          l_i[sl][h] += __shfl_xor_sync(0xffffffffu, l_i[sl][h], 2);
+        }
+      auto write_row = [&](const float* v, float inv, int qrow) {  // v[4j + e] scaled by inv -> output dims 8j + c2 + e
+        uint32_t* dh = reinterpret_cast<uint32_t*>(pr.Oh + (size_t)qrow * 256 + sg.h * 64 + c2);
+        uint32_t* dl = reinterpret_cast<uint32_t*>(pr.Ol + (size_t)qrow * 256 + sg.h * 64 + c2);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          uint32_t hi, lo;
+          if (SINGLE) {  // SDPA returns half: the message is the fp16 rounding of the fp32 accumulator
+            const __half2 hh = __floats2half2_rn(tc::clamp_h(v[4 * j] * inv), tc::clamp_h(v[4 * j + 1] * inv));
+            hi = *reinterpret_cast<const uint32_t*>(&hh), lo = 0u;
+          } else {
+            tc::split2(v[4 * j] * inv, v[4 * j + 1] * inv, hi, lo);
+          }
+          dh[4 * j] = hi;
+          dl[4 * j] = lo;
+        }
+      };
+      if (sg.nsplits == 1) {
+#pragma unroll
+        for (int sl = 0; sl < 2; ++sl)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int qrow = sg.q0 + q * AW_Q + sl * 64 + rq + 8 * h;
+            if (qrow >= pr.Nq) continue;
+            float v[32];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) v[4 * j] = o[sl][4 * j + 2 * h], v[4 * j + 1] = o[sl][4 * j + 2 * h + 1];
+            write_row(v, 1.0f / l_i[sl][h], qrow);
+          }
       } else {
         // partial of a cut item; the warpgroup that completes the item (last to arrive) merges all of them
         const size_t slot0 = (size_t)sg.itemg * args.max_splits;
-        const size_t rowi = (slot0 + sg.split) * 256 + q * AW_Q + r;
-        if (qrow < pr.Nq) {
-          float4* dst = reinterpret_cast<float4*>(args.Opart + rowi * 64);
 #pragma unroll
-          for (int c = 0; c < 16; ++c) dst[c] = make_float4(o[4 * c], o[4 * c + 1], o[4 * c + 2], o[4 * c + 3]);
-          *reinterpret_cast<float2*>(args.ml + rowi * 2) = make_float2(m_ref, l_i);
-        }
+        for (int sl = 0; sl < 2; ++sl)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int rl = q * AW_Q + sl * 64 + rq + 8 * h;
+            if (sg.q0 + rl >= pr.Nq) continue;
+            const size_t rowi = (slot0 + sg.split) * 256 + rl;
+            float* dst = args.Opart + rowi * 64 + c2;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(dst + 8 * j) = make_float2(o[sl][4 * j + 2 * h], o[sl][4 * j + 2 * h + 1]);
+            if (c2 == 0) *reinterpret_cast<float2*>(args.ml + rowi * 2) = make_float2(m_ref[sl][h], l_i[sl][h]);
+          }
         __threadfence();  // partial visible device-wide before this warpgroup is counted
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + q) : "memory");
+        wg_bar();
         if (r == 0) {
           int* cnt = args.arrivals + sg.itemg * 2 + q;
           const int old = atomicAdd(cnt, 1);
@@ -391,53 +320,38 @@ static __global__ void __launch_bounds__(AS_THREADS, 1) k_flash_ps(const __grid_
           if (last) atomicExch(cnt, 0);  // nobody else touches it in this launch; zero again for the next one
           last_flag[q] = last;
         }
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + q) : "memory");
-        if (last_flag[q] && qrow < pr.Nq) {
+        wg_bar();
+        if (last_flag[q]) {
           __threadfence();
-          float m = -INFINITY;
-          for (int sp = 0; sp < sg.nsplits; ++sp) m = fmaxf(m, __ldcg(args.ml + ((slot0 + sp) * 256 + q * AW_Q + r) * 2));
-          float l = 0.f;
+#pragma unroll 1
+          for (int sl = 0; sl < 2; ++sl)
+#pragma unroll 1
+            for (int h = 0; h < 2; ++h) {
+              const int rl = q * AW_Q + sl * 64 + rq + 8 * h;
+              const int qrow = sg.q0 + rl;
+              if (qrow >= pr.Nq) continue;
+              float m = -INFINITY;
+              for (int sp = 0; sp < sg.nsplits; ++sp) m = fmaxf(m, __ldcg(args.ml + ((slot0 + sp) * 256 + rl) * 2));
+              float l = 0.f, v[32];
 #pragma unroll
-          for (int j = 0; j < 64; ++j) o[j] = 0.f;
-          for (int sp = 0; sp < sg.nsplits; ++sp) {
-            const size_t ri = (slot0 + sp) * 256 + q * AW_Q + r;
-            const float2 mlv = __ldcg(reinterpret_cast<const float2*>(args.ml + ri * 2));
-            const float wgt = tc::ex2(mlv.x - m);
-            l = fmaf(mlv.y, wgt, l);
-            const float4* src = reinterpret_cast<const float4*>(args.Opart + ri * 64);
+              for (int j = 0; j < 32; ++j) v[j] = 0.f;
+              for (int sp = 0; sp < sg.nsplits; ++sp) {
+                const size_t ri = (slot0 + sp) * 256 + rl;
+                const float2 mlv = __ldcg(reinterpret_cast<const float2*>(args.ml + ri * 2));
+                const float wgt = tc::ex2(mlv.x - m);
+                l = fmaf(mlv.y, wgt, l);
+                const float* src = args.Opart + ri * 64 + c2;
 #pragma unroll
-            for (int c = 0; c < 16; ++c) {
-              const float4 v = __ldcg(src + c);
-              o[4 * c] = fmaf(v.x, wgt, o[4 * c]), o[4 * c + 1] = fmaf(v.y, wgt, o[4 * c + 1]);
-              o[4 * c + 2] = fmaf(v.z, wgt, o[4 * c + 2]), o[4 * c + 3] = fmaf(v.w, wgt, o[4 * c + 3]);
-            }
-          }
-          const float inv = 1.0f / l;
-          uint4* dh = reinterpret_cast<uint4*>(pr.Oh + (size_t)qrow * 256 + sg.h * 64);
-          uint4* dl = reinterpret_cast<uint4*>(pr.Ol + (size_t)qrow * 256 + sg.h * 64);
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            uint32_t hi[4], lo[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              if (SINGLE) {  // SDPA returns half: the message is the fp16 rounding of the fp32 accumulator
-                const __half2 hh = __floats2half2_rn(tc::clamp_h(o[8 * c + 2 * i] * inv), tc::clamp_h(o[8 * c + 2 * i + 1] * inv));
-                hi[i] = *reinterpret_cast<const uint32_t*>(&hh), lo[i] = 0u;
-              } else {
-                tc::split2(o[8 * c + 2 * i] * inv, o[8 * c + 2 * i + 1] * inv, hi[i], lo[i]);
+                for (int j = 0; j < 8; ++j) {
+                  const float2 x = __ldcg(reinterpret_cast<const float2*>(src + 8 * j));
+                  v[4 * j] = fmaf(x.x, wgt, v[4 * j]), v[4 * j + 1] = fmaf(x.y, wgt, v[4 * j + 1]);
+                }
               }
+              write_row(v, 1.0f / l, qrow);
             }
-            dh[c] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            dl[c] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-          }
         }
       }
     }
   }
-  __syncwarp();
   if (!ok && args.err_flag) *args.err_flag = 1;
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 9) tc::tmem_dealloc(tmem, 512);
 }
-

@@ -1,4 +1,4 @@
-// Shared context / helpers for libgtsfm_b200.so.  sm_100a only.
+// Shared context / helpers for libgtsfm_b200.so.  sm_90a only.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -101,7 +101,7 @@ constexpr int B2_FEAT_CACHE_SLOTS = 96;
 
 struct b2_context {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   int reserve_sms = 0;  // SMs the persistent kernels of this context leave free (b2_set_option "reserve_sms")
   int lg_batch = 0;     // pairs per LightGlue batch (0 = the library maximum, 8); b2_set_option "lightglue_batch"
   int sp_graph = -1;    // SuperPoint network as a CUDA graph: 1 / 0, -1 = B2_SP_GRAPH env (default off)

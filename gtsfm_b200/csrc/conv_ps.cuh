@@ -1,6 +1,5 @@
-// 3x3 convolution (pad 1) + bias + ReLU (+ fused 2x2/2 max-pool): persistent, warp-specialised tcgen05 implicit GEMM with
-// HALO REUSE, split-fp16 (~fp32).  Replaces the one-tile-per-CTA kernel of round 1 (conv_tma.cuh), which re-loaded the
-// activation tile once per tap (9x the L2 -> shared-memory traffic) through a 2-stage ring and was latency-bound.
+// 3x3 convolution (pad 1) + bias + ReLU (+ fused 2x2/2 max-pool): persistent, warp-specialised wgmma implicit GEMM with
+// HALO REUSE, split-fp16 (~fp32).
 //
 // The SuperPoint encoder / head convolutions (thirdparty/SuperGluePretrainedNetwork/models/superpoint.py:119-134,148-162)
 // are GEMMs with M = pixels, N = output channels, K = 9 taps x Cin.  Activations live in HBM as NHWC fp16 hi / lo planes
@@ -9,20 +8,16 @@
 //   * Output tile = 16 rows x 8 columns of pixels (M = 128, m = h * 8 + w) by 64 output channels.  ONE 3-D TMA box
 //     {64 ch, 10 px, 18 rows} per plane and 64-channel chunk brings the tile with its halo; out-of-image coordinates are
 //     zero-filled by the TMA unit = the convolution's zero padding.  Pixels are 128-byte rows (128-byte swizzle).
-//   * The 9 taps are 9 UMMA descriptors into the SAME buffer: start address + ((dy + 1) * 10 + (dx + 1)) * 128 bytes, 8-row
+//   * The 9 taps are 9 wgmma descriptors into the SAME buffer: start address + ((dy + 1) * 10 + (dx + 1)) * 128 bytes, 8-row
 //     group stride 10 * 128 bytes (a group = 8 consecutive pixels of one tile row).  The start is not 1024-byte aligned and
 //     the stride not a multiple of 1024: that works because the tensor core applies the 128-byte swizzle to ABSOLUTE
-//     shared-memory address bits, exactly like the TMA unit that wrote the tile (measured: scratch/halo_test.cu - exact for
-//     every tap with descriptor base_offset = 0, wrong with the "(start >> 7) & 7" some documents suggest).
+//     shared-memory address bits, exactly like the TMA unit that wrote the tile (descriptor base_offset = 0).
 //   * Weights of the CTA's 64 output channels and the current 64-channel chunk stay resident in shared memory (9 taps x
-//     [Bh (64 rows); Bl (64 rows)] x 64 K = 144 KB): loaded once per CTA when Cin = 64, once per (group of 4 tiles, chunk)
-//     when Cin = 128.  Stacking Bh over Bl makes  Ah x [Bh; Bl]^T  ONE N = 128 MMA (columns 0-63: Ah Bh, 64-127: Ah Bl);
-//     Al x Bh^T (N = 64) adds into columns 64-127.  Shared-memory operand traffic per tap and k-step: 8 KB / 64 clk + 6 KB /
-//     32 clk (round 1: 18 KB / 96 clk).
-//   * Warp 0 = TMA producer (3 plane buffers), warp 1 = MMA issuer (warp-uniform issue), warps 2-5 = epilogue (thread =
-//     pixel = TMEM lane): 4 TMEM accumulators of 128 columns, so a tile's epilogue overlaps the next tiles' MMAs.
-//   * Epilogue: acc0 + acc1 * 2^-11, 2x2 max-pool by two warp shuffles (partners lane ^ 1 and lane ^ 8), bias, ReLU,
-//     fp16 planes for the next convolution and / or fp32 for the SIMT head kernels.
+//     [Bh (64 rows); Bl (64 rows)] x 64 K = 144 KB): loaded once per CTA when Cin = 64, once per (tile, chunk) when
+//     Cin = 128 (the register accumulators hold one tile).  Stacking Bh over Bl makes  Ah x [Bh; Bl]^T  ONE N = 128 MMA
+//     (columns 0-63: Ah Bh, 64-127: Ah Bl); Al x Bh^T (N = 64) goes to a third accumulator.
+//   * Warp 8 = TMA producer (3 plane buffers); warpgroup w (warps 4w .. 4w + 3) owns pixels 64w .. 64w + 63: MMAs, then
+//     hh + (hl + lh) * 2^-11, 2x2 max-pool (partners: row + 8 in the fragment, lane ^ 4), bias, ReLU, planes and / or fp32.
 #pragma once
 #include "common.cuh"
 #include "tma.cuh"
@@ -34,8 +29,7 @@ constexpr int CP_A_BYTES = 23 * 1024;                // buffer pitch (1024-align
 constexpr int CP_NA = 3;                             // activation plane buffers
 constexpr int CP_B_TAP = 128 * 128;                  // [Bh; Bl] x 64 K halves
 constexpr int CP_B_BYTES = 9 * CP_B_TAP;
-constexpr int CP_NACC = 4, CP_ACC_COLS = 128;
-constexpr int CP_THREADS = 192;
+constexpr int CP_THREADS = 256 + 32;
 constexpr size_t CP_SMEM = (size_t)CP_B_BYTES + CP_NA * CP_A_BYTES + 1024 + 512;
 
 struct ConvPsMaps {
@@ -60,16 +54,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst_smem, const CUtensorMap
       ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// K-major, 128-byte swizzle, arbitrary 8-row group stride (multiple of 16 bytes), base_offset 0 (see the header comment)
-__device__ __forceinline__ uint64_t smem_desc_sw128_sbo(uint32_t saddr, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
 }  // namespace tc
 
 __device__ __forceinline__ void cp_stamp(float* dbg, int slot) {
@@ -87,12 +71,9 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
   const uint32_t sB = smem0, sA = smem0 + CP_B_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + CP_B_BYTES + CP_NA * CP_A_BYTES);
   uint64_t* fullA = bars;               // [CP_NA]
-  uint64_t* emptyA = fullA + CP_NA;     // [CP_NA]
+  uint64_t* emptyA = fullA + CP_NA;     // [CP_NA] one arrival per consumer warp
   uint64_t* fullB = emptyA + CP_NA;     // [9]
-  uint64_t* emptyB = fullB + 9;         // [9]
-  uint64_t* accFull = emptyB + 9;       // [CP_NACC]
-  uint64_t* accEmpty = accFull + CP_NACC;  // [CP_NACC]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accEmpty + CP_NACC);
+  uint64_t* emptyB = fullB + 9;         // [9] one arrival per consumer warp
 
   const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
   const int nblk = g.Cout / 64, nchunk = g.Cin / 64;
@@ -102,30 +83,26 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
 
   if (t == 0) {
     cp_stamp(g.dbg, 0);
-    for (int i = 0; i < CP_NA; ++i) tc::mbar_init(&fullA[i], 1), tc::mbar_init(&emptyA[i], 1);
-    for (int i = 0; i < 9; ++i) tc::mbar_init(&fullB[i], 1), tc::mbar_init(&emptyB[i], 1);
-    for (int i = 0; i < CP_NACC; ++i) tc::mbar_init(&accFull[i], 1), tc::mbar_init(&accEmpty[i], 4);
+    for (int i = 0; i < CP_NA; ++i) tc::mbar_init(&fullA[i], 1), tc::mbar_init(&emptyA[i], 8);
+    for (int i = 0; i < 9; ++i) tc::mbar_init(&fullB[i], 1), tc::mbar_init(&emptyB[i], 8);
     tc::fence_mbar_init();
     tc::tma_prefetch_desc(&maps.ah);
     tc::tma_prefetch_desc(&maps.al);
     tc::tma_prefetch_desc(&maps.wh);
     tc::tma_prefetch_desc(&maps.wl);
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, CP_NACC * CP_ACC_COLS);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
   bool ok = true;
   if (t == 0) cp_stamp(g.dbg, 1), g.dbg ? (void)(g.dbg[blockIdx.x * 8 + 7] = (float)nt) : (void)0;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       uint32_t a_cnt = 0, bver = 0;
-      for (int g0 = 0; g0 < nt; g0 += CP_NACC) {
-        const int gsz = nt - g0 < CP_NACC ? nt - g0 : CP_NACC;
+      for (int k = 0; k < nt; ++k) {
+        const int tile = lane_id + k * stride;
+        const int x0 = (tile % tiles_x) * CP_TW, y0 = (tile / tiles_x) * CP_TH;
         for (int c = 0; c < nchunk; ++c) {
-          if (nchunk > 1 || bver == 0) {  // (re)load the weights of (nb, c): tap slot by tap slot, as the MMA warp frees them
+          if (nchunk > 1 || bver == 0) {  // (re)load the weights of (nb, c): tap slot by tap slot, as the consumers free them
             for (int tap = 0; tap < 9; ++tap) {
               if (bver > 0) ok = tc::mbar_wait(&emptyB[tap], (bver - 1) & 1) && ok;
               tc::mbar_expect_tx(&fullB[tap], CP_B_TAP);
@@ -134,153 +111,133 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
             }
             ++bver;
           }
-          for (int i = 0; i < gsz; ++i) {
-            const int tile = lane_id + (g0 + i) * stride;
-            const int x0 = (tile % tiles_x) * CP_TW, y0 = (tile / tiles_x) * CP_TH;
-            for (int plane = 0; plane < 2; ++plane, ++a_cnt) {
-              const uint32_t buf = a_cnt % CP_NA, use = a_cnt / CP_NA;
-              if (use > 0) ok = tc::mbar_wait(&emptyA[buf], (use - 1) & 1) && ok;
-              tc::mbar_expect_tx(&fullA[buf], CP_A_LOAD);
-              tc::tma_load_3d(sA + buf * CP_A_BYTES, plane ? &maps.al : &maps.ah, &fullA[buf], c * 64, x0 - 1, y0 - 1);
-            }
+          for (int plane = 0; plane < 2; ++plane, ++a_cnt) {
+            const uint32_t buf = a_cnt % CP_NA, use = a_cnt / CP_NA;
+            if (use > 0) ok = tc::mbar_wait(&emptyA[buf], (use - 1) & 1) && ok;
+            tc::mbar_expect_tx(&fullA[buf], CP_A_LOAD);
+            tc::tma_load_3d(sA + buf * CP_A_BYTES, plane ? &maps.al : &maps.ah, &fullA[buf], c * 64, x0 - 1, y0 - 1);
           }
         }
       }
     }
-  } else if (warp == 1) {  // whole warp, one elected lane issues (tc.cuh: warp-uniform issue)
-    const uint32_t id128 = tc::idesc_f16(128, 128), id64 = tc::idesc_f16(128, 64);
+  } else {
+    // ---- consumer warpgroup wg: tile rows h = 8 wg .. 8 wg + 7; thread rows (h0, wc) and (h0 + 1, wc) ------------------
+    const int wg = warp >> 2;
+    const int h0 = wg * 8 + (warp & 3) * 2, wc = lane >> 2, c2 = (lane & 3) * 2;
+    const int OH = g.pool ? g.H >> 1 : g.H, OW = g.pool ? g.W >> 1 : g.W;
     uint32_t a_cnt = 0, bver = 0;
-    for (int g0 = 0; g0 < nt; g0 += CP_NACC) {
-      const int gsz = nt - g0 < CP_NACC ? nt - g0 : CP_NACC;
-      const uint32_t u = (uint32_t)(g0 / CP_NACC);
+    for (int k = 0; k < nt; ++k) {
+      const int tile = lane_id + k * stride;
+      const int x0 = (tile % tiles_x) * CP_TW, y0 = (tile / tiles_x) * CP_TH;
+      float acc[64], accl[32];  // acc columns 0-63: Ah Bh, 64-127: Ah Bl; accl: Al Bh
       for (int c = 0; c < nchunk; ++c) {
         const bool new_b = nchunk > 1 || bver == 0;
         if (new_b) ++bver;
-        for (int i = 0; i < gsz; ++i) {
-          const uint32_t acc = tmem + i * CP_ACC_COLS;
-          if (c == 0 && u > 0) {
-            ok = tc::mbar_wait(&accEmpty[i], (u - 1) & 1) && ok;
-            tc::fence_after_sync();
-          }
-          {  // hi plane: Ah x [Bh; Bl]^T
-            const uint32_t buf = a_cnt % CP_NA;
-            ok = tc::mbar_wait(&fullA[buf], (a_cnt / CP_NA) & 1) && ok;
-            tc::fence_after_sync();
-            const uint32_t base = sA + buf * CP_A_BYTES;
-            if (a_cnt == 0 && lane == 0) cp_stamp(g.dbg, 2);
+        {  // hi plane: Ah x [Bh; Bl]^T
+          const uint32_t buf = a_cnt % CP_NA;
+          ok = tc::mbar_wait(&fullA[buf], (a_cnt / CP_NA) & 1) && ok;
+          const uint32_t base = sA + buf * CP_A_BYTES;
+          if (a_cnt == 0 && t == 0) cp_stamp(g.dbg, 2);
 #pragma unroll 1
-            for (int tap = 0; tap < 9; ++tap) {
-              if (new_b && i == 0) {
-                ok = tc::mbar_wait(&fullB[tap], (bver - 1) & 1) && ok;
-                tc::fence_after_sync();
-              }
-              const uint64_t dA = tc::smem_desc_sw128_sbo(base + ((tap / 3) * CP_HW + tap % 3) * 128, CP_HW * 128);
-              const uint64_t dB = tc::smem_desc_sw128(sB + tap * CP_B_TAP);
+          for (int tap = 0; tap < 9; ++tap) {
+            if (new_b) ok = tc::mbar_wait(&fullB[tap], (bver - 1) & 1) && ok;
+            const uint64_t dA = tc::wg_desc_sw128(base + ((tap / 3 + wg * 8) * CP_HW + tap % 3) * 128, CP_HW * 128);
+            const uint64_t dB = tc::wg_desc_sw128(sB + tap * CP_B_TAP);
+            tc::wg_fence();
 #pragma unroll
-              for (int ks = 0; ks < 4; ++ks)
-                tc::umma_f16_w(acc, dA + (uint64_t)(ks * 2), dB + (uint64_t)(ks * 2), id128, (c == 0 && tap == 0 && ks == 0) ? 0u : 1u);
-            }
-            tc::umma_commit_w(&emptyA[buf]);
-            ++a_cnt;
+            for (int ks = 0; ks < 4; ++ks)
+              tc::wg_ss_n128(acc, dA + (uint64_t)(ks * 2), dB + (uint64_t)(ks * 2), (c == 0 && tap == 0 && ks == 0) ? 0u : 1u);
+            tc::wg_commit();
           }
-          {  // lo plane: Al x Bh^T into columns 64..127
-            const uint32_t buf = a_cnt % CP_NA;
-            ok = tc::mbar_wait(&fullA[buf], (a_cnt / CP_NA) & 1) && ok;
-            tc::fence_after_sync();
-            const uint32_t base = sA + buf * CP_A_BYTES;
+          tc::wg_wait<0>();
+          if (lane == 0) tc::mbar_arrive(&emptyA[buf]);
+          ++a_cnt;
+        }
+        {  // lo plane: Al x Bh^T into accl
+          const uint32_t buf = a_cnt % CP_NA;
+          ok = tc::mbar_wait(&fullA[buf], (a_cnt / CP_NA) & 1) && ok;
+          const uint32_t base = sA + buf * CP_A_BYTES;
 #pragma unroll 1
-            for (int tap = 0; tap < 9; ++tap) {
-              const uint64_t dA = tc::smem_desc_sw128_sbo(base + ((tap / 3) * CP_HW + tap % 3) * 128, CP_HW * 128);
-              const uint64_t dB = tc::smem_desc_sw128(sB + tap * CP_B_TAP);
+          for (int tap = 0; tap < 9; ++tap) {
+            const uint64_t dA = tc::wg_desc_sw128(base + ((tap / 3 + wg * 8) * CP_HW + tap % 3) * 128, CP_HW * 128);
+            const uint64_t dB = tc::wg_desc_sw128(sB + tap * CP_B_TAP);
+            tc::wg_fence();
 #pragma unroll
-              for (int ks = 0; ks < 4; ++ks) tc::umma_f16_w(acc + 64, dA + (uint64_t)(ks * 2), dB + (uint64_t)(ks * 2), id64, 1u);
-              if (nchunk > 1 && i == gsz - 1) tc::umma_commit_w(&emptyB[tap]);  // last use of this tap's weights in the phase
+            for (int ks = 0; ks < 4; ++ks) tc::wg_ss_n64(accl, dA + (uint64_t)(ks * 2), dB + (uint64_t)(ks * 2), (c == 0 && tap == 0 && ks == 0) ? 0u : 1u);
+            tc::wg_commit();
+            if (nchunk > 1 && tap > 0) {  // the previous tap's weights are no longer read: hand the slot back
+              tc::wg_wait<1>();
+              if (lane == 0) tc::mbar_arrive(&emptyB[tap - 1]);
             }
-            tc::umma_commit_w(&emptyA[buf]);
-            ++a_cnt;
           }
-          if (c == nchunk - 1) tc::umma_commit_w(&accFull[i]);
+          tc::wg_wait<0>();
+          if (lane == 0) {
+            if (nchunk > 1) tc::mbar_arrive(&emptyB[8]);
+            tc::mbar_arrive(&emptyA[buf]);
+          }
+          ++a_cnt;
         }
       }
-    }
-    if (lane == 0) cp_stamp(g.dbg, 3);
-  } else {
-    // ---- epilogue warps: thread = tile pixel m = TMEM lane; (h, w) = (m / 8, m % 8) ---------------------------------
-    const int q = warp & 3, m = q * 32 + lane, h = m >> 3, w = m & 7;
-    const int OH = g.pool ? g.H >> 1 : g.H, OW = g.pool ? g.W >> 1 : g.W;
-    for (int k = 0; k < nt; ++k) {
-      const int slot = k % CP_NACC;
-      const uint32_t u = (uint32_t)(k / CP_NACC);
-      const int tile = lane_id + k * stride;
-      const int x0 = (tile % tiles_x) * CP_TW, y0 = (tile / tiles_x) * CP_TH;
-      int oy, ox;
-      bool writer;
-      if (g.pool) {
-        oy = (y0 + h) >> 1, ox = (x0 + w) >> 1;
-        writer = ((h & 1) == 0) && ((w & 1) == 0) && oy < OH && ox < OW;
-      } else {
-        oy = y0 + h, ox = x0 + w;
-        writer = oy < OH && ox < OW;
-      }
-      const size_t opix = ((size_t)oy * OW + ox) * g.Cout + nb * 64;
-      ok = tc::mbar_wait(&accFull[slot], u & 1) && ok;
-      tc::fence_after_sync();
-      if (t == 64 && (k == 0 || k == nt - 1)) cp_stamp(g.dbg, k == 0 ? 4 : 5);
-      const uint32_t lane_base = tmem + ((uint32_t)(q * 32) << 16) + slot * CP_ACC_COLS;
-#pragma unroll 1
-      for (int cc = 0; cc < 2; ++cc) {
-        float a0[32], a1[32];
-        tc::tmem_ld32(lane_base + cc * 32, a0);
-        tc::tmem_ld32(lane_base + 64 + cc * 32, a1);
-        float v[32];
+      if (k == 0 && t == 0) cp_stamp(g.dbg, 3);
+      // ---- epilogue: v[4j + 2i + e] = pixel (h0 + i, wc), channel 8j + c2 + e ----
+      float v[32];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = fmaf(a1[j], tc::LO_INV, a0[j]);
-        if (g.pool) {  // max over the 2x2 window: partners are lane ^ 1 (w) and lane ^ 8 (h); max commutes with bias (+ ReLU)
+      for (int i = 0; i < 32; ++i) v[i] = fmaf(acc[32 + i] + accl[i], tc::LO_INV, acc[i]);
+      const float* bp = g.bias + nb * 64 + c2;
+      if (g.pool) {  // max over the 2x2 window; max commutes with bias (+ ReLU)
+        const int oy = (y0 + h0) >> 1, ox = (x0 + wc) >> 1;
+        const bool writer = (wc & 1) == 0 && oy < OH && ox < OW;
+        float p[16];
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            v[j] = fmaxf(v[j], __shfl_xor_sync(0xffffffffu, v[j], 1));
-            v[j] = fmaxf(v[j], __shfl_xor_sync(0xffffffffu, v[j], 8));
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float m = fmaxf(v[4 * j + e], v[4 * j + 2 + e]);
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+            p[2 * j + e] = m;
           }
-        }
         if (writer) {
-          const float4* bp = reinterpret_cast<const float4*>(g.bias + nb * 64 + cc * 32);
+          const size_t opix = ((size_t)oy * OW + ox) * g.Cout + nb * 64 + c2;
 #pragma unroll
-          for (int j4 = 0; j4 < 8; ++j4) {
-            const float4 b = __ldg(bp + j4);
-            v[4 * j4] += b.x, v[4 * j4 + 1] += b.y, v[4 * j4 + 2] += b.z, v[4 * j4 + 3] += b.w;
+          for (int j = 0; j < 8; ++j) {
+            const float2 b = make_float2(__ldg(bp + 8 * j), __ldg(bp + 8 * j + 1));
+            float a0 = p[2 * j] + b.x, a1 = p[2 * j + 1] + b.y;
+            if (g.relu) a0 = fmaxf(a0, 0.f), a1 = fmaxf(a1, 0.f);
+            if (g.Of) *reinterpret_cast<float2*>(g.Of + opix + 8 * j) = make_float2(a0, a1);
+            if (g.Oh) {
+              uint32_t hi, lo;
+              tc::split2(a0, a1, hi, lo);
+              *reinterpret_cast<uint32_t*>(g.Oh + opix + 8 * j) = hi;
+              *reinterpret_cast<uint32_t*>(g.Ol + opix + 8 * j) = lo;
+            }
           }
-          if (g.relu) {
+        }
+      } else {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-          }
-          if (g.Of) {
-            float4* d = reinterpret_cast<float4*>(g.Of + opix + cc * 32);
+        for (int i = 0; i < 2; ++i) {
+          const int oy = y0 + h0 + i, ox = x0 + wc;
+          if (oy >= OH || ox >= OW) continue;
+          const size_t opix = ((size_t)oy * OW + ox) * g.Cout + nb * 64 + c2;
 #pragma unroll
-            for (int j4 = 0; j4 < 8; ++j4) d[j4] = make_float4(v[4 * j4], v[4 * j4 + 1], v[4 * j4 + 2], v[4 * j4 + 3]);
-          }
-          if (g.Oh) {
-            uint4* dh = reinterpret_cast<uint4*>(g.Oh + opix + cc * 32);
-            uint4* dl = reinterpret_cast<uint4*>(g.Ol + opix + cc * 32);
-#pragma unroll
-            for (int c4 = 0; c4 < 4; ++c4) {
-              uint32_t hi[4], lo[4];
-#pragma unroll
-              for (int i = 0; i < 4; ++i) tc::split2(v[8 * c4 + 2 * i], v[8 * c4 + 2 * i + 1], hi[i], lo[i]);
-              dh[c4] = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-              dl[c4] = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+          for (int j = 0; j < 8; ++j) {
+            const float2 b = make_float2(__ldg(bp + 8 * j), __ldg(bp + 8 * j + 1));
+            float a0 = v[4 * j + 2 * i] + b.x, a1 = v[4 * j + 2 * i + 1] + b.y;
+            if (g.relu) a0 = fmaxf(a0, 0.f), a1 = fmaxf(a1, 0.f);
+            if (g.Of) *reinterpret_cast<float2*>(g.Of + opix + 8 * j) = make_float2(a0, a1);
+            if (g.Oh) {
+              uint32_t hi, lo;
+              tc::split2(a0, a1, hi, lo);
+              *reinterpret_cast<uint32_t*>(g.Oh + opix + 8 * j) = hi;
+              *reinterpret_cast<uint32_t*>(g.Ol + opix + 8 * j) = lo;
             }
           }
         }
       }
-      tc::fence_before_sync();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&accEmpty[slot]);
+      if (k == nt - 1 && t == 0) cp_stamp(g.dbg, 5);
     }
   }
   if (!ok && g.err_flag) *g.err_flag = 1;
-  tc::fence_before_sync();
   __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem, CP_NACC * CP_ACC_COLS);
   if (t == 0) cp_stamp(g.dbg, 6);
 }
 

@@ -1,4 +1,4 @@
-// Test-only entry points: run one GEMM through the SIMT fp32 kernel or the tcgen05 split-fp16 kernel (parity tests).
+// Test-only entry points: run one GEMM through the SIMT fp32 kernel or the wgmma split-fp16 kernel (parity tests).
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -24,7 +24,7 @@ extern "C" int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, con
   if (mode == 0) {
     rc = launch_gemm(ctx, st, gemm_linear(dA.as<float>(), K, K, dB.as<float>(), bias ? dBias.as<float>() : nullptr, dC.as<float>(), N, M, N));
   } else {
-    // modes 1 and 2 both run the tcgen05 kernel on operands split here (A and B as fp16 hi / lo planes)
+    // modes 1 and 2 both run the wgmma kernel on operands split here (A and B as fp16 hi / lo planes)
     DevBuf dAh, dAl;
     B2_CUDA(ctx, dAh.ensure((size_t)M * K * 2));
     B2_CUDA(ctx, dAl.ensure((size_t)M * K * 2));
@@ -53,6 +53,6 @@ extern "C" int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, con
     if (e != cudaSuccess) rc = b2_fail(ctx, B2_ERR_CUDA, std::string("debug gemm: ") + cudaGetErrorString(e));
   }
   dA.release(), dB.release(), dC.release(), dBias.release(), dBh.release(), dBl.release(), dErr.release();
-  if (rc == B2_OK && err) rc = b2_fail(ctx, B2_ERR_STATE, "tcgen05 pipeline timed out on an mbarrier (kernel bug)");
+  if (rc == B2_OK && err) rc = b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
   return rc;
 }

@@ -1,5 +1,5 @@
 // fp32 SIMT "NT" GEMM used by the matcher blocks: C[M,N] = [A1 | A2][M,K1+K2] * B[N,K]^T (+bias) (*scale) (+resid).
-// Exact-fp32 path (the parity reference on the device); the tcgen05 split-precision GEMM replaces it on the hot layers.
+// Exact-fp32 path (the parity reference on the device); the wgmma split-precision GEMM replaces it on the hot layers.
 #pragma once
 #include "common.cuh"
 

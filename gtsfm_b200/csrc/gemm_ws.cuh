@@ -1,24 +1,16 @@
-// Persistent, warp-specialised tcgen05 + TMA split-fp16 "NT" GEMM over a BATCH of problems that share one weight matrix:
+// Persistent, warp-specialised wgmma + TMA split-fp16 "NT" GEMM over a BATCH of problems that share one weight matrix:
 //     C_z[M_z, N] = [A1_z | A2_z][M_z, K] * B[N, K]^T        z = 0 .. nprob-1  (images of a batch of pairs)
 // or, with `b_per_problem`, one (A_z, B_z, N_z) triple per problem (the assignment similarity of every pair of a batch).
 //
 // Arithmetic: every fp32 value travels as two fp16 planes, x ~= hi + lo * 2^-11 (the producing kernel's epilogue writes
 // them); three MMAs per K step,  acc0 += Ah Bh ; acc1 += Ah Bl + Al Bh ; result = acc0 + acc1 * 2^-11, both fp32
-// accumulators in TMEM.  The dropped Al * Bl term is 2^-22 relative.
+// accumulators in registers.  The dropped Al * Bl term is 2^-22 relative.
 //
 // Schedule: one CTA per SM walks output tiles `blockIdx.x + i * gridDim.x` of the whole batch (problem-major, then row
 // tile, then column tile - concurrently running CTAs share the A row tile through L2):
-//   warp 0 (lane 0)  TMA producer: K chunks of consecutive tiles flow through one 2-stage ring (2 x 64 KB) without draining
-//   warp 1           TMEM allocator (512 columns = two accumulator sets of 2 x 128) + MMA issuer (warp-uniform issue, tc.cuh)
-//   warps 2-17       epilogue, ONE 32 x 32 block of the tile each (TMEM lane quarter w % 4 = rows, column block (w - 2) / 4):
-//                    operands that do not depend on the accumulator (bias) are fetched first, then wait acc_full[set] ->
-//                    tcgen05.ld -> release the set (acc_empty) -> 128-bit stores into a padded transpose pad -> read back as
-//                    (row, 4 consecutive columns) per lane -> bias / scale / ReLU / residual -> 16-byte fp32 and 8-byte
-//                    plane stores (8 lanes cover 128 contiguous bytes of a row).  Tile t's epilogue overlaps tile t + 1's MMAs.
-// Tile = 128 x 128: per 64-wide K chunk the tensor pipe needs 768 cycles for the three products.  With K = 256 / 512 a
-// tile is only 3072 / 6144 tensor cycles for 16 384 outputs, so the EPILOGUE, not the operand traffic, paces the linears
-// (ncu, profiles/r02_gemm_ws.txt: round-2's first version with 8 epilogue warps and scalar stores spent 12.4 k cycles per
-// tile, tensor pipe 27 %); hence one block per warp, vector accesses and no exposed dependent global load.
+//   warp 8 (lane 0)  TMA producer: a 3-stage ring (3 x 64 KB) that keeps loading the next tile during the epilogue
+//   warps 0-7        warpgroup w: rows 64w .. 64w + 63 of the 128 x 128 tile, wgmma m64n128k16 into two register
+//                    accumulators, then bias / scale / ReLU / residual / split-plane stores from the fragment.
 #pragma once
 #include "tma.cuh"
 
@@ -27,19 +19,16 @@ constexpr int GW_M = 128, GW_N = 128, GW_K = 64;
 constexpr int GW_A_BYTES = GW_M * GW_K * 2;  // 16 KB per plane
 constexpr int GW_B_BYTES = GW_N * GW_K * 2;  // 16 KB per plane
 constexpr int GW_STAGE_BYTES = 2 * GW_A_BYTES + 2 * GW_B_BYTES;  // 64 KB
-constexpr int GW_STAGES = 2;
-constexpr int GW_EPI_WARPS = 16;
-constexpr int GW_THREADS = 64 + 32 * GW_EPI_WARPS;  // producer warp + MMA warp + 16 epilogue warps
-constexpr int GW_PAD = 36;  // fp32 row pitch of the transpose pad: 16-byte aligned rows, conflict-free for 128-bit accesses
-constexpr int GW_SCRATCH = GW_EPI_WARPS * 32 * GW_PAD * 4;  // one 32 x 36 fp32 transpose pad per epilogue warp
-constexpr size_t GW_SMEM = GW_STAGES * GW_STAGE_BYTES + GW_SCRATCH + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int GW_STAGES = 3;
+constexpr int GW_THREADS = 256 + 32;  // two consumer warpgroups + the TMA producer warp
+constexpr size_t GW_SMEM = GW_STAGES * GW_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 
 struct GemmProblem {
   const float* resid;  // [M][ldr] fp32 or null, added after bias / scale
   float* C;            // optional fp32 output, row-major [M][ldc]
   __half *Ch, *Cl;     // optional split output planes
   int M, N, ldc;
-  int vec4;      // outputs / residual may be accessed 16 bytes at a time (leading dimensions and bases 16-byte aligned)
+  int vec4;      // outputs / residual may be accessed in pairs (8-byte fp32, 4-byte plane accesses; host checks 16-byte alignment)
   int tiles_n;   // ceil(N / 128)
   int tile_end;  // running total of tiles up to and including this problem
 };
@@ -68,28 +57,19 @@ static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_c
   const uint32_t raw = tc::smem_u32(gw_raw);
   const uint32_t smem0 = (raw + 1023u) & ~1023u;
   unsigned char* sm = gw_raw + (smem0 - raw);
-  float* scratch_all = reinterpret_cast<float*>(sm + GW_STAGES * GW_STAGE_BYTES);
-  uint64_t* full = reinterpret_cast<uint64_t*>(sm + GW_STAGES * GW_STAGE_BYTES + GW_SCRATCH);
-  uint64_t* empty = full + GW_STAGES;
-  uint64_t* acc_full = empty + GW_STAGES;  // [2] all MMAs of the tile in accumulator set b have completed
-  uint64_t* acc_empty = acc_full + 2;      // [2] the 8 epilogue warps have read set b out of TMEM
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
+  uint64_t* full = reinterpret_cast<uint64_t*>(sm + GW_STAGES * GW_STAGE_BYTES);
+  uint64_t* empty = full + GW_STAGES;  // one arrival per consumer warp
 
   const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
   const int nk = (g.K1 + g.K2) / GW_K;
 
   if (t == 0) {
-    for (int s = 0; s < GW_STAGES; ++s) tc::mbar_init(&full[s], 1), tc::mbar_init(&empty[s], 1);
-    for (int b = 0; b < 2; ++b) tc::mbar_init(&acc_full[b], 1), tc::mbar_init(&acc_empty[b], GW_EPI_WARPS);
+    for (int s = 0; s < GW_STAGES; ++s) tc::mbar_init(&full[s], 1), tc::mbar_init(&empty[s], 8);
     tc::fence_mbar_init();
     tc::tma_prefetch_desc(&maps.bh[0]);
     tc::tma_prefetch_desc(&maps.bl[0]);
   }
-  if (warp == 1) tc::tmem_alloc(tmem_slot, 512);
-  tc::fence_before_sync();
   __syncthreads();
-  tc::fence_after_sync();
-  const uint32_t tmem = *tmem_slot;
   bool ok = true;
 
   auto decode = [&](int tile, int& z, int& m0, int& n0) {
@@ -101,7 +81,7 @@ static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_c
     m0 = mt * GW_M;
   };
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       // ===== TMA producer =====
       int gk = 0;
@@ -126,147 +106,111 @@ static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (whole warp, one elected lane issues) =====
-    const uint32_t idesc = tc::idesc_f16(GW_M, GW_N);
-    int gk = 0, it = 0;
-    bool hint = false;  // next stage already seen full by a pre-poll
-    for (int tile = blockIdx.x; tile < g.tiles; tile += gridDim.x, ++it) {
-      const int b = it & 1;
-      if (it >= 2) ok = tc::mbar_wait(&acc_empty[b], ((it >> 1) - 1) & 1) && ok;
-      const uint32_t acc = tmem + b * (2 * GW_N);
+  } else {
+    // ===== consumer warpgroup wg: rows 64 wg .. 64 wg + 63 of every tile =====
+    const int wg = warp >> 2;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // fragment rows r0, r0 + 8
+    const int c2 = (lane & 3) * 2;                           // fragment columns 8j + c2, + 1
+    const float scale = g.scale;
+    const int relu = g.relu;
+    int gk = 0;
+    for (int tile = blockIdx.x; tile < g.tiles; tile += gridDim.x) {
+      int z, m0, n0;
+      decode(tile, z, m0, n0);
+      float acc0[64], acc1[64];
       for (int kc = 0; kc < nk; ++kc, ++gk) {
         const int s = gk % GW_STAGES;
-        if (!hint) ok = tc::mbar_wait(&full[s], (gk / GW_STAGES) & 1) && ok;
-        __syncwarp();
-        tc::fence_after_sync();
-        hint = tc::mbar_test(&full[(gk + 1) % GW_STAGES], ((gk + 1) / GW_STAGES) & 1);
-        const uint32_t aH = smem0 + s * GW_STAGE_BYTES, aL = aH + GW_A_BYTES, bH = aH + 2 * GW_A_BYTES, bL = bH + GW_B_BYTES;
-        const uint64_t dAh = tc::smem_desc_sw128(aH), dAl = tc::smem_desc_sw128(aL), dBh = tc::smem_desc_sw128(bH), dBl = tc::smem_desc_sw128(bL);
+        ok = tc::mbar_wait(&full[s], (gk / GW_STAGES) & 1) && ok;
+        const uint32_t aH = smem0 + s * GW_STAGE_BYTES + wg * (64 * 128), aL = aH + GW_A_BYTES;
+        const uint32_t bH = smem0 + s * GW_STAGE_BYTES + 2 * GW_A_BYTES, bL = bH + GW_B_BYTES;
+        const uint64_t dAh = tc::wg_desc_sw128(aH), dAl = tc::wg_desc_sw128(aL), dBh = tc::wg_desc_sw128(bH), dBl = tc::wg_desc_sw128(bL);
+        tc::wg_fence();
 #pragma unroll
         for (int ks = 0; ks < GW_K / 16; ++ks) {
           const uint64_t adv = (uint64_t)(ks * 2);  // 32 bytes per K step, in 16-byte units of the start-address field
           const uint32_t first = (kc == 0 && ks == 0) ? 0u : 1u;
-          tc::umma_f16_w(acc, dAh + adv, dBh + adv, idesc, first);         // acc0 (+)= Ah Bh
-          tc::umma_f16_w(acc + GW_N, dAh + adv, dBl + adv, idesc, first);  // acc1 (+)= Ah Bl
-          tc::umma_f16_w(acc + GW_N, dAl + adv, dBh + adv, idesc, 1u);     // acc1  += Al Bh
+          tc::wg_ss_n128(acc0, dAh + adv, dBh + adv, first);  // acc0 (+)= Ah Bh
+          tc::wg_ss_n128(acc1, dAh + adv, dBl + adv, first);  // acc1 (+)= Ah Bl
+          tc::wg_ss_n128(acc1, dAl + adv, dBh + adv, 1u);     // acc1  += Al Bh
         }
-        tc::umma_commit_w(&empty[s]);
+        tc::wg_commit();
+        if (kc > 0) {  // the previous chunk's MMAs have completed: release its stage
+          tc::wg_wait<1>();
+          if (lane == 0) tc::mbar_arrive(&empty[(gk - 1) % GW_STAGES]);
+        }
       }
-      tc::umma_commit_w(&acc_full[b]);
-    }
-  } else {
-    // ===== epilogue warps: warp e owns ONE 32 x 32 block of every tile (rows = its TMEM lane quarter, column block e / 4) =====
-    const int ew = warp - 2;                 // 0..15
-    const int quarter = warp & 3;            // TMEM lane quarter this warp may access
-    const int cb = ew >> 2;                  // 32-column block of the tile
-    float* scratch = scratch_all + ew * (32 * GW_PAD);
-    const float scale = g.scale;
-    const int relu = g.relu;
-    const int rsub = lane >> 3, c4 = (lane & 7) * 4;  // read-back: 4 rows per pass, lane -> (row rsub, columns c4 .. c4 + 3)
-    int it = 0;
-    for (int tile = blockIdx.x; tile < g.tiles; tile += gridDim.x, ++it) {
-      int z, m0, n0;
-      decode(tile, z, m0, n0);
+      tc::wg_wait<0>();
+      if (lane == 0) tc::mbar_arrive(&empty[(gk - 1) % GW_STAGES]);
+
+      // ===== epilogue from the accumulator fragment =====
       const GemmProblem& pb = g.p[z];
       const int M = pb.M, N = pb.N;
-      const int b = it & 1;
-      const int mw = m0 + quarter * 32;
-      const int n = n0 + cb * 32 + c4;  // first of this lane's 4 columns
-      // operands that do not depend on the accumulator are fetched before the wait
-      float bias4[4] = {0.f, 0.f, 0.f, 0.f};
-      if (g.bias) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j)
-          if (n + j < N) bias4[j] = __ldg(g.bias + n + j);
-      }
-      const bool vec = pb.vec4 && n + 3 < N;  // 16-byte accesses allowed for this lane's chunk
-      ok = tc::mbar_wait(&acc_full[b], (it >> 1) & 1) && ok;
-      tc::fence_after_sync();
-      const uint32_t lane_base = tmem + b * (2 * GW_N) + ((uint32_t)(quarter * 32) << 16) + cb * 32;
-      {
-        float a0[32], a1[32];
-        tc::tmem_ld32(lane_base, a0);
-        tc::tmem_ld32(lane_base + GW_N, a1);
-        tc::fence_before_sync();
-        __syncwarp();
-        if (lane == 0) tc::mbar_arrive(&acc_empty[b]);  // this warp's share of the set is in registers
-        float4* dst = reinterpret_cast<float4*>(scratch + lane * GW_PAD);
-#pragma unroll
-        for (int c = 0; c < 8; ++c)
-          dst[c] = make_float4(fmaf(a1[4 * c], tc::LO_INV, a0[4 * c]), fmaf(a1[4 * c + 1], tc::LO_INV, a0[4 * c + 1]),
-                               fmaf(a1[4 * c + 2], tc::LO_INV, a0[4 * c + 2]), fmaf(a1[4 * c + 3], tc::LO_INV, a0[4 * c + 3]));
-      }
-      __syncwarp();
-      if (n < N) {
+      for (int j = 0; j < 16; ++j) {
+        const int n = n0 + 8 * j + c2;  // first of this thread's 2 columns
+        if (n >= N) continue;
+        const bool pair = n + 1 < N;
+        const bool vec = pb.vec4 && pair;  // 8-byte fp32 and 4-byte plane accesses allowed
+        float b2[2] = {0.f, 0.f};
+        if (g.bias) {
+          b2[0] = __ldg(g.bias + n);
+          if (pair) b2[1] = __ldg(g.bias + n + 1);
+        }
         const size_t hm_col = (size_t)(n >> 6) * M * 64 + (n & 63);  // head-major: [N / 64][M][64]
 #pragma unroll
-        for (int ps = 0; ps < 8; ++ps) {
-          const int r = ps * 4 + rsub;
-          const int row = mw + r;
-          if (row >= M) break;  // rows ascend with ps: nothing further for this lane
-          const float4 x4 = *reinterpret_cast<const float4*>(scratch + r * GW_PAD + c4);
-          float v[4] = {x4.x, x4.y, x4.z, x4.w};
+        for (int h = 0; h < 2; ++h) {
+          const int row = m0 + r0 + 8 * h;
+          if (row >= M) continue;
+          float v[2];
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            v[j] = (v[j] + bias4[j]) * scale;
-            if (relu) v[j] = fmaxf(v[j], 0.f);
+          for (int e = 0; e < 2; ++e) {
+            const int i = 4 * j + 2 * h + e;
+            v[e] = (fmaf(acc1[i], tc::LO_INV, acc0[i]) + b2[e]) * scale;
+            if (relu) v[e] = fmaxf(v[e], 0.f);
           }
           if (pb.resid) {
             const float* rp = pb.resid + (size_t)row * g.ldr + n;
             if (vec) {
-              const float4 rr = *reinterpret_cast<const float4*>(rp);
-              v[0] += rr.x, v[1] += rr.y, v[2] += rr.z, v[3] += rr.w;
+              const float2 rr = *reinterpret_cast<const float2*>(rp);
+              v[0] += rr.x, v[1] += rr.y;
             } else {
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                if (n + j < N) v[j] += rp[j];
+              v[0] += rp[0];
+              if (pair) v[1] += rp[1];
             }
           }
           const size_t off_c = g.head_major ? hm_col + (size_t)row * 64 : (size_t)row * pb.ldc + n;
           const size_t off_s = g.head_major ? hm_col + (size_t)row * 64 : (size_t)row * g.ldch + n;
           if (pb.C) {
             if (vec) {
-              *reinterpret_cast<float4*>(pb.C + off_c) = make_float4(v[0], v[1], v[2], v[3]);
+              *reinterpret_cast<float2*>(pb.C + off_c) = make_float2(v[0], v[1]);
             } else {
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                if (n + j < N) pb.C[off_c + j] = v[j];
+              pb.C[off_c] = v[0];
+              if (pair) pb.C[off_c + 1] = v[1];
             }
           }
           if (pb.Ch) {
             if (vec) {
-              uint32_t h01, l01, h23, l23;
-              if (g.lo_unscaled) {
-                tc::split2_unscaled_clamped(v[0], v[1], h01, l01);
-                tc::split2_unscaled_clamped(v[2], v[3], h23, l23);
-              } else {
-                tc::split2(v[0], v[1], h01, l01);
-                tc::split2(v[2], v[3], h23, l23);
-              }
-              *reinterpret_cast<uint2*>(pb.Ch + off_s) = make_uint2(h01, h23);
-              *reinterpret_cast<uint2*>(pb.Cl + off_s) = make_uint2(l01, l23);
+              uint32_t h01, l01;
+              if (g.lo_unscaled) tc::split2_unscaled_clamped(v[0], v[1], h01, l01);
+              else tc::split2(v[0], v[1], h01, l01);
+              *reinterpret_cast<uint32_t*>(pb.Ch + off_s) = h01;
+              *reinterpret_cast<uint32_t*>(pb.Cl + off_s) = l01;
             } else {
 #pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                if (n + j < N) {
+              for (int e = 0; e < 2; ++e) {
+                if (e == 0 || pair) {
                   __half hh, ll;
-                  if (g.lo_unscaled) tc::split_h_unscaled(v[j], hh, ll);
-                  else tc::split_h(v[j], hh, ll);
-                  pb.Ch[off_s + j] = hh;
-                  pb.Cl[off_s + j] = ll;
+                  if (g.lo_unscaled) tc::split_h_unscaled(v[e], hh, ll);
+                  else tc::split_h(v[e], hh, ll);
+                  pb.Ch[off_s + e] = hh;
+                  pb.Cl[off_s + e] = ll;
                 }
               }
             }
           }
         }
       }
-      __syncwarp();  // scratch is reused by the next tile
     }
   }
-  __syncwarp();
   if (!ok && g.err_flag) *g.err_flag = 1;
-  tc::fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tc::tmem_dealloc(tmem, 512);
 }

@@ -1,4 +1,4 @@
-// LightGlue matcher for sm_100a, as GTSfM drives it (features = "superpoint").
+// LightGlue matcher for sm_90a, as GTSfM drives it (features = "superpoint").
 //
 // Reference semantics restated (paths relative to the reference repo):
 //   thirdparty/LightGlue/lightglue/lightglue.py:31-43 (bbox keypoint normalisation), :68-81 (rotary table),
@@ -54,8 +54,8 @@ struct LgPair {  // one pair of the running batch: sides 2 * slot, 2 * slot + 1
 
 struct LightGlueState {
   bool loaded = false;
-  int persist_ctas = 148;  // CTAs of the persistent kernels = SMs of the device minus the context's reserve_sms
-  DevBuf wblob, wblob_h, wblob_l, errflag;  // fp32 weights + their split-fp16 (hi, lo * 2^11) copies for tcgen05
+  int persist_ctas = 132;  // CTAs of the persistent kernels = SMs of the device minus the context's reserve_sms
+  DevBuf wblob, wblob_h, wblob_l, errflag;  // fp32 weights + their split-fp16 (hi, lo * 2^11) copies for wgmma
   bool use_tc = true;                          // force_simt keeps every GEMM on the exact-fp32 SIMT kernel
   float* wr = nullptr;
   SelfW sw[LG_LAYERS];
@@ -169,7 +169,7 @@ __global__ void __launch_bounds__(256) k_lg_load_desc(const __grid_constant__ Jo
 }
 
 // qkv [N][768] with feature (h*64 + j)*3 + {q,k,v} (lightglue.py:166-167) -> rotary on q,k (:58-65) -> [4][N][64],
-// either as fp32 (SIMT attention) or split into fp16 hi / lo planes (tcgen05 attention; plane stride = 4*N*64 halves).
+// either as fp32 (SIMT attention) or split into fp16 hi / lo planes (wgmma attention; plane stride = 4*N*64 halves).
 struct RotJob {  // one image's share of a two-image launch (blockIdx.y)
   const float *qkv, *cs, *sn;
   int n;
@@ -777,7 +777,7 @@ static int lg_self_layer(b2_context* ctx, cudaStream_t st, LightGlueState* s, co
     }
     const int mx = lg_max_n(s, act);
     if (mx > 0) {
-      if (s->use_tc)  // q, k, v all feed the TMEM-operand attention: unscaled lo planes (bits 0 and 1)
+      if (s->use_tc)  // q, k, v all feed the wgmma attention: unscaled lo planes (bits 0 and 1)
         B2_LAUNCH(ctx, k_lg_split_rotary<true>, dim3(cdiv(mx * 128, 256), act.n), 256, 0, st, rj, 3);
       else
         B2_LAUNCH(ctx, k_lg_split_rotary<false>, dim3(cdiv(mx * 128, 256), act.n), 256, 0, st, rj, 0);
@@ -1015,7 +1015,7 @@ static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, con
   B2_CUDA(ctx, cudaMemcpyAsync(hread + 4 * LG_MAX_PAIRS, counters + 4 * LG_MAX_PAIRS, LG_MAX_PAIRS * sizeof(int), cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaMemcpyAsync(hread + 5 * LG_MAX_PAIRS, s->errflag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
-  if (s->use_tc && hread[5 * LG_MAX_PAIRS]) return b2_fail(ctx, B2_ERR_STATE, "tcgen05 pipeline timed out on an mbarrier (kernel bug)");
+  if (s->use_tc && hread[5 * LG_MAX_PAIRS]) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
   for (int li = 0; li < nlive; ++li) pairs[live[li]].out_k = hread[4 * LG_MAX_PAIRS + live[li]];
   ctx->debug["lg_desc0"] = {s->side[0].x[s->side[0].cur].as<float>(), (int64_t)s->side[0].n * 256};
   ctx->debug["lg_desc1"] = {s->side[1].x[s->side[1].cur].as<float>(), (int64_t)s->side[1].n * 256};

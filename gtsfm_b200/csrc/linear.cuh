@@ -1,5 +1,5 @@
 // Shared host-side dispatch for the matcher networks: one "linear" / attention call site expressed for both execution
-// paths (tcgen05 split-fp16 planes, or the exact-fp32 SIMT kernels under b2_set_option("force_simt", 1)), over a BATCH
+// paths (wgmma split-fp16 planes, or the exact-fp32 SIMT kernels under b2_set_option("force_simt", 1)), over a BATCH
 // of problems (the images of up to 8 pairs) per launch.
 #pragma once
 #include "attn_ps.cuh"
@@ -16,7 +16,7 @@ struct TcWeights {  // a model's weight blob in fp32 and as split-fp16 planes (s
   DevBuf* attn_part = nullptr;  // scratch for key-split attention partials (O) ...
   DevBuf* attn_ml = nullptr;    // ... (m, l) ...
   DevBuf* attn_cnt = nullptr;   // ... and the arrival counters of the in-kernel merge
-  int sm_count = 148;
+  int sm_count = 132;
 };
 
 struct Pl {  // split-fp16 planes of an activation
@@ -26,7 +26,7 @@ struct Pl {  // split-fp16 planes of an activation
 static inline Pl planes_of(const DevBuf& b, size_t elems) { return {b.as<__half>(), b.as<__half>() + elems}; }
 
 // One linear / GEMM call site of ONE problem, expressed for both execution paths: fp32 views feed the exact-fp32 SIMT
-// kernel, split-fp16 plane views feed the tcgen05 kernel.
+// kernel, split-fp16 plane views feed the wgmma kernel.
 struct LinArgs {
   const float* a1f = nullptr;
   Pl a1p{nullptr, nullptr};
@@ -42,9 +42,9 @@ struct LinArgs {
   float scale = 1.f;
   const float* resid = nullptr;
   int ldr = 0;
-  float* cf = nullptr;  // fp32 output (always written on the SIMT path; on the tcgen05 path only if tc_want_f32)
+  float* cf = nullptr;  // fp32 output (always written on the SIMT path; on the wgmma path only if tc_want_f32)
   int ldc = 0;
-  Pl cp{nullptr, nullptr};  // plane output (tcgen05 path)
+  Pl cp{nullptr, nullptr};  // plane output (wgmma path)
   int ldch = 0;
   int head_major = 0;
   bool tc_want_f32 = false;
@@ -54,7 +54,7 @@ struct LinArgs {
 };
 
 // `a[0 .. np)`: the same linear applied to np problems.  With a weight operand (a[0].w) every problem shares weights, K,
-// N and epilogue, and the tcgen05 path runs them as ONE persistent launch; with activation B operands (a[i].bf / bp: the
+// N and epilogue, and the wgmma path runs them as ONE persistent launch; with activation B operands (a[i].bf / bp: the
 // assignment similarity of each pair) N, ldc and B are per problem, K and the epilogue flags are a[0]'s.
 static int run_linear(b2_context* ctx, cudaStream_t st, const TcWeights& tw, const LinArgs* a, int np) {
   if (np <= 0) return B2_OK;
@@ -122,7 +122,7 @@ static int run_linear(b2_context* ctx, cudaStream_t st, const TcWeights& tw, con
   return B2_OK;
 }
 
-// One attention problem of a batched launch.  tcgen05 path: q / k / v / o buffers hold split fp16 planes (hi, then lo at
+// One attention problem of a batched launch.  wgmma path: q / k / v / o buffers hold split fp16 planes (hi, then lo at
 // + cap * 256 halves).
 struct FlashJob {
   const DevBuf *q, *k, *v, *o;
@@ -140,7 +140,7 @@ static int run_flash(b2_context* ctx, cudaStream_t st, const TcWeights& tw, cons
     }
     return B2_OK;
   }
-  if (!tma_encoder() || !tw.attn_part) return b2_fail(ctx, B2_ERR_CUDA, "tcgen05 attention needs cuTensorMapEncodeTiled and its scratch buffers");
+  if (!tma_encoder() || !tw.attn_part) return b2_fail(ctx, B2_ERR_CUDA, "wgmma attention needs cuTensorMapEncodeTiled and its scratch buffers");
   static thread_local AttnPsMaps tmaps;
   AttnPsArgs pa{};
   bool okm = true;

@@ -7,7 +7,7 @@
 //   -> sum of assignment-weighted residuals to the centres -> intra-normalisation -> flatten (d major, k minor) -> L2
 //   -> whitening Linear(32768 -> 4096) -> L2.
 //
-// The 12 convolutions with Cin >= 64 run on the SuperPoint convolution kernel (conv_ps.cuh: persistent tcgen05 implicit GEMM,
+// The 12 convolutions with Cin >= 64 run on the SuperPoint convolution kernel (conv_ps.cuh: persistent wgmma implicit GEMM,
 // halo reuse, split-fp16 = fp32-equivalent); the soft-assignment projection and the whitening layer run on the shared GEMM
 // (gemm_ws.cuh), the latter over a BATCH of images with K = 32768 walked in chunks (see retrieval.cu on the accumulator).
 // HBM layout: activations NHWC fp16 hi / lo planes, ping-pong; whitening weights as planes (2 x 268 MB), resident.
@@ -347,7 +347,7 @@ extern "C" int b2_netvlad_describe_dev(b2_context* ctx, const float* images, int
   int err = 0;
   B2_CUDA(ctx, cudaMemcpyAsync(&err, s->errflag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
-  if (err) return b2_fail(ctx, B2_ERR_STATE, "tcgen05 pipeline timed out on an mbarrier (kernel bug)");
+  if (err) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
   return B2_OK;
 }
 

@@ -1,4 +1,4 @@
-// RANSAC verifier for sm_100a: 5-point essential / 8-point fundamental hypotheses, squared-Sampson (E) or
+// RANSAC verifier for sm_90a: 5-point essential / 8-point fundamental hypotheses, squared-Sampson (E) or
 // symmetric-epiline (F) MSAC scoring, least-squares local optimisation, cheirality pose recovery.
 //
 // Replaces what the reference delegates to OpenCV at gtsfm/frontend/verifier/ransac.py:74-81,103-110 and
@@ -262,7 +262,7 @@ __device__ double block_sum(double v, double* sh) {
 // each of the 9 rounds of a sweep applies FOUR rotations on disjoint index pairs at once - their angles come from lanes
 // 0..3, the 4 x 9 two-element column updates of A and V and then the 4 x 9 row updates of A are spread over the lanes.
 // Disjoint rotations commute, so a round equals the same four rotations applied one after the other.  A single thread
-// walking the run-time indexed matrix in local memory (rmath::jacobi_eig<9>) took ~45 us per call on B200.
+// walking the run-time indexed matrix in local memory (rmath::jacobi_eig<9>) is much slower.
 __device__ void jacobi9_warp(double* A, double* V, int lane) {
   __shared__ double rc[4], rs[4];
   __shared__ int rp[4], rq[4];

@@ -5,7 +5,7 @@
 // lower triangle + diagonal + below min_score -> -inf, torch.topk per row, finite entries kept in (row, rank) order).
 // The global descriptors come from netvlad.cu (NetVLAD) or from the reference's own networks (MegaLoc).
 //
-// sim runs on the shared split-fp16 tcgen05 GEMM (fp32-equivalent); the selection is one warp per query row: `num_matched`
+// sim runs on the shared split-fp16 wgmma GEMM (fp32-equivalent); the selection is one warp per query row: `num_matched`
 // rounds of a warp arg-max over the row's valid entries strictly "after" the previous pick in (score desc, index asc) order.
 #include "common.cuh"
 #include "linear.cuh"
@@ -98,6 +98,6 @@ extern "C" int b2_similarity_pairs_host(b2_context* ctx, const float* desc, int 
   if (out_sim) B2_CUDA(ctx, cudaMemcpyAsync(out_sim, s->sim.p, (size_t)n * n * 4, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaMemcpyAsync(&err, s->err.p, 4, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
-  if (err) return b2_fail(ctx, B2_ERR_STATE, "tcgen05 pipeline timed out on an mbarrier (kernel bug)");
+  if (err) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
   return B2_OK;
 }

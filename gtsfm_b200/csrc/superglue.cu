@@ -1,4 +1,4 @@
-// SuperGlue matcher for sm_100a, as GTSfM drives it (outdoor weights, 20 Sinkhorn iterations, threshold 0.2).
+// SuperGlue matcher for sm_90a, as GTSfM drives it (outdoor weights, 20 Sinkhorn iterations, threshold 0.2).
 //
 // Reference semantics restated (paths relative to the reference repo):
 //   thirdparty/SuperGluePretrainedNetwork/models/superglue.py:63-82 (keypoint normalisation + encoder MLP),
@@ -7,7 +7,7 @@
 //   gtsfm/frontend/matcher/superglue_matcher.py:47-115.
 //
 // Features are kept [N][256] row-major (the reference's (1, 256, N) transposed): every Conv1d(k=1) is the same NT GEMM
-// as an nn.Linear and shares the tcgen05 split-fp16 kernels with LightGlue.  The host loader has already folded the
+// as an nn.Linear and shares the wgmma split-fp16 kernels with LightGlue.  The host loader has already folded the
 // eval-mode BatchNorms and permuted the q/k/v projection rows (and the merge columns) from the reference's
 // channel = dim * 4 + head interleave (superglue.py:104) to head-major, so attention runs on plain [4][N][64] operands.
 // The (M+1) x (N+1) coupling matrix is never materialised: the dustbin row / column are handled analytically.
@@ -477,7 +477,7 @@ static int sg_match_impl(b2_context* ctx, const float* kp0, const float* sc0, co
   B2_CUDA(ctx, cudaMemcpyAsync(&hres[0], counters, sizeof(int), cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaMemcpyAsync(&hres[1], s->errflag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
-  if (hres[1]) return b2_fail(ctx, B2_ERR_STATE, "tcgen05 pipeline timed out on an mbarrier (kernel bug)");
+  if (hres[1]) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
   *out_k = hres[0];
   ctx->debug["sg_desc0"] = {a.x.as<float>(), (int64_t)a.n * 256};
   return B2_OK;

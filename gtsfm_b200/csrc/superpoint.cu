@@ -1,4 +1,4 @@
-// SuperPoint detect + describe for sm_100a.
+// SuperPoint detect + describe for sm_90a.
 //
 // Reference semantics restated (file:line relative to the reference repo):
 //   thirdparty/SuperGluePretrainedNetwork/models/superpoint.py:145-202 (forward), :47-62 (simple_nms),
@@ -31,7 +31,7 @@ struct SuperPointState {
   DevBuf wblob;
   float* w[SP_NCONV] = {};
   float* b[SP_NCONV] = {};
-  // tcgen05 path: 3x3 weights as [cout][tap * cin] split-fp16 planes (B operand of the implicit GEMM)
+  // wgmma path: 3x3 weights as [cout][tap * cin] split-fp16 planes (B operand of the implicit GEMM)
   DevBuf wsplit_h, wsplit_l, errflag, conv_dbg, logits;
   struct ConvMapCache {
     ConvPsMaps maps;
@@ -128,24 +128,22 @@ __global__ void __launch_bounds__(C1A_THREADS) k_conv1a(const uint8_t* __restric
       const int yy = y + wr - 1, xx = x0 + wc - 1;
       if (lane < 18 && yy >= 0 && yy < H && xx >= 0 && xx < W) win = (float)__ldg(gray + (size_t)yy * W + xx) / 255.0f;
     }
-    float2 acc2[4];  // packed pairs: FFMA2 = two IEEE fp32 FMAs per issue slot, same bits as scalar fmaf
+    float acc[8];
 #pragma unroll
-    for (int c = 0; c < 4; ++c) acc2[c] = make_float2(b[2 * c], b[2 * c + 1]);
+    for (int c = 0; c < 8; ++c) acc[c] = b[c];
 #pragma unroll
     for (int dy = 0; dy < 3; ++dy) {
 #pragma unroll
       for (int dx = 0; dx < 3; ++dx) {
         const float v = __shfl_sync(0xffffffffu, win, dy * 6 + sub + dx);
 #pragma unroll
-        for (int c = 0; c < 4; ++c)
-          acc2[c] = tc::ffma2(make_float2(v, v), make_float2(w[dy * 3 + dx][2 * c], w[dy * 3 + dx][2 * c + 1]), acc2[c]);
+        for (int c = 0; c < 8; ++c) acc[c] = fmaf(v, w[dy * 3 + dx][c], acc[c]);
       }
     }
-    float acc[8];
 #pragma unroll
-    for (int c = 0; c < 4; ++c) acc[2 * c] = fmaxf(acc2[c].x, 0.f), acc[2 * c + 1] = fmaxf(acc2[c].y, 0.f);
+    for (int c = 0; c < 8; ++c) acc[c] = fmaxf(acc[c], 0.f);
     if (x0 + sub >= W) continue;
-    if (oh) {  // split fp16 planes for the tcgen05 convolutions
+    if (oh) {  // split fp16 planes for the wgmma convolutions
       uint32_t hi[4], lo[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) tc::split2(acc[2 * i], acc[2 * i + 1], hi[i], lo[i]);
@@ -313,7 +311,7 @@ __global__ void __launch_bounds__(128) k_head_scores(const float* __restrict__ c
   }
 }
 
-// tcgen05 path of the two 1x1 heads: the channel mixing runs on k_gemm_ws (linear.cuh), these finish the job.
+// wgmma path of the two 1x1 heads: the channel mixing runs on k_gemm_ws (linear.cuh), these finish the job.
 // softmax over the 65 logits of a cell, drop the dustbin, depth-to-space (superpoint.py:162-166): one warp per cell.
 __global__ void __launch_bounds__(256) k_head_softmax(const float* __restrict__ logits, int ld, float* __restrict__ heat, int Hc, int Wc) {
   const int cell = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -341,8 +339,8 @@ __global__ void __launch_bounds__(256) k_head_l2norm(float* __restrict__ dense, 
 
 // simple_nms with radius 4 (superpoint.py:47-62), fused over a tile with a 20-pixel halo, followed by the
 // threshold + border test (superpoint.py:170-178) feeding per-row keypoint counts.
-// tile 64 x 40: a VGA score map is 10 x 12 = 120 tiles = ONE wave of 1-CTA-per-SM blocks (64 x 32 gave 150 tiles = two waves on
-// 148 SMs: half of the 47 us the kernel took was the second, 2-block wave)
+// tile 64 x 40: a VGA score map is 10 x 12 = 120 tiles = ONE wave of 1-CTA-per-SM blocks (64 x 32 gives 150 tiles = two waves on
+// 132 SMs)
 constexpr int NT_W = 64, NT_H = 40, NR = 4, NHALO = 5 * NR;
 constexpr int NRW = NT_W + 2 * NHALO, NRH = NT_H + 2 * NHALO;  // 104 x 80 region = tile + the 20-px halo the five pools need
 constexpr int NREG = NRW * NRH;
@@ -625,7 +623,7 @@ static int sp_conv3x3(b2_context* ctx, cudaStream_t st, const float* in, int li,
   return B2_OK;
 }
 
-// tcgen05 implicit-GEMM convolution on split-fp16 NHWC planes (conv_ps.cuh: persistent, halo reuse, resident weights).
+// wgmma implicit-GEMM convolution on split-fp16 NHWC planes (conv_ps.cuh: persistent, halo reuse, resident weights).
 // `in` / `out` buffers hold the hi plane followed by the lo plane (+ pixels * channels halves).
 static int sp_conv3x3_tc(b2_context* ctx, cudaStream_t st, const DevBuf& in, int li, int H, int W, bool pool, DevBuf* out_planes,
                          float* out_f32) {
@@ -649,9 +647,10 @@ static int sp_conv3x3_tc(b2_context* ctx, cudaStream_t st, const DevBuf& in, int
   if (out_planes) a.Oh = out_planes->as<__half>(), a.Ol = a.Oh + (size_t)OH * OW * Cout;
   a.Of = out_f32, a.err_flag = s->errflag.as<int>();
   if (getenv("B2_CONV_DBG")) {  // profiling runs: per-CTA timestamps of layer li, read back through b2_debug_fetch("conv_dbg")
-    if (s->conv_dbg.ensure((size_t)12 * 148 * 8 * sizeof(float)) == cudaSuccess) {
-      a.dbg = s->conv_dbg.as<float>() + (size_t)li * 148 * 8;
-      ctx->debug["conv_dbg"] = {s->conv_dbg.as<float>(), (int64_t)12 * 148 * 8};
+    const size_t per_layer = (size_t)ctx->sm_count * 8;
+    if (s->conv_dbg.ensure(12 * per_layer * sizeof(float)) == cudaSuccess) {
+      a.dbg = s->conv_dbg.as<float>() + li * per_layer;
+      ctx->debug["conv_dbg"] = {s->conv_dbg.as<float>(), (int64_t)(12 * per_layer)};
     }
   }
   const int nblk = Cout / 64, units = cdiv(W, CP_TW) * cdiv(H, CP_TH) * nblk;
@@ -663,7 +662,7 @@ static int sp_conv3x3_tc(b2_context* ctx, cudaStream_t st, const DevBuf& in, int
   return B2_OK;
 }
 
-// 1x1 head (convPb / convDb) on the shared tcgen05 GEMM: out[cell][n] = sum_k in[cell][k] * W[n][k] + bias[n]  (fp32-equivalent)
+// 1x1 head (convPb / convDb) on the shared wgmma GEMM: out[cell][n] = sum_k in[cell][k] * W[n][k] + bias[n]  (fp32-equivalent)
 static int sp_head_gemm(b2_context* ctx, cudaStream_t st, const DevBuf& in_planes, int li, int cells, float* out, int ldc) {
   SuperPointState* s = ctx->sp;
   const int K = SP_CI[li], N = SP_CO[li];
@@ -723,7 +722,7 @@ extern "C" int b2_superpoint_set_weights(b2_context* ctx, const float* blob, siz
     B2_CUDA(ctx, cudaMemcpy(s->w[l], packed.data() + woff[l], nw * sizeof(float), cudaMemcpyHostToDevice));
     B2_CUDA(ctx, cudaMemcpy(s->b[l], packed.data() + boff[l], SP_CO[l] * sizeof(float), cudaMemcpyHostToDevice));
   }
-  // tcgen05 path: [cout][tap * cin + ci] fp32 -> split planes (one device split kernel over a host-built fp32 staging copy)
+  // wgmma path: [cout][tap * cin + ci] fp32 -> split planes (one device split kernel over a host-built fp32 staging copy)
   {
     size_t tot = 0;
     for (int l = 0; l < SP_NCONV; ++l) {
@@ -781,12 +780,12 @@ static int sp_enqueue_network(b2_context* ctx, cudaStream_t st, int H, int W, fl
   float* head = s->head.as<float>();
   int rc;
   const bool tcp = s->use_tc;
-  DevBuf& featp = s->kpxy;  // (tcgen05 path) split planes of conv4b's output: operand of convPa and convDa
+  DevBuf& featp = s->kpxy;  // (wgmma path) split planes of conv4b's output: operand of convPa and convDa
   if (tcp) {
     __half* p0 = s->a0.as<__half>();
     B2_LAUNCH(ctx, k_conv1a, (unsigned)(ctx->sm_count * 8), C1A_THREADS, 0, st, s->gray.as<uint8_t>(), s->w[0], s->b[0], a0, H, W, p0, p0 + px * 64);
     B2_CHECK_LAUNCH(ctx);
-    // encoder (superpoint.py:148-158) as TMA-fed tcgen05 implicit GEMMs on split-fp16 planes; pools fused
+    // encoder (superpoint.py:148-158) as TMA-fed wgmma implicit GEMMs on split-fp16 planes; pools fused
     if ((rc = sp_conv3x3_tc(ctx, st, s->a0, 1, H, W, true, &s->a1, nullptr))) return rc;      // conv1b + pool
     if ((rc = sp_conv3x3_tc(ctx, st, s->a1, 2, H2, W2, false, &s->a0, nullptr))) return rc;   // conv2a
     if ((rc = sp_conv3x3_tc(ctx, st, s->a0, 3, H2, W2, true, &s->a1, nullptr))) return rc;    // conv2b + pool
@@ -887,9 +886,8 @@ static int sp_detect_impl(b2_context* ctx, const uint8_t* image, int H, int W, i
   B2_LAUNCH(ctx, k_to_gray, dim3(cdiv(W, 256), H), 256, 0, st, image, pitch, channels, H, W, s->gray.as<uint8_t>());
   B2_CHECK_LAUNCH(ctx);
   // OPT-IN (b2_set_option "superpoint_graph" / B2_SP_GRAPH=1): the network's ~21 launches replayed as ONE CUDA graph per (shape,
-  // parameters, buffers) key, captured on a private stream the first time the key is seen.  Measured on B200 at 640x480: 2140
-  // img/s with the graph against 2290 with direct launches - the host enqueues faster than the GPU drains, so there is no
-  // launch gap for a graph to remove, and a graph launch starts later than the first direct launch.  Direct launches when one of its kernels is being profiled, on the SIMT path, with
+  // parameters, buffers) key, captured on a private stream the first time the key is seen.  The host
+  // enqueues faster than the GPU drains, so there is no launch gap for a graph to remove.  Direct launches when one of its kernels is being profiled, on the SIMT path, with
   // B2_SP_GRAPH=0, or when the key keeps changing (caller-owned output pointers that move on every call).
   int rc;
   SuperPointState::GraphSlot* hit = nullptr;
@@ -951,7 +949,7 @@ static int sp_detect_impl(b2_context* ctx, const uint8_t* image, int H, int W, i
     B2_CUDA(ctx, cudaMemcpyAsync(&n, s->rowoff.as<int>() + H8, sizeof(int), cudaMemcpyDeviceToHost, st));
     if (tcp) B2_CUDA(ctx, cudaMemcpyAsync(&err, s->errflag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     B2_CUDA(ctx, cudaStreamSynchronize(st));
-    if (err) return b2_fail(ctx, B2_ERR_STATE, "tcgen05 conv pipeline timed out on an mbarrier (kernel bug)");
+    if (err) return b2_fail(ctx, B2_ERR_STATE, "wgmma conv pipeline timed out on an mbarrier (kernel bug)");
   }
   s->n_kp = n;
   s->have_dense = true;
@@ -1196,7 +1194,7 @@ extern "C" int b2_superpoint_extract_dev(b2_context* ctx, const uint8_t* image, 
   B2_CUDA(ctx, cudaMemcpyAsync(&n, s->sel_cnt.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaMemcpyAsync(&err, s->errflag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
-  if (err) return b2_fail(ctx, B2_ERR_STATE, "tcgen05 conv pipeline timed out on an mbarrier (kernel bug)");
+  if (err) return b2_fail(ctx, B2_ERR_STATE, "wgmma conv pipeline timed out on an mbarrier (kernel bug)");
   *out_n = n;
   return B2_OK;
 }
@@ -1227,6 +1225,6 @@ extern "C" int b2_superpoint_finish_dev(b2_context* ctx, void* stream) {
   int err = 0;
   B2_CUDA(ctx, cudaMemcpyAsync(&err, s->errflag.p, sizeof(int), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   B2_CUDA(ctx, cudaStreamSynchronize((cudaStream_t)stream));
-  if (err) return b2_fail(ctx, B2_ERR_STATE, "tcgen05 conv pipeline timed out on an mbarrier (kernel bug)");
+  if (err) return b2_fail(ctx, B2_ERR_STATE, "wgmma conv pipeline timed out on an mbarrier (kernel bug)");
   return B2_OK;
 }

@@ -1,7 +1,7 @@
-// Tensor Memory Accelerator helpers shared by the tcgen05 kernels: 128-byte-swizzled K-major UMMA descriptors, TMA tile
-// loads signalled on mbarriers (complete_tx), host-side tensor-map construction, and the fp32 -> split-fp16 plane kernel.
+// Tensor Memory Accelerator helpers shared by the wgmma kernels: TMA tile loads signalled on mbarriers (complete_tx),
+// host-side tensor-map construction, and the fp32 -> split-fp16 plane kernel.
 //
-// Shared-memory tile = [rows][64 halves] with 128-byte rows, XOR-swizzled in 8-row x 128-byte atoms: the UMMA descriptor
+// Shared-memory tile = [rows][64 halves] with 128-byte rows, XOR-swizzled in 8-row x 128-byte atoms: the wgmma descriptor
 // is layout SWIZZLE_128B, SBO = 1024 B (one atom), and one MMA K step (16 halves) advances the start address by 32 B.
 // Tiles are 1024-byte aligned.
 #pragma once
@@ -12,18 +12,6 @@
 #include "tc.cuh"
 
 namespace tc {
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;               // leading byte offset field (unused for swizzled K-major; canonical value 1)
-  d |= (uint64_t)(1024 >> 4) << 32;     // stride byte offset: one 8-row x 128-byte swizzle atom
-  d |= (uint64_t)1 << 46;               // descriptor version 1 (Blackwell)
-  d |= (uint64_t)2 << 61;               // layout type SWIZZLE_128B
-  return d;
-}
-// MN-major operand stored [k][64 mn-elements] with 128-byte rows, 128-byte swizzle: SBO = 8-row group stride
-__device__ __forceinline__ uint64_t smem_desc_sw128_mn(uint32_t saddr) { return smem_desc_sw128(saddr); }
-
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }

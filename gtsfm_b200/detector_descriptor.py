@@ -1,11 +1,11 @@
-"""B200 SuperPoint detector-descriptor plugin.
+"""SuperPoint detector-descriptor plugin.
 
 Drop-in for gtsfm/frontend/detector_descriptor/superpoint.py:32-93 (`SuperPointDetectorDescriptor`): same constructor
 arguments, same `detect_and_describe(image) -> (Keypoints, (N, 256) float32)` contract, same post-processing order
 (mask filter, then `Keypoints.get_top_k` i.e. numpy argpartition, gtsfm/.../superpoint.py:87-91), lazily created
 device state so the object stays picklable (tests/frontend/detector/test_detector_base.py:51-56).
 
-All arithmetic runs in libgtsfm_b200.so (CUDA, sm_100a); this file only moves numpy buffers across the C ABI.  The one
+All arithmetic runs in libgtsfm_b200.so (CUDA, sm_90a); this file only moves numpy buffers across the C ABI.  The one
 deliberate difference from the reference data flow: descriptors are sampled on the GPU only for the keypoints that
 survive the host-side mask / top-k selection, instead of for every detection (identical values, 3x less D2H at 5000 of
 17000 keypoints).
@@ -77,7 +77,7 @@ class SuperPointEngine:
 
 
 class B200SuperPointDetectorDescriptor(DetectorDescriptorBase):
-    """SuperPoint on hand-written sm_100a kernels behind GTSfM's DetectorDescriptorBase."""
+    """SuperPoint on hand-written sm_90a kernels behind GTSfM's DetectorDescriptorBase."""
 
     def __init__(self, max_keypoints: int = 5000, use_cuda: bool = True, weights_path: Union[Path, str, dict, None] = None,
                  device: int = 0) -> None:

@@ -1,10 +1,10 @@
-"""B200 NetVLAD global descriptor plugin (SURVEY.md section 8f rank 4: the retrieval front of deep_front_end.yaml:6-15).
+"""NetVLAD global descriptor plugin (SURVEY.md section 8f rank 4: the retrieval front of deep_front_end.yaml:6-15).
 
 Drop-in for gtsfm/frontend/global_descriptor/netvlad_global_descriptor.py:24-71 (`NetVLADGlobalDescriptor`, a
 `GlobalDescriptorBase`): same `get_preprocessing_transforms` / `describe_batch(images (B, 3, H, W) float in [0, 1]) -> list of
 (4096,) arrays` contract, model loaded lazily on first use.  The network of thirdparty/hloc/netvlad.py runs in
-libgtsfm_b200.so (`b2_netvlad_describe_dev`): VGG16 convolutions on the SuperPoint tcgen05 convolution kernel, soft assignment
-and whitening on the shared tcgen05 GEMM.
+libgtsfm_b200.so (`b2_netvlad_describe_dev`): VGG16 convolutions on the SuperPoint wgmma convolution kernel, soft assignment
+and whitening on the shared wgmma GEMM.
 """
 from __future__ import annotations
 

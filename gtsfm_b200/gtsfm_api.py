@@ -1,6 +1,6 @@
 """The reference's plugin API, re-used when GTSfM is importable and mirrored when it is not.
 
-Inside a GTSfM environment the B200 plugins subclass the reference's own abstract bases so they drop into
+Inside a GTSfM environment the plugins subclass the reference's own abstract bases so they drop into
 scene_optimizer.py through a Hydra `_target_` swap (SURVEY.md §8b):
 
   * gtsfm/frontend/detector_descriptor/detector_descriptor_base.py:19-57   DetectorDescriptorBase

@@ -1,4 +1,4 @@
-"""B200 LightGlue / SuperGlue matcher plugins.
+"""LightGlue / SuperGlue matcher plugins.
 
 Drop-ins for gtsfm/frontend/matcher/lightglue_matcher.py:24-112 (`LightGlueMatcher`) and
 gtsfm/frontend/matcher/superglue_matcher.py:30-115 (`SuperGlueMatcher`): same `match(...)` signature, argument
@@ -55,7 +55,7 @@ class LightGlueEngine:
 
 
 class B200LightGlueMatcher(MatcherBase):
-    """LightGlue on hand-written sm_100a kernels behind GTSfM's MatcherBase.
+    """LightGlue on hand-written sm_90a kernels behind GTSfM's MatcherBase.
 
     `cpu_semantics=True` (default) reproduces what the reference computes on its CPU front-end (pruning attempted at
     every layer, lightglue.py:339-344) and is what the parity fixtures pin; False uses the reference's CUDA+flash
@@ -142,7 +142,7 @@ class SuperGlueEngine:
 
 
 class B200SuperGlueMatcher(MatcherBase):
-    """SuperGlue on hand-written sm_100a kernels behind GTSfM's MatcherBase (gtsfm/frontend/matcher/superglue_matcher.py:30-115)."""
+    """SuperGlue on hand-written sm_90a kernels behind GTSfM's MatcherBase (gtsfm/frontend/matcher/superglue_matcher.py:30-115)."""
 
     def __init__(self, use_cuda: bool = True, use_outdoor_model: bool = True, weights_path: Union[Path, str, dict, None] = None, device: int = 0):
         super().__init__()

@@ -32,14 +32,14 @@ class DeviceFeatures:
         return int(self.kp.shape[0])
 
 
-# concurrent LightGlue instances used by match_many.  Default 1: measured on B200 (40-pair steps of 5000 x 5000 keypoints) 215.8 /
-# 224.5 / 217.0 pairs/s with 1 / 2 / 3 lanes - the matcher's persistent kernels already fill the GPU, unlike SuperPoint's
+# concurrent LightGlue instances used by match_many.  Default 1: the matcher's persistent kernels already fill the GPU (H100,
+# 40-pair steps of 5000 x 5000 keypoints: 99-105 pairs/s for 1 to 4 lanes, within run-to-run spread)
 MATCH_LANES = int(os.environ.get("B2_MATCH_LANES", "1"))
-# concurrent SuperGlue instances used by match_superglue_many: 117.9 / 122.7 / 129.3 / 130.9 pairs/s with 1 / 2 / 3 / 4 lanes (B200,
-# 40-pair steps at 5000 keypoints, RANSAC on its own stream)
-SG_LANES = int(os.environ.get("B2_SG_LANES", "3"))
+SG_LANES = int(os.environ.get("B2_SG_LANES", "3"))  # concurrent SuperGlue instances used by match_superglue_many
 DETECT_LANES = int(os.environ.get("B2_DETECT_LANES", "4"))  # concurrent SuperPoint instances used by detect_many
-RESERVE_SMS_FOR_VERIFY = int(os.environ.get("B2_RESERVE_SMS", "8"))  # k_rs_hyp_E keeps 16 x 64-thread CTAs busy for ~1 ms
+# SMs the matcher's persistent kernels leave to the concurrent RANSAC kernels.  H100 (132 SMs), 40-pair LightGlue steps:
+# 99 pairs/s reserving 8, 103-107 reserving 0-4; 4 keeps k_rs_hyp_E's CTAs off the matcher's SMs at no measured cost
+RESERVE_SMS_FOR_VERIFY = int(os.environ.get("B2_RESERVE_SMS", "4"))
 
 
 class DeviceFrontEnd:

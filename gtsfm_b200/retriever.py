@@ -1,4 +1,4 @@
-"""B200 similarity retriever (SURVEY.md section 8f rank 4: the pair-selection step in front of the hot path).
+"""similarity retriever (SURVEY.md section 8f rank 4: the pair-selection step in front of the hot path).
 
 Drop-in for gtsfm/retriever/similarity_retriever.py:35-182 (`SimilarityRetriever`): same constructor, `get_image_pairs`
 contract (ValueError without descriptors, RuntimeError above MAX_NUM_IMAGES, pairs (i1 < i2) per query image best first),

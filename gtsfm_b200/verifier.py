@@ -1,4 +1,4 @@
-"""B200 RANSAC verifier plugin.
+"""RANSAC verifier plugin.
 
 Drop-in for gtsfm/frontend/verifier/ransac.py:51-111 (`Ransac`, an `OpencvVerifierBase`): same constructor, same
 `verify(...) -> (Rot3 | None, Unit3 | None, (K', 2) rows of match_indices, inlier ratio)` contract, same guards and
@@ -87,7 +87,7 @@ class RansacEngine:
 
 
 class B200Ransac(VerifierBase):
-    """5-point / 8-point RANSAC on sm_100a kernels behind GTSfM's VerifierBase."""
+    """5-point / 8-point RANSAC on sm_90a kernels behind GTSfM's VerifierBase."""
 
     def __init__(self, use_intrinsics_in_verification: bool, estimation_threshold_px: float, device: int = 0, seed: int = DEFAULT_SEED) -> None:
         super().__init__(use_intrinsics_in_verification, estimation_threshold_px)

@@ -1,5 +1,5 @@
 /*
- * gtsfm_b200 — C ABI of the B200-native pairwise deep front-end (SuperPoint -> LightGlue/SuperGlue -> RANSAC).
+ * gtsfm_b200 — C ABI of the H100-native pairwise deep front-end (SuperPoint -> LightGlue/SuperGlue -> RANSAC).
  *
  * This is the drop-in boundary (SURVEY.md §8b).  Every entry point is plain C: opaque handle, raw pointers, sizes,
  * an `int` status (0 = ok, <0 = error; text via b2_last_error).  No torch / C++ types cross it.  `*_dev` entry points
@@ -35,7 +35,7 @@ typedef struct b2_context b2_context;
 
 /* ---- lifecycle -------------------------------------------------------------------------------------------------- */
 int b2_version(void);
-/* Creates a context on CUDA device `device`.  Fails (returns <0, *out = NULL) when no sm_100 device is present. */
+/* Creates a context on CUDA device `device`.  Fails (returns <0, *out = NULL) when no sm_90 device is present. */
 int b2_create(int device, b2_context** out);
 void b2_destroy(b2_context* ctx);
 const char* b2_last_error(const b2_context* ctx);
@@ -48,10 +48,10 @@ uint64_t b2_h2d_bytes(const b2_context* ctx);
  * kernels of OTHER contexts / streams running concurrently (the batched front-end overlaps pair k's RANSAC with pair
  * k+1's matching; a one-CTA-per-SM kernel that finds an SM busy would otherwise wait for a whole CTA lifetime).
  * "lightglue_batch" = 0..8: pairs per lock-step batch of b2_lightglue_match_batched_dev (0 = 8, the maximum).
- * "force_simt" = 0 | 1: models whose weights are set afterwards run the exact-fp32 SIMT kernels instead of the tcgen05
+ * "force_simt" = 0 | 1: models whose weights are set afterwards run the exact-fp32 SIMT kernels instead of the wgmma
  * split-fp16 ones (the on-device cross-check of the tensor-core path; tests only).
  * "superpoint_graph" = 0 (default) | 1: launch every kernel of the SuperPoint network directly / replay the ~21 launches as one
- * CUDA graph per (image shape, parameters, buffers) key (measured slower on B200: the path is GPU-bound, not launch-bound).
+ * CUDA graph per (image shape, parameters, buffers) key (the path is GPU-bound, not launch-bound).
  * "feature_cache" = 0 | 1: drop every cached device copy of host feature arrays and (0, default) copy on every call like the
  * reference / (1) keep device copies keyed by (host pointer, size) and validated by a hash of the FULL contents, so arrays
  * edited in place are re-sent.  Only pays off for callers that pass the same numpy buffers repeatedly (it does nothing for
@@ -65,8 +65,8 @@ int b2_profile_stop(b2_context* ctx, double* total_ms, uint64_t* launches, doubl
 /* Copies a named intermediate device buffer of the last call to host (tests only). Returns #floats written or <0. */
 int64_t b2_debug_fetch(b2_context* ctx, const char* name, float* host_out, int64_t max_floats);
 
-/* Test-only: C[M,N] = A[M,K] * B[N,K]^T (+ bias) on HOST fp32 buffers.  mode 0 = SIMT fp32 kernel, 1 = tcgen05 split-fp16
- * kernel with fp32 B converted in-kernel, 2 = tcgen05 split-fp16 kernel with pre-split fp16 B.  K must be a multiple of 64. */
+/* Test-only: C[M,N] = A[M,K] * B[N,K]^T (+ bias) on HOST fp32 buffers.  mode 0 = SIMT fp32 kernel, 1 = wgmma split-fp16
+ * kernel with fp32 B converted in-kernel, 2 = wgmma split-fp16 kernel with pre-split fp16 B.  K must be a multiple of 64. */
 int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, const float* B, const float* bias, float* C, int M, int N,
                        int K);
 

@@ -11,7 +11,7 @@ GOLDEN = ROOT / "tests" / "golden"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run on the GPU box with `pytest -m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (`pytest -m gpu`)")
 
 
 def pytest_sessionstart(session):

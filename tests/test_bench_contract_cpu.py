@@ -1,5 +1,5 @@
-"""CPU: the committed bench lines (profiles/r02_bench_*.json, produced by `python bench.py --workload W` on a B200) carry every key of
-the bench contract, with consistent values - a schema guard for bench.py's output, not a measurement."""
+"""CPU: the committed bench lines (profiles/h100_bench_*.json, produced by `python bench.py --workload W` on an H100) carry every key
+of the bench contract, with consistent values - a schema guard for bench.py's output, not a measurement."""
 import json
 from pathlib import Path
 
@@ -11,7 +11,7 @@ WORKLOADS = ["vga_lightglue", "mp1_lightglue", "seq_superglue", "superpoint_only
 
 @pytest.mark.parametrize("w", WORKLOADS)
 def test_line_has_the_contract_keys(w):
-    d = json.loads((PROFILES / f"r02_bench_{w}.json").read_text())
+    d = json.loads((PROFILES / f"h100_bench_{w}.json").read_text())
     for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline", "dtype",
               "data", "config", "clocks", "e2e", "gpu_launches", "roofline", "cpu_baseline"):
         assert k in d, k
@@ -25,15 +25,15 @@ def test_line_has_the_contract_keys(w):
     assert 0 < r["frac"] < 0.4 and "traffic" in r
     c = d["cpu_baseline"]
     assert c["kind"] in ("reference", "port") and c["value"] > 0 and c["cores"] >= 1 and c["unit"] == d["unit"] and c["sample"]
-    assert d["value"] / c["value"] > 50  # north_star: >= 50x the reference's CPU path on one B200
+    assert d["value"] / c["value"] > 50  # north_star: >= 50x the reference's CPU path on one GPU
     k = d["clocks"]
     assert not {"hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown"} & set(k["reasons"])
 
 
 def test_default_line_is_the_dominant_kernel_story():
-    d = json.loads((PROFILES / "r02_bench_vga_lightglue.json").read_text())
+    d = json.loads((PROFILES / "h100_bench_vga_lightglue.json").read_text())
     r = d["roofline"]
-    assert r["kernel"].startswith("k_flash") and r["traffic"] and 0.5 < r["kernel_share_of_step"] < 0.65
+    assert r["kernel"].startswith("k_flash") and "traffic" in r and 0.5 < r["kernel_share_of_step"] < 0.65
     fam = d["extra"]["kernel_family_ms_per_step"]
     assert fam["k_gemm_ws"]["ms_per_step"] < r["kernel_ms_per_step"]  # attention, not the linears, dominates the step
     assert d["e2e"]["host_threads"] >= 1 and d["e2e"]["single_thread"] <= d["e2e"]["value"] * 1.05

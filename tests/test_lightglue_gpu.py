@@ -57,7 +57,7 @@ def test_bench_sequence_chain(b200_ctx, golden_dir):
 @pytest.mark.parametrize("tag", ["full_5", "prune_7", "stop_8"])
 def test_exact_fp32_simt_path(golden_dir, tag):
     """The exact-fp32 SIMT kernels (set_option force_simt: no tensor cores, no planes) are the on-device cross-check of the
-    split-fp16 tcgen05 path; they must reproduce the same fixtures."""
+    split-fp16 wgmma path; they must reproduce the same fixtures."""
     from gtsfm_b200 import _lib
 
     ctx = _lib.Context(0)

@@ -67,8 +67,7 @@ def test_detection_equals_reference(b200_ctx, golden_dir, i):
 
 
 def test_moved_keypoints_are_rare(b200_ctx, golden_dir):
-    """Over the 207 000 detections of the 12 frames at most 3 may sit in a different pixel of their NMS window
-    (measured on B200: 2, both in frame 6 around (414, 113))."""
+    """Over the 207 000 detections of the 12 frames at most 3 may sit in a different pixel of their NMS window."""
     _features(b200_ctx, golden_dir)
     assert sum(len(m[1]) for m in _cache.get("moved", [])) <= 3, _cache.get("moved")
 

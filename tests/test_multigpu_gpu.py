@@ -1,6 +1,6 @@
 """GPU, 2 devices: ONE job split over two ranks (NCCL) through B200CorrespondenceGenerator - every image detected on one rank, features
 all-gathered, pairs sharded p mod world, two-view verification under the matching - gives exactly the single-process results.
-Skipped on one-GPU boxes (the 2-GPU evidence run executes it: profiles/bench_r02_2gpu.sh)."""
+Skipped on machines with one GPU."""
 import os
 
 import numpy as np

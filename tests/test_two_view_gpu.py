@@ -43,7 +43,7 @@ def test_batch_equals_per_pair_plugins():
 
 def test_batch_matches_the_oracle():
     """Putative matches must be the oracle's LightGlue rows bit for bit; pose / verified rows must agree with what
-    cv2.findEssentialMat(USAC_ACCURATE) + recoverPose return for them (OpenCV's RANSAC is not in /root/reference, so the
+    cv2.findEssentialMat(USAC_ACCURATE) + recoverPose return for them (OpenCV's RANSAC is not part of the reference project, so the
     verified set is compared by IoU and the pose by angle: the tolerances of tests/test_verifier_gpu.py)."""
     from oracle import lightglue_ref, verifier_ref
 
