@@ -8,9 +8,25 @@
 //
 // Schedule: one CTA per SM walks output tiles `blockIdx.x + i * gridDim.x` of the whole batch (problem-major, then row
 // tile, then column tile - concurrently running CTAs share the A row tile through L2):
-//   warp 8 (lane 0)  TMA producer: a 3-stage ring (3 x 64 KB) that keeps loading the next tile during the epilogue
-//   warps 0-7        warpgroup w: rows 64w .. 64w + 63 of the 128 x 128 tile, wgmma m64n128k16 into two register
-//                    accumulators, then bias / scale / ReLU / residual / split-plane stores from the fragment.
+//   warps 0-7        consumer warpgroup w: rows 64w .. 64w + 63 of the 128 x 128 tile, wgmma m64n128k16 into two register
+//                    accumulators; at the end of the tile they write fmaf(acc1, 2^-11, acc0) as fp32 into a shared
+//                    staging tile and go straight on to the next tile's MMAs
+//   warps 8-11       epilogue warpgroup: reads the staging tile row by row and applies bias / scale / ReLU / residual,
+//                    then writes fp32 and / or split planes with 16-byte (fp32) and 8-byte (plane) coalesced stores
+//   warp 12 (lane 0) TMA producer: a 2-stage ring (2 x 64 KB) that runs ahead into the next tile's K chunks; warps 13-15
+//                    only exist so that the producer has a warpgroup of its own for setmaxnreg
+// With K = 256 or 512 a tile is only 6 k - 12 k tensor cycles while its epilogue writes 64 - 192 KB, so the epilogue, not
+// the operand traffic, paces the linears: running it in the consumers left the tensor cores idle for the whole of it.
+// Here the epilogue of tile t overlaps the MMAs of tile t + 1; the single staging buffer is handed over with two
+// mbarriers (sfull: 256 consumer arrivals, sempty: 128 epilogue arrivals).
+// Registers: 512 threads start at 128 each; setmaxnreg moves them to the consumers (184), leaving the epilogue 104 and the
+// producer 40 (ptxas: no spills, no serialised wgmma).  Without the rebalance, a fourth epilogue warp (416 threads) made
+// ptxas cap the kernel at 128 registers and spill the accumulators; with 3 epilogue warps and no rebalance the family took
+// 91-93 ms per vga_lightglue step against 85 ms with 4 (H100 80GB HBM3, three alternated runs each).
+// Shared memory: 2 x 64 KB ring + 68 KB staging (a third ring stage no longer fits).  The epilogue computes exactly what
+// the consumers used to: (fmaf(acc1, 2^-11, acc0) + bias) * scale, ReLU, + residual, then the same split helpers.  Its
+// mode flags (relu, head-major, unscaled lo, which outputs) are read once per tile and are warp-uniform; they are not
+// compile-time specialisations.
 #pragma once
 #include "tma.cuh"
 
@@ -19,16 +35,21 @@ constexpr int GW_M = 128, GW_N = 128, GW_K = 64;
 constexpr int GW_A_BYTES = GW_M * GW_K * 2;  // 16 KB per plane
 constexpr int GW_B_BYTES = GW_N * GW_K * 2;  // 16 KB per plane
 constexpr int GW_STAGE_BYTES = 2 * GW_A_BYTES + 2 * GW_B_BYTES;  // 64 KB
-constexpr int GW_STAGES = 3;
-constexpr int GW_THREADS = 256 + 32;  // two consumer warpgroups + the TMA producer warp
-constexpr size_t GW_SMEM = GW_STAGES * GW_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int GW_STAGES = 2;
+// staging pitch in floats: 136 = 8 (mod 32) puts the 4 rows of a half-warp's 8-byte fragment stores on disjoint banks
+constexpr int GW_PITCH = GW_N + 8;
+constexpr int GW_STG_BYTES = GW_M * GW_PITCH * 4;  // 68 KB
+constexpr int GW_RB = 8;  // epilogue rows per warp whose residual loads are in flight together
+constexpr int GW_EW = 4;  // epilogue warps
+constexpr int GW_THREADS = 512;  // two consumer warpgroups, the epilogue warpgroup, the producer warpgroup (one thread works)
+constexpr size_t GW_SMEM = GW_STAGES * GW_STAGE_BYTES + GW_STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 
 struct GemmProblem {
   const float* resid;  // [M][ldr] fp32 or null, added after bias / scale
   float* C;            // optional fp32 output, row-major [M][ldc]
   __half *Ch, *Cl;     // optional split output planes
   int M, N, ldc;
-  int vec4;      // outputs / residual may be accessed in pairs (8-byte fp32, 4-byte plane accesses; host checks 16-byte alignment)
+  int vec4;      // outputs / residual may be accessed 4 columns at a time (host checks 16-byte alignment of bases and lds)
   int tiles_n;   // ceil(N / 128)
   int tile_end;  // running total of tiles up to and including this problem
 };
@@ -57,14 +78,19 @@ static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_c
   const uint32_t raw = tc::smem_u32(gw_raw);
   const uint32_t smem0 = (raw + 1023u) & ~1023u;
   unsigned char* sm = gw_raw + (smem0 - raw);
-  uint64_t* full = reinterpret_cast<uint64_t*>(sm + GW_STAGES * GW_STAGE_BYTES);
+  float* stg = reinterpret_cast<float*>(sm + GW_STAGES * GW_STAGE_BYTES);
+  uint64_t* full = reinterpret_cast<uint64_t*>(sm + GW_STAGES * GW_STAGE_BYTES + GW_STG_BYTES);
   uint64_t* empty = full + GW_STAGES;  // one arrival per consumer warp
+  uint64_t* sfull = empty + GW_STAGES;  // staging tile written: every consumer thread arrives
+  uint64_t* sempty = sfull + 1;         // staging tile read: every epilogue thread arrives
 
   const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
   const int nk = (g.K1 + g.K2) / GW_K;
 
   if (t == 0) {
     for (int s = 0; s < GW_STAGES; ++s) tc::mbar_init(&full[s], 1), tc::mbar_init(&empty[s], 8);
+    tc::mbar_init(sfull, 256);
+    tc::mbar_init(sempty, 32 * GW_EW);
     tc::fence_mbar_init();
     tc::tma_prefetch_desc(&maps.bh[0]);
     tc::tma_prefetch_desc(&maps.bl[0]);
@@ -81,8 +107,9 @@ static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_c
     m0 = mt * GW_M;
   };
 
-  if (warp == 8) {
-    if (lane == 0) {
+  if (warp >= 12) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    if (warp == 12 && lane == 0) {
       // ===== TMA producer =====
       int gk = 0;
       for (int tile = blockIdx.x; tile < g.tiles; tile += gridDim.x) {
@@ -106,17 +133,14 @@ static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_c
         }
       }
     }
-  } else {
+  } else if (warp < 8) {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 184;\n" ::: "memory");
     // ===== consumer warpgroup wg: rows 64 wg .. 64 wg + 63 of every tile =====
     const int wg = warp >> 2;
     const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // fragment rows r0, r0 + 8
     const int c2 = (lane & 3) * 2;                           // fragment columns 8j + c2, + 1
-    const float scale = g.scale;
-    const int relu = g.relu;
-    int gk = 0;
-    for (int tile = blockIdx.x; tile < g.tiles; tile += gridDim.x) {
-      int z, m0, n0;
-      decode(tile, z, m0, n0);
+    int gk = 0, it = 0;
+    for (int tile = blockIdx.x; tile < g.tiles; tile += gridDim.x, ++it) {
       float acc0[64], acc1[64];
       for (int kc = 0; kc < nk; ++kc, ++gk) {
         const int s = gk % GW_STAGES;
@@ -142,74 +166,107 @@ static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_c
       tc::wg_wait<0>();
       if (lane == 0) tc::mbar_arrive(&empty[(gk - 1) % GW_STAGES]);
 
-      // ===== epilogue from the accumulator fragment =====
-      const GemmProblem& pb = g.p[z];
-      const int M = pb.M, N = pb.N;
+      // ===== hand the combined accumulators to the epilogue warps =====
+      if (it > 0) ok = tc::mbar_wait(sempty, (it - 1) & 1) && ok;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int n = n0 + 8 * j + c2;  // first of this thread's 2 columns
-        if (n >= N) continue;
-        const bool pair = n + 1 < N;
-        const bool vec = pb.vec4 && pair;  // 8-byte fp32 and 4-byte plane accesses allowed
-        float b2[2] = {0.f, 0.f};
-        if (g.bias) {
-          b2[0] = __ldg(g.bias + n);
-          if (pair) b2[1] = __ldg(g.bias + n + 1);
-        }
-        const size_t hm_col = (size_t)(n >> 6) * M * 64 + (n & 63);  // head-major: [N / 64][M][64]
+      for (int j = 0; j < 16; ++j)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const int row = m0 + r0 + 8 * h;
-          if (row >= M) continue;
-          float v[2];
+          const int i = 4 * j + 2 * h;
+          *reinterpret_cast<float2*>(stg + (r0 + 8 * h) * GW_PITCH + 8 * j + c2) =
+              make_float2(fmaf(acc1[i], tc::LO_INV, acc0[i]), fmaf(acc1[i + 1], tc::LO_INV, acc0[i + 1]));
+        }
+      tc::mbar_arrive(sfull);
+    }
+  } else {
+    // ===== epilogue: warp 8 + ew takes rows ew, ew + 4, ...; lane takes columns 4 lane .. 4 lane + 3 =====
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 104;\n" ::: "memory");
+    const int ew = warp - 8;
+    const int c = 4 * lane;
+    const float scale = g.scale;
+    const int relu = g.relu, hm = g.head_major, lo_unscaled = g.lo_unscaled, ldr = g.ldr, ldch = g.ldch;
+    int it = 0;
+    for (int tile = blockIdx.x; tile < g.tiles; tile += gridDim.x, ++it) {
+      int z, m0, n0;
+      decode(tile, z, m0, n0);
+      const GemmProblem& pb = g.p[z];
+      const float* resid = pb.resid;
+      float* C = pb.C;
+      __half *Ch = pb.Ch, *Cl = pb.Cl;
+      const int M = pb.M, ldc = pb.ldc;
+      const int n = n0 + c;
+      const int ncols = min(4, pb.N - n);  // this thread's valid columns (<= 0 past the end)
+      const bool vec = pb.vec4 && ncols == 4;
+      const int rows = min(GW_M, M - m0);
+      float b4[4] = {0.f, 0.f, 0.f, 0.f};
+      if (g.bias)
 #pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int i = 4 * j + 2 * h + e;
-            v[e] = (fmaf(acc1[i], tc::LO_INV, acc0[i]) + b2[e]) * scale;
-            if (relu) v[e] = fmaxf(v[e], 0.f);
-          }
-          if (pb.resid) {
-            const float* rp = pb.resid + (size_t)row * g.ldr + n;
-            if (vec) {
-              const float2 rr = *reinterpret_cast<const float2*>(rp);
-              v[0] += rr.x, v[1] += rr.y;
-            } else {
-              v[0] += rp[0];
-              if (pair) v[1] += rp[1];
+        for (int e = 0; e < 4; ++e)
+          if (e < ncols) b4[e] = __ldg(g.bias + n + e);
+      const size_t hm_col = (size_t)(n >> 6) * M * 64 + (n & 63);  // head-major: [N / 64][M][64] (4 columns stay in one head)
+      // Rows go in batches of GW_RB per warp with the batch's residual loads issued together (the first batch's before the
+      // staging wait), so the residual's DRAM latency is paid once per batch rather than once per row.  In-place use
+      // (resid == C) stays safe: every element is read and then written by this thread alone.
+      const bool vres = resid && vec;
+      float4 rr[GW_RB];
+      auto load_resid = [&](int rb) {
+#pragma unroll
+        for (int i = 0; i < GW_RB; ++i)
+          if (rb + GW_EW * i < rows) rr[i] = *reinterpret_cast<const float4*>(resid + (size_t)(m0 + rb + GW_EW * i) * ldr + n);
+      };
+      if (vres) load_resid(ew);
+      ok = tc::mbar_wait(sfull, it & 1) && ok;
+      if (ncols > 0) {
+        for (int rb = ew; rb < rows; rb += GW_EW * GW_RB) {
+          if (vres && rb != ew) load_resid(rb);
+#pragma unroll
+          for (int i = 0; i < GW_RB; ++i) {
+            const int r = rb + GW_EW * i;
+            if (r >= rows) break;
+            const int row = m0 + r;
+            const float4 a = *reinterpret_cast<const float4*>(stg + r * GW_PITCH + c);
+            float v[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              v[e] = (v[e] + b4[e]) * scale;
+              if (relu) v[e] = fmaxf(v[e], 0.f);
             }
-          }
-          const size_t off_c = g.head_major ? hm_col + (size_t)row * 64 : (size_t)row * pb.ldc + n;
-          const size_t off_s = g.head_major ? hm_col + (size_t)row * 64 : (size_t)row * g.ldch + n;
-          if (pb.C) {
+            const size_t off_c = hm ? hm_col + (size_t)row * 64 : (size_t)row * ldc + n;
+            const size_t off_s = hm ? hm_col + (size_t)row * 64 : (size_t)row * ldch + n;
             if (vec) {
-              *reinterpret_cast<float2*>(pb.C + off_c) = make_float2(v[0], v[1]);
-            } else {
-              pb.C[off_c] = v[0];
-              if (pair) pb.C[off_c + 1] = v[1];
-            }
-          }
-          if (pb.Ch) {
-            if (vec) {
-              uint32_t h01, l01;
-              if (g.lo_unscaled) tc::split2_unscaled_clamped(v[0], v[1], h01, l01);
-              else tc::split2(v[0], v[1], h01, l01);
-              *reinterpret_cast<uint32_t*>(pb.Ch + off_s) = h01;
-              *reinterpret_cast<uint32_t*>(pb.Cl + off_s) = l01;
+              if (resid) v[0] += rr[i].x, v[1] += rr[i].y, v[2] += rr[i].z, v[3] += rr[i].w;
+              if (C) *reinterpret_cast<float4*>(C + off_c) = make_float4(v[0], v[1], v[2], v[3]);
+              if (Ch) {
+                uint32_t h01, l01, h23, l23;
+                if (lo_unscaled) {
+                  tc::split2_unscaled_clamped(v[0], v[1], h01, l01);
+                  tc::split2_unscaled_clamped(v[2], v[3], h23, l23);
+                } else {
+                  tc::split2(v[0], v[1], h01, l01);
+                  tc::split2(v[2], v[3], h23, l23);
+                }
+                *reinterpret_cast<uint2*>(Ch + off_s) = make_uint2(h01, h23);
+                *reinterpret_cast<uint2*>(Cl + off_s) = make_uint2(l01, l23);
+              }
             } else {
 #pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                if (e == 0 || pair) {
+              for (int e = 0; e < 4; ++e) {
+                if (e >= ncols) break;
+                if (resid) v[e] += resid[(size_t)row * ldr + n + e];
+                if (C) C[off_c + e] = v[e];
+                if (Ch) {
                   __half hh, ll;
-                  if (g.lo_unscaled) tc::split_h_unscaled(v[e], hh, ll);
+                  if (lo_unscaled) tc::split_h_unscaled(v[e], hh, ll);
                   else tc::split_h(v[e], hh, ll);
-                  pb.Ch[off_s + e] = hh;
-                  pb.Cl[off_s + e] = ll;
+                  Ch[off_s + e] = hh;
+                  Cl[off_s + e] = ll;
                 }
               }
             }
           }
         }
       }
+      tc::mbar_arrive(sempty);
     }
   }
   if (!ok && g.err_flag) *g.err_flag = 1;
