@@ -26,6 +26,14 @@ class LightGluePair(C.Structure):
                 ("out_matches", C.c_void_p), ("out_scores", C.c_void_p), ("out_k", C.c_int), ("out_stop_layer", C.c_int)]
 
 
+class MnnPair(C.Structure):
+    _fields_ = [("desc0", C.c_void_p), ("n0", C.c_int), ("desc1", C.c_void_p), ("n1", C.c_int), ("out_matches", C.c_void_p),
+                ("out_dist", C.c_void_p), ("out_k", C.c_int)]
+
+
+MNN_ERR_RATIO = -4  # b2_mnn_*: ratio test with fewer than 2 descriptors on one side
+
+
 class RansacParams(C.Structure):
     _fields_ = [("threshold", C.c_double), ("confidence", C.c_double), ("max_iters", C.c_int), ("seed", C.c_uint64)]
 
@@ -72,6 +80,8 @@ SIGNATURES = {
     "b2_ransac_fundamental_host": (_i, [_vp, _vp, _vp, _i, C.POINTER(RansacParams), _vp, _vp, _ip]),
     "b2_ransac_essential_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, C.POINTER(RansacParams), _vp, _vp, _ip, _vp, _vp, _vp]),
     "b2_recover_pose_host": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _ip]),
+    "b2_mnn_match_batched_dev": (_i, [_vp, C.POINTER(MnnPair), _i, _i, _i, C.c_double, _vp]),
+    "b2_mnn_match_host": (_i, [_vp, _vp, _i, _vp, _i, _i, _i, C.c_double, _vp, _vp, _ip]),
 }
 
 

@@ -35,6 +35,7 @@ extern "C" void b2_destroy(b2_context* ctx) {
   rs_destroy(ctx);
   rt_destroy(ctx);
   nv_destroy(ctx);
+  mn_destroy(ctx);
   for (auto& b : ctx->stage_d) b.release();
   for (auto& b : ctx->stage_h) b.release();
   for (auto& e : ctx->fcache) e.buf.release();

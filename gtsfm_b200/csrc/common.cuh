@@ -17,6 +17,7 @@
 #define B2_ERR_CUDA -1
 #define B2_ERR_ARG -2
 #define B2_ERR_STATE -3
+#define B2_ERR_MNN_RATIO -4  // ratio test requested with fewer than 2 descriptors on one side (include/gtsfm_b200.h)
 
 struct DevBuf {  // grow-only device allocation
   void* p = nullptr;
@@ -84,6 +85,7 @@ struct SuperGlueState;
 struct RansacState;
 struct RetrievalState;
 struct NetVladState;
+struct MnnState;
 
 // Device copies of host feature arrays handed to the *_host matcher entry points.  GTSfM matches one image's (keypoints,
 // descriptors) against ~20-40 partners, always passing the same host arrays, so re-uploading 5 MB per image per pair is
@@ -118,6 +120,7 @@ struct b2_context {
   RansacState* rs = nullptr;
   RetrievalState* rt = nullptr;
   NetVladState* nv = nullptr;
+  MnnState* mn = nullptr;
   // staging shared by the *_host entry points
   DevBuf stage_d[8];
   HostBuf stage_h[4];
@@ -181,6 +184,7 @@ void sg_destroy(b2_context* ctx);
 void rs_destroy(b2_context* ctx);
 void rt_destroy(b2_context* ctx);
 void nv_destroy(b2_context* ctx);
+void mn_destroy(b2_context* ctx);
 
 // shared device helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

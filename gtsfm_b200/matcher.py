@@ -1,13 +1,15 @@
-"""LightGlue / SuperGlue matcher plugins.
+"""LightGlue / SuperGlue / two-way matcher plugins.
 
-Drop-ins for gtsfm/frontend/matcher/lightglue_matcher.py:24-112 (`LightGlueMatcher`) and
-gtsfm/frontend/matcher/superglue_matcher.py:30-115 (`SuperGlueMatcher`): same `match(...)` signature, argument
-meaning, errors and output dtypes ((K, 2) int64 for LightGlue, uint32 for SuperGlue, rows ascending in column 0).
+Drop-ins for gtsfm/frontend/matcher/lightglue_matcher.py:24-112 (`LightGlueMatcher`),
+gtsfm/frontend/matcher/superglue_matcher.py:30-115 (`SuperGlueMatcher`) and gtsfm/frontend/matcher/twoway_matcher.py
+(`TwoWayMatcher`): same `match(...)` signature, argument meaning, errors and output dtypes ((K, 2) int64 for LightGlue,
+uint32 for SuperGlue, rows ascending in column 0; uint32 rows ordered by distance for the two-way matcher).
 All arithmetic runs in libgtsfm_b200.so; lazily created device state keeps the objects picklable
 (tests/frontend/matcher/test_matcher_base.py:102-107).
 """
 from __future__ import annotations
 
+from enum import Enum
 from pathlib import Path
 from typing import Optional, Tuple, Union
 
@@ -178,3 +180,112 @@ class B200SuperGlueMatcher(MatcherBase):
         eng = self._ensure_engine()
         return eng.match(keypoints_i1.coordinates, keypoints_i1.responses, descriptors_i1, keypoints_i2.coordinates,
                          keypoints_i2.responses, descriptors_i2, im_shape_i1, im_shape_i2, self._config["sinkhorn_iterations"])
+
+
+class MatchingDistanceType(Enum):
+    """gtsfm/frontend/matcher/twoway_matcher.py:17-21."""
+
+    HAMMING = 1
+    EUCLIDEAN = 2
+
+
+class TwoWayEngine:
+    """Mutual-nearest-neighbour matching on k_mnn_top2 (csrc/mnn.cu).  `ratio=None`: no ratio test."""
+
+    def __init__(self, device: int = 0, ctx: Optional[_lib.Context] = None):
+        self.ctx = ctx or _lib.Context(device)
+
+    def _check(self, rc: int, what: str) -> None:
+        if rc == _lib.MNN_ERR_RATIO:
+            raise ValueError("the ratio test needs at least 2 descriptors per image (cv2 knnMatch(k=2) found one neighbour)")
+        self.ctx.check(rc, what)
+
+    def match(self, desc0: np.ndarray, desc1: np.ndarray, ratio: Optional[float] = None, return_dist: bool = False):
+        """Host arrays (float32 or uint8, no NaN) -> (K, 2) int64 rows (i0, i1) ordered by (0 -> 1 distance, i0)."""
+        dt = 1 if desc0.dtype == np.uint8 and desc1.dtype == np.uint8 else 0
+        npd = np.uint8 if dt else np.float32
+        d0, d1 = np.ascontiguousarray(desc0, npd), np.ascontiguousarray(desc1, npd)
+        dim = d0.shape[1] if d0.ndim == 2 else d1.shape[1]
+        n0, n1 = len(d0), len(d1)
+        cap = max(1, min(n0, n1))
+        out = np.empty((cap, 2), np.int64)
+        dist = np.empty(cap, np.float32)
+        k = _lib.C.c_int(0)
+        rc = self.ctx.lib.b2_mnn_match_host(self.ctx.handle, _lib.ptr(d0), n0, _lib.ptr(d1), n1, int(dim), dt,
+                                            -1.0 if ratio is None else float(ratio), _lib.ptr(out), _lib.ptr(dist), _lib.C.byref(k))
+        self._check(rc, "mnn_match_host")
+        if return_dist:
+            return out[: k.value].copy(), dist[: k.value].copy()
+        return out[: k.value].copy()
+
+    def match_batched_dev(self, pairs, ratio: Optional[float] = None, return_dist: bool = False):
+        """pairs: sequence of (desc0, desc1) CUDA tensors (float32 or uint8, [n][dim]).  -> list of device int64 (K, 2) tensors
+        (and float32 distances), one library call per (dim, dtype) group of pairs."""
+        import torch
+
+        groups = {}
+        for i, (a, b) in enumerate(pairs):
+            dim = a.shape[1] if a.dim() == 2 else b.shape[1]
+            dt = 1 if a.dtype == torch.uint8 and b.dtype == torch.uint8 else 0
+            groups.setdefault((int(dim), dt), []).append(i)
+        res = [None] * len(pairs)
+        for (dim, dt), idx in groups.items():
+            tdt = torch.uint8 if dt else torch.float32
+            ins, outs, st = [], [], (_lib.MnnPair * len(idx))()
+            for s, i in enumerate(idx):
+                a, b = (x.to(tdt).reshape(-1, dim).contiguous() for x in pairs[i])
+                cap = max(1, min(len(a), len(b)))
+                m = torch.empty((cap, 2), dtype=torch.int64, device=a.device)
+                d = torch.empty(cap, dtype=torch.float32, device=a.device)
+                ins.append((a, b))
+                outs.append((m, d))
+                st[s] = _lib.MnnPair(a.data_ptr(), len(a), b.data_ptr(), len(b), m.data_ptr(), d.data_ptr(), 0)
+            stream = torch.cuda.current_stream(ins[0][0].device).cuda_stream
+            rc = self.ctx.lib.b2_mnn_match_batched_dev(self.ctx.handle, st, len(idx), dim, dt,
+                                                       -1.0 if ratio is None else float(ratio), _lib.C.c_void_p(stream))
+            self._check(rc, "mnn_match_batched_dev")
+            for s, i in enumerate(idx):
+                m, d = outs[s]
+                kk = st[s].out_k
+                res[i] = (m[:kk], d[:kk]) if return_dist else m[:kk]
+        return res
+
+
+class B200TwoWayMatcher(MatcherBase):
+    """Drop-in for gtsfm/frontend/matcher/twoway_matcher.py (`TwoWayMatcher`): mutual nearest neighbours under cv2's L2
+    distance with an optional ratio test, on hand-written sm_90a kernels.  Integer-valued descriptors of dimension <= 258
+    (cv2 SIFT, ORB, BRISK) give cv2's indices, order and distances bit for bit; other float descriptors can differ from cv2
+    on near-ties."""
+
+    def __init__(self, distance_type: MatchingDistanceType = MatchingDistanceType.EUCLIDEAN, ratio_test_threshold: Optional[float] = None,
+                 device: int = 0):
+        super().__init__()
+        if distance_type is not MatchingDistanceType.EUCLIDEAN:
+            raise NotImplementedError("B200TwoWayMatcher implements the EUCLIDEAN distance only")
+        self._distance_type = distance_type
+        self._ratio_test_threshold = ratio_test_threshold
+        self._device = device
+        self._engine: Optional[TwoWayEngine] = None
+
+    def __getstate__(self):
+        st = dict(self.__dict__)
+        st["_engine"] = None
+        return st
+
+    def _ensure_engine(self) -> TwoWayEngine:
+        if self._engine is None:
+            self._engine = TwoWayEngine(self._device)
+        return self._engine
+
+    def match(self, keypoints_i1: Keypoints, keypoints_i2: Keypoints, descriptors_i1: np.ndarray, descriptors_i2: np.ndarray,
+              im_shape_i1: Tuple[int, int, int], im_shape_i2: Tuple[int, int, int]) -> np.ndarray:
+        if descriptors_i1.size == 0 or descriptors_i2.size == 0:
+            return np.array([])  # the reference's return value (twoway_matcher.py:72-73)
+        v1 = np.nonzero(~np.isnan(descriptors_i1).any(axis=1))[0]
+        v2 = np.nonzero(~np.isnan(descriptors_i2).any(axis=1))[0]
+        if len(v1) == 0 or len(v2) == 0:
+            return np.array([])
+        m = self._ensure_engine().match(descriptors_i1[v1], descriptors_i2[v2], self._ratio_test_threshold)
+        if len(m) == 0:
+            return np.array([])
+        return np.stack([v1[m[:, 0]], v2[m[:, 1]]], 1).astype(np.uint32)

@@ -44,7 +44,7 @@ uint64_t b2_launch_count(const b2_context* ctx);
 /* Host-to-device bytes actually copied so far by the entry points that keep device copies of their host inputs
  * (b2_lightglue_match_host: feature arrays already uploaded for an earlier pair are not sent again). */
 uint64_t b2_h2d_bytes(const b2_context* ctx);
-/* Tuning knobs.  "reserve_sms" = n: the persistent kernels (attention, GEMM) launch sm_count - n CTAs, leaving n SMs to
+/* Tuning knobs.  "reserve_sms" = n: the persistent kernels (attention, GEMM, two-way matcher) launch sm_count - n CTAs, leaving n SMs to
  * kernels of OTHER contexts / streams running concurrently (the batched front-end overlaps pair k's RANSAC with pair
  * k+1's matching; a one-CTA-per-SM kernel that finds an SM busy would otherwise wait for a whole CTA lifetime).
  * "lightglue_batch" = 0..8: pairs per lock-step batch of b2_lightglue_match_batched_dev (0 = 8, the maximum).
@@ -237,6 +237,33 @@ int b2_netvlad_describe_host(b2_context* ctx, const float* images, int batch, in
  * (Descriptors: b2_netvlad_describe_* above, or any other unit-norm global descriptor.) */
 int b2_similarity_pairs_host(b2_context* ctx, const float* desc, int n, int dim, int num_matched, float min_score,
                              int32_t* out_partners, float* out_sim);
+
+/* ---- two-way (mutual nearest neighbour) descriptor matcher (gtsfm/frontend/matcher/twoway_matcher.py) -------------------- */
+/* cv2.BFMatcher(NORM_L2) in both directions (knnMatch k = 2 with the ratio test `d1 <= ratio * d2` compared in double, or
+ * match without it), mutual check, rows ordered by (0 -> 1 distance, i0).  Descriptors are [n][dim] row-major, dtype 0 =
+ * float32, 1 = uint8; 1 <= dim <= 32768, n <= 32768 per image.  uint8 input, and float32 input whose values are all integers
+ * in [0, 255] with dim <= 258, is matched in exact integer arithmetic (|a|^2 + |b|^2 - 2 a.b in int32, then sqrtf).  cv2 sums
+ * (a - b)^2 in float for both types, exactly while dim * 255^2 < 2^24, so for dim <= 258 (cv2 SIFT, ORB, BRISK) indices,
+ * order and distances equal cv2's bit for bit; for uint8 with a larger dim cv2's distances may differ in the last bits.
+ * Other float32 input uses split-fp16 products; d^2 = |a|^2 + |b|^2 - 2 a.b cancels for near-duplicate rows, so distances and
+ * the resolution of near-ties can differ from cv2's.  The choice is made per pair from the data.  ratio < 0: no ratio test
+ * (the reference's None).  With a ratio test, a pair with a non-empty side of fewer than 2 rows fails with -4 (cv2's
+ * knnMatch returns one neighbour there).
+ * Nothing proportional to n0 * n1 is allocated. */
+typedef struct b2_mnn_pair {
+  const void* desc0; /* DEVICE [n0][dim] */
+  int n0;
+  const void* desc1; /* DEVICE [n1][dim] */
+  int n1;
+  int64_t* out_matches; /* DEVICE [min(n0, n1)][2] rows (i0, i1) */
+  float* out_dist;      /* DEVICE [min(n0, n1)] cv2 DMatch.distance of the 0 -> 1 match, or NULL */
+  int out_k;            /* written on the HOST struct: number of matches */
+} b2_mnn_pair;
+/* All pairs of a batch share dim and dtype; one synchronisation of `stream` at the end. */
+int b2_mnn_match_batched_dev(b2_context* ctx, b2_mnn_pair* pairs, int n_pairs, int dim, int dtype, double ratio, void* stream);
+/* HOST pointers (float32 integer-valued input is sent as uint8); out_matches [min(n0,n1)][2], out_dist may be NULL. */
+int b2_mnn_match_host(b2_context* ctx, const void* desc0, int n0, const void* desc1, int n1, int dim, int dtype, double ratio,
+                      int64_t* out_matches, float* out_dist, int* out_k);
 
 #ifdef __cplusplus
 }
