@@ -34,6 +34,24 @@ class MnnPair(C.Structure):
 MNN_ERR_RATIO = -4  # b2_mnn_*: ratio test with fewer than 2 descriptors on one side
 
 
+class SiftKeypoint(C.Structure):
+    _fields_ = [("x", C.c_float), ("y", C.c_float), ("size", C.c_float), ("angle", C.c_float), ("response", C.c_float),
+                ("octave", C.c_int32)]
+
+
+# numpy twin of b2_sift_keypoint (24 bytes, the fields of cv2.KeyPoint)
+SIFT_KEYPOINT_DTYPE = np.dtype([("x", np.float32), ("y", np.float32), ("size", np.float32), ("angle", np.float32),
+                                ("response", np.float32), ("octave", np.int32)])
+
+
+class SiftImage(C.Structure):
+    _fields_ = [("image", C.c_void_p), ("mask", C.c_void_p), ("max_keypoints", C.c_int), ("out_keypoints", C.c_void_p),
+                ("out_desc", C.c_void_p), ("out_n", C.c_int), ("out_total", C.c_int)]
+
+
+SIFT_CAPACITY = -5  # b2_sift_detect_host: more keypoints than the capacity; *out_n holds the count needed
+
+
 class RansacParams(C.Structure):
     _fields_ = [("threshold", C.c_double), ("confidence", C.c_double), ("max_iters", C.c_int), ("seed", C.c_uint64)]
 
@@ -82,6 +100,8 @@ SIGNATURES = {
     "b2_recover_pose_host": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _ip]),
     "b2_mnn_match_batched_dev": (_i, [_vp, C.POINTER(MnnPair), _i, _i, _i, C.c_double, _vp]),
     "b2_mnn_match_host": (_i, [_vp, _vp, _i, _vp, _i, _i, _i, C.c_double, _vp, _vp, _ip]),
+    "b2_sift_detect_batched_dev": (_i, [_vp, C.POINTER(SiftImage), _i, _i, _i, _i, _sz, _vp]),
+    "b2_sift_detect_host": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _ip]),
 }
 
 

@@ -36,6 +36,7 @@ extern "C" void b2_destroy(b2_context* ctx) {
   rt_destroy(ctx);
   nv_destroy(ctx);
   mn_destroy(ctx);
+  sf_destroy(ctx);
   for (auto& b : ctx->stage_d) b.release();
   for (auto& b : ctx->stage_h) b.release();
   for (auto& e : ctx->fcache) e.buf.release();

@@ -18,6 +18,7 @@
 #define B2_ERR_ARG -2
 #define B2_ERR_STATE -3
 #define B2_ERR_MNN_RATIO -4  // ratio test requested with fewer than 2 descriptors on one side (include/gtsfm_b200.h)
+#define B2_SIFT_CAPACITY -5  // b2_sift_detect_host: more keypoints than the caller's capacity, *out_n = the count needed
 
 struct DevBuf {  // grow-only device allocation
   void* p = nullptr;
@@ -86,6 +87,7 @@ struct RansacState;
 struct RetrievalState;
 struct NetVladState;
 struct MnnState;
+struct SiftState;
 
 // Device copies of host feature arrays handed to the *_host matcher entry points.  GTSfM matches one image's (keypoints,
 // descriptors) against ~20-40 partners, always passing the same host arrays, so re-uploading 5 MB per image per pair is
@@ -121,6 +123,7 @@ struct b2_context {
   RetrievalState* rt = nullptr;
   NetVladState* nv = nullptr;
   MnnState* mn = nullptr;
+  SiftState* sf = nullptr;
   // staging shared by the *_host entry points
   DevBuf stage_d[8];
   HostBuf stage_h[4];
@@ -185,6 +188,7 @@ void rs_destroy(b2_context* ctx);
 void rt_destroy(b2_context* ctx);
 void nv_destroy(b2_context* ctx);
 void mn_destroy(b2_context* ctx);
+void sf_destroy(b2_context* ctx);
 
 // shared device helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

@@ -13,7 +13,9 @@
 
 #include "common.cuh"
 #include "conv_ps.cuh"
+#include "image.cuh"
 #include "linear.cuh"
+#include "topk.cuh"
 
 namespace {
 
@@ -81,21 +83,13 @@ void sp_destroy(b2_context* ctx) {
 // kernels
 // ------------------------------------------------------------------------------------------------------------------
 
-// cv2 COLOR_RGB2GRAY / COLOR_RGBA2GRAY for 8-bit: (9798 R + 19235 G + 3735 B + 2^14) >> 15   (utils/images.py:36-38)
+// cv2 COLOR_RGB2GRAY / COLOR_RGBA2GRAY (image.cuh)
 __global__ void k_to_gray(const uint8_t* __restrict__ img, size_t pitch, int channels, int H, int W,
                           uint8_t* __restrict__ gray) {
   int x = blockIdx.x * blockDim.x + threadIdx.x;
   int y = blockIdx.y;
   if (x >= W) return;
-  const uint8_t* p = img + (size_t)y * pitch + (size_t)x * channels;
-  uint8_t g;
-  if (channels == 1) {
-    g = p[0];
-  } else {
-    int v = 9798 * (int)p[0] + 19235 * (int)p[1] + 3735 * (int)p[2] + (1 << 14);
-    g = (uint8_t)(v >> 15);
-  }
-  gray[(size_t)y * W + x] = g;
+  gray[(size_t)y * W + x] = b2_gray_u8(img + (size_t)y * pitch + (size_t)x * channels, channels);
 }
 
 // conv1a: 1 -> 64 channels, 3x3, pad 1, bias, ReLU; input gray u8 / 255 (gtsfm/.../superpoint.py:74).
@@ -1034,92 +1028,12 @@ extern "C" int b2_superpoint_describe_host(b2_context* ctx, uint64_t map_token, 
 
 // ------------------------------------------------------------------------------------------------------------------
 // device top-k for the batched path: the k largest scores (ties at the k-th value -> lowest indices), kept in their
-// original (row-major) order.  4-pass 8-bit radix select on the float bit patterns (scores are positive), then an
-// ordered compaction.  Single CTA: n is a few 10^4.
+// original (row-major) order (topk.cuh).  Single CTA: n is a few 10^4.
 // ------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) k_topk_select(const float* __restrict__ score, int n, const int* __restrict__ n_dev, int k,
                                                        int* __restrict__ out_idx, int* __restrict__ out_count) {
   if (n_dev) n = min(n, *n_dev);  // candidate count still on the device (single-sync extract): n is then the capacity bound
-  __shared__ unsigned hist[256];
-  __shared__ unsigned prefix, need;
-  __shared__ int wtot[32];
-  __shared__ int carry, eq_carry;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (k >= n) {
-    for (int i = threadIdx.x; i < n; i += 1024) out_idx[i] = i;
-    if (threadIdx.x == 0) *out_count = n;
-    return;
-  }
-  if (threadIdx.x == 0) prefix = 0, need = (unsigned)k;
-  __syncthreads();
-  for (int pass = 0; pass < 4; ++pass) {
-    const int shift = 24 - 8 * pass;
-    const unsigned himask = pass == 0 ? 0u : (0xffffffffu << (shift + 8));
-    for (int i = threadIdx.x; i < 256; i += 1024) hist[i] = 0;
-    __syncthreads();
-    for (int i = threadIdx.x; i < n; i += 1024) {
-      unsigned key = __float_as_uint(score[i]);
-      if ((key & himask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      unsigned acc = 0;
-      int b = 255;
-      for (; b > 0; --b) {
-        if (acc + hist[b] >= need) break;
-        acc += hist[b];
-      }
-      need -= acc;  // how many still have to come from bin b
-      prefix |= ((unsigned)b) << shift;
-    }
-    __syncthreads();
-  }
-  // prefix = bit pattern of the k-th largest score; take everything above it and the first `need` equal to it
-  const unsigned T = prefix;
-  if (threadIdx.x == 0) carry = 0, eq_carry = 0;
-  __syncthreads();
-  for (int base = 0; base < n; base += 1024) {
-    int i = base + threadIdx.x;
-    unsigned key = i < n ? __float_as_uint(score[i]) : 0u;
-    bool gt = i < n && key > T, eq = i < n && key == T;
-    // rank among equals, in index order
-    unsigned em = __ballot_sync(0xffffffffu, eq);
-    if (lane == 0) wtot[warp] = __popc(em);
-    __syncthreads();
-    if (warp == 0) {
-      int w = wtot[lane], ws = w;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        int u = __shfl_up_sync(0xffffffffu, ws, o);
-        if (lane >= o) ws += u;
-      }
-      wtot[lane] = ws - w;
-    }
-    __syncthreads();
-    int eq_rank = eq_carry + wtot[warp] + __popc(em & ((1u << lane) - 1));
-    bool take = gt || (eq && (unsigned)eq_rank < need);
-    __syncthreads();
-    if (threadIdx.x == 1023) eq_carry = eq_rank + (eq ? 1 : 0);
-    unsigned tm = __ballot_sync(0xffffffffu, take);
-    if (lane == 0) wtot[warp] = __popc(tm);
-    __syncthreads();
-    if (warp == 0) {
-      int w = wtot[lane], ws = w;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        int u = __shfl_up_sync(0xffffffffu, ws, o);
-        if (lane >= o) ws += u;
-      }
-      wtot[lane] = ws - w;
-    }
-    __syncthreads();
-    int pos = carry + wtot[warp] + __popc(tm & ((1u << lane) - 1));
-    if (take) out_idx[pos] = i;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry = pos + (take ? 1 : 0);
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *out_count = carry;
+  b2_topk_select_cta(score, n, k, out_idx, out_count);
 }
 
 extern "C" int b2_topk_indices_dev(b2_context* ctx, const float* scores, int n, int k, int32_t* out_idx, int* out_k,

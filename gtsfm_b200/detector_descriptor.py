@@ -1,4 +1,4 @@
-"""SuperPoint detector-descriptor plugin.
+"""SuperPoint and SIFT detector-descriptor plugins.
 
 Drop-in for gtsfm/frontend/detector_descriptor/superpoint.py:32-93 (`SuperPointDetectorDescriptor`): same constructor
 arguments, same `detect_and_describe(image) -> (Keypoints, (N, 256) float32)` contract, same post-processing order
@@ -9,6 +9,10 @@ All arithmetic runs in libgtsfm_b200.so (CUDA, sm_90a); this file only moves num
 deliberate difference from the reference data flow: descriptors are sampled on the GPU only for the keypoints that
 survive the host-side mask / top-k selection, instead of for every detection (identical values, 3x less D2H at 5000 of
 17000 keypoints).
+
+`B200SIFTDetectorDescriptor` is the drop-in for gtsfm/frontend/detector_descriptor/sift.py:24-55 (`SIFTDetectorDescriptor`):
+cv2.SIFT_create() with its defaults, restated in csrc/sift.cu.  Its one deliberate difference: an image without keypoints
+gives (empty Keypoints, (0, 128) float32) where the reference raises a TypeError.
 """
 from __future__ import annotations
 
@@ -118,3 +122,133 @@ class B200SuperPointDetectorDescriptor(DetectorDescriptorBase):
                 return keypoints, np.zeros((0, DESC_DIM), np.float32)
             descriptors = eng.describe(np.asarray(keypoints.coordinates, np.float32), token)
         return keypoints, descriptors
+
+
+SIFT_DESC_DIM = 128
+SIFT_WORKSPACE_BUDGET = 4 << 30  # bytes of device workspace one batched call may use (csrc/sift.cu: ~151 H W per image)
+
+
+class SiftEngine:
+    """cv2.SIFT_create() defaults on csrc/sift.cu: host calls (every keypoint, as cv2 returns them) and batched device calls
+    (the max_keypoints largest responses, uint8 descriptors left on the GPU for TwoWayEngine.match_batched_dev)."""
+
+    def __init__(self, device: int = 0, ctx: Optional[_lib.Context] = None, capacity: int = 8192):
+        self.ctx = ctx or _lib.Context(device)
+        self.capacity = capacity  # first guess of the host call's output size; grown to the count the library reports
+        self.lock = threading.RLock()
+
+    def detect_and_describe(self, image: np.ndarray, mask: Optional[np.ndarray] = None):
+        """Host uint8 image (H, W) / (H, W, 3) / (H, W, 4) and optional (H, W) mask -> (keypoint records
+        `_lib.SIFT_KEYPOINT_DTYPE`, (N, 128) uint8 descriptors), every keypoint in cv2's order."""
+        img = np.ascontiguousarray(image)
+        if img.dtype != np.uint8:
+            raise ValueError("image must be uint8")
+        if img.ndim == 3 and img.shape[2] not in (3, 4) or img.ndim not in (2, 3):
+            raise ValueError("Input image dimensions are wrong")
+        h, w = img.shape[:2]
+        ch = 1 if img.ndim == 2 else img.shape[2]
+        m = None
+        if mask is not None:
+            if mask.shape[:2] != (h, w):
+                raise ValueError("mask must have the image's height and width")
+            m = np.ascontiguousarray(mask != 0, np.uint8)
+        with self.lock:
+            while True:
+                cap = self.capacity
+                kp = np.empty(cap, _lib.SIFT_KEYPOINT_DTYPE)
+                desc = np.empty((cap, SIFT_DESC_DIM), np.uint8)
+                n = _lib.C.c_int(0)
+                rc = self.ctx.lib.b2_sift_detect_host(self.ctx.handle, _lib.ptr(img), h, w, ch, _lib.ptr(m), _lib.ptr(kp),
+                                                      _lib.ptr(desc), cap, _lib.C.byref(n))
+                if rc == _lib.SIFT_CAPACITY:
+                    self.capacity = n.value
+                    continue
+                self.ctx.check(rc, "sift_detect_host")
+                return kp[: n.value].copy(), desc[: n.value].copy()
+
+    @staticmethod
+    def images_per_call(h: int, w: int) -> int:
+        return int(max(1, min(64, SIFT_WORKSPACE_BUDGET // (151 * h * w))))
+
+    def extract_many(self, images, masks=None, max_keypoints: int = 5000):
+        """images: sequence of same-shape CUDA uint8 tensors (H, W) / (H, W, C), rows may be pitched (stride(0) >= W C, unit
+        inner strides); masks: None or a per-image sequence of CUDA (H, W) uint8 tensors / None.  -> list of (keypoint records
+        as a (n, 6) float32 view [x, y, size, angle, response, octave bits], (n, 128) uint8 descriptors, total before top-k)."""
+        import torch
+
+        if len(images) == 0:
+            return []
+        shape = tuple(images[0].shape)
+        if any(tuple(x.shape) != shape for x in images):
+            raise ValueError("extract_many takes images of one shape")
+        h, w = shape[:2]
+        ch = 1 if len(shape) == 2 else shape[2]
+        masks = [None] * len(images) if masks is None else list(masks)
+        dev = images[0].device
+        per = self.images_per_call(h, w)
+        out = []
+        with self.lock:
+            for c0 in range(0, len(images), per):
+                idx = range(c0, min(len(images), c0 + per))
+                st = (_lib.SiftImage * len(idx))()
+                keep = []
+                pitch = None
+                for s, i in enumerate(idx):
+                    x = images[i]
+                    if x.dtype != torch.uint8:
+                        raise ValueError("images must be uint8")
+                    if x.stride(-1) != 1 or (x.dim() == 3 and x.stride(1) != ch):
+                        x = x.contiguous()
+                    p = x.stride(0)
+                    if pitch is None:
+                        pitch = p
+                    elif p != pitch:
+                        x = x.contiguous()
+                        if x.stride(0) != pitch:
+                            raise ValueError("images of one call must share a row pitch")
+                    m = masks[i]
+                    if m is not None:
+                        m = (m != 0).to(torch.uint8).contiguous()
+                    kp = torch.empty((max_keypoints, 6), dtype=torch.float32, device=dev)
+                    desc = torch.empty((max_keypoints, SIFT_DESC_DIM), dtype=torch.uint8, device=dev)
+                    keep.append((x, m, kp, desc))
+                    st[s] = _lib.SiftImage(x.data_ptr(), 0 if m is None else m.data_ptr(), int(max_keypoints), kp.data_ptr(),
+                                           desc.data_ptr(), 0, 0)
+                stream = torch.cuda.current_stream(dev).cuda_stream
+                rc = self.ctx.lib.b2_sift_detect_batched_dev(self.ctx.handle, st, len(idx), h, w, ch, int(pitch), _lib.C.c_void_p(stream))
+                self.ctx.check(rc, "sift_detect_batched_dev")
+                for s, (_, _, kp, desc) in enumerate(keep):
+                    n = st[s].out_n
+                    out.append((kp[:n], desc[:n], st[s].out_total))
+        return out
+
+
+class B200SIFTDetectorDescriptor(DetectorDescriptorBase):
+    """cv2 SIFT (default parameters) on hand-written sm_90a kernels behind GTSfM's DetectorDescriptorBase."""
+
+    def __init__(self, max_keypoints: int = 5000, device: int = 0) -> None:
+        super().__init__(max_keypoints=max_keypoints)
+        self._device = device
+        self._engine: Optional[SiftEngine] = None  # lazy, never pickled
+
+    def __getstate__(self):
+        st = dict(self.__dict__)
+        st["_engine"] = None
+        return st
+
+    def _ensure_engine(self) -> SiftEngine:
+        if self._engine is None:
+            self._engine = SiftEngine(self._device)
+        return self._engine
+
+    def detect_and_describe(self, image: Image) -> Tuple[Keypoints, np.ndarray]:
+        arr = image.value_array
+        if arr.ndim == 3 and arr.shape[2] not in (3, 4):
+            raise ValueError("Input image dimensions are wrong")  # gtsfm/utils/images.py:39-40
+        kp, desc = self._ensure_engine().detect_and_describe(arr, getattr(image, "mask", None))
+        if len(kp) == 0:
+            return Keypoints(np.zeros((0, 2))), np.zeros((0, SIFT_DESC_DIM), np.float32)
+        keypoints = Keypoints(np.stack([kp["x"], kp["y"]], 1).astype(np.float64), scales=kp["size"].astype(np.float64),
+                              responses=kp["response"].astype(np.float64))
+        keypoints, sel = keypoints.get_top_k(self.max_keypoints)  # gtsfm/.../sift.py:53-54
+        return keypoints, desc[sel].astype(np.float32)

@@ -265,6 +265,36 @@ int b2_mnn_match_batched_dev(b2_context* ctx, b2_mnn_pair* pairs, int n_pairs, i
 int b2_mnn_match_host(b2_context* ctx, const void* desc0, int n0, const void* desc1, int n1, int dim, int dtype, double ratio,
                       int64_t* out_matches, float* out_dist, int* out_k);
 
+/* ---- SIFT detector-descriptor (gtsfm/frontend/detector_descriptor/sift.py) --------------------------------------------------- */
+/* cv2.SIFT_create() with its defaults restated: 3 layers per octave, contrast threshold 0.04, edge threshold 10, sigma 1.6, the
+ * image doubled first (octave -1).  Images are uint8 H x W x {1, 3, 4} interleaved (RGB / RGBA go through cv2's fixed-point
+ * COLOR_RGB2GRAY); H x W <= 2^24 and each side <= 16384, larger input fails with -2.  Keypoints come in cv2's order (x, y
+ * ascending, size descending, angle, response descending, octave descending), consecutive duplicates in (x, y, size, angle)
+ * dropped, then the mask applied as cv2 does (kept where mask[(int)(y + 0.5)][(int)(x + 0.5)] != 0).  Descriptors are 128
+ * uint8 values per keypoint (cv2's float descriptors hold the same integers).  Results do not depend on the batch or the run.
+ * Workspace: about 151 H W bytes per image of a batch (the Gaussian pyramid is 128 H W). */
+typedef struct b2_sift_keypoint { /* the fields of cv2.KeyPoint */
+  float x, y, size, angle, response;
+  int32_t octave;
+} b2_sift_keypoint;
+typedef struct b2_sift_image {
+  const uint8_t* image;             /* DEVICE image, row pitch as passed to the call */
+  const uint8_t* mask;              /* DEVICE H x W uint8, dense, or NULL */
+  int max_keypoints;                /* >= 1: the max_keypoints largest responses (ties to the lower index), cv2's order kept */
+  b2_sift_keypoint* out_keypoints;  /* DEVICE [max_keypoints] */
+  uint8_t* out_desc;                /* DEVICE [max_keypoints][128] */
+  int out_n;                        /* written on the HOST struct: keypoints written */
+  int out_total;                    /* written on the HOST struct: keypoints after the mask, before the top-k */
+} b2_sift_image;
+/* Up to 64 same-shape images: every pyramid and extrema stage is one launch over the batch, counts stay on the device, and
+ * `stream` is synchronised once at the end. */
+int b2_sift_detect_batched_dev(b2_context* ctx, b2_sift_image* images, int n_images, int height, int width, int channels,
+                               size_t pitch, void* stream);
+/* HOST pointers, dense image, optional mask: every keypoint (no top-k).  When there are more than `capacity` keypoints nothing
+ * is written and the call returns -5 with *out_n = the number needed; otherwise *out_n = the number written. */
+int b2_sift_detect_host(b2_context* ctx, const uint8_t* image, int height, int width, int channels, const uint8_t* mask,
+                        b2_sift_keypoint* out_keypoints, uint8_t* out_desc, int capacity, int* out_n);
+
 #ifdef __cplusplus
 }
 #endif

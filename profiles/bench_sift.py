@@ -1,0 +1,166 @@
+"""SIFT detector-descriptor throughput on two workloads: the 12 lund-door frames at loader resolution (1135 x 760 gray) and
+21 seeded 2880 x 3840 RGB synthetic_sequence frames (bench_twoway.py's).
+
+Arms, per workload:
+- images/s of the batched device path (SiftEngine.extract_many, top 5000, images already on the GPU), of the plugin on host
+  arrays (B200SIFTDetectorDescriptor.detect_and_describe) and of the reference's cv2 SIFT (oracle/sift_ref.py) with one
+  single-threaded process per host core;
+- pairs/s of the whole SIFT front end on sequential pairs: device detect -> TwoWayEngine.match_batched_dev at ratio 0.8, against
+  cv2 SIFT on every frame plus cv2 two-way matching of every pair, on every core;
+- device time per stage (CUDA events around the k_sift_* launches), and the bytes the pyramid kernels (k_sift_blur, k_sift_down)
+  must move, computed from the shapes, over their time as a share of the H100 SXM's 3.35 TB/s.
+The card name and power limit are read in the same run.  Writes one JSON line to --out.
+
+    python profiles/bench_sift.py --out profiles/h100_sift.json
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import multiprocessing as mp
+import os
+import subprocess
+import sys
+import time
+from pathlib import Path
+
+import numpy as np
+
+ROOT = Path(__file__).resolve().parent.parent
+sys.path.insert(0, str(ROOT))
+
+HBM_TBS = 3.35  # H100 SXM data sheet
+STAGES = ("k_sift_blur", "k_sift_down", "k_sift_extrema", "k_sift_orient", "k_sift_rank", "k_sift_compact", "k_sift_topk",
+          "k_sift_describe")
+
+
+def pyramid_bytes(h: int, w: int, channels: int) -> int:
+    """Bytes the pyramid kernels must read and write for one image: the uint8 input once, every blurred level read once and
+    written once, every decimated level read (its pixels) and written once."""
+    from oracle.sift_ref import n_octaves
+
+    total, ww, hh = h * w * channels, 2 * w, 2 * h
+    for o in range(n_octaves(h, w)):
+        p = ww * hh * 4
+        total += p * (1 + 2 * 5) + (p if o else 0)  # level 0 written (plus its decimated source read), levels 1..5 read + written
+        ww, hh = ww // 2, hh // 2
+    return total
+
+
+def _cv2_detect(arr):
+    import cv2
+
+    cv2.setNumThreads(1)
+    from oracle import sift_ref
+
+    return sift_ref.detect_and_describe(arr)[3]
+
+
+def _cv2_match(args):
+    import cv2
+
+    cv2.setNumThreads(1)
+    from oracle import twoway_ref
+
+    return len(twoway_ref.twoway_match(args[0], args[1], 0.8)[0])
+
+
+def workload(name, frames, reps, pool, cores, ctx):
+    import torch
+
+    from gtsfm_b200.detector_descriptor import B200SIFTDetectorDescriptor, SiftEngine
+    from gtsfm_b200.gtsfm_api import Image
+    from gtsfm_b200.matcher import TwoWayEngine
+
+    eng, mt = SiftEngine(ctx=ctx), TwoWayEngine(ctx=ctx)
+    dev = [torch.from_numpy(f).cuda() for f in frames]
+    n, npairs = len(frames), len(frames) - 1
+
+    def front_end():
+        out = eng.extract_many(dev, max_keypoints=5000)
+        return out, mt.match_batched_dev([(out[i][1], out[i + 1][1]) for i in range(npairs)], 0.8)
+
+    for _ in range(2):
+        front_end()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(reps):
+        eng.extract_many(dev, max_keypoints=5000)
+    torch.cuda.synchronize()
+    dev_ips = reps * n / (time.perf_counter() - t0)
+    t0 = time.perf_counter()
+    for _ in range(reps):
+        out, res = front_end()
+    torch.cuda.synchronize()
+    dev_pps = reps * npairs / (time.perf_counter() - t0)
+    stage_ms = {}
+    for st in STAGES:
+        ctx.profile_start(st)
+        for _ in range(reps):
+            eng.extract_many(dev, max_keypoints=5000)
+        ms, launches, _ = ctx.profile_stop()
+        stage_ms[st] = round(ms / (reps * n), 4)
+    h, w = frames[0].shape[:2]
+    ch = 1 if frames[0].ndim == 2 else frames[0].shape[2]
+    pyr_s = (stage_ms["k_sift_blur"] + stage_ms["k_sift_down"]) * 1e-3
+    pyr_tbs = pyramid_bytes(h, w, ch) / pyr_s / 1e12
+
+    det = B200SIFTDetectorDescriptor(max_keypoints=5000)
+    det._engine = eng
+    det.detect_and_describe(Image(frames[0]))
+    plug_reps = max(1, reps // 4)
+    t0 = time.perf_counter()
+    for _ in range(plug_reps):
+        for f in frames:
+            det.detect_and_describe(Image(f))
+    plugin_ips = plug_reps * n / (time.perf_counter() - t0)
+
+    pool.map(_cv2_detect, frames[: min(n, cores)])
+    work = frames * max(1, (2 * cores + n - 1) // n)
+    t0 = time.perf_counter()
+    pool.map(_cv2_detect, work, chunksize=1)
+    cv2_ips = len(work) / (time.perf_counter() - t0)
+    t0 = time.perf_counter()
+    desc = pool.map(_cv2_detect, frames, chunksize=1)
+    counts = pool.map(_cv2_match, [(desc[i], desc[i + 1]) for i in range(npairs)], chunksize=1)
+    cv2_pps = npairs / (time.perf_counter() - t0)
+    return {"workload": name, "frames": n, "frame": list(frames[0].shape), "mean_kp": float(np.mean([len(o[0]) for o in out])),
+            "mean_total_kp": float(np.mean([o[2] for o in out])), "mean_matches": float(np.mean([len(m) for m in res])),
+            "cv2_mean_matches": float(np.mean(counts)), "batched_dev_images_per_s": round(dev_ips, 1),
+            "plugin_host_images_per_s": round(plugin_ips, 1), "cv2_images_per_s": round(cv2_ips, 2),
+            "batched_vs_cv2": round(dev_ips / cv2_ips, 1), "front_end_dev_pairs_per_s": round(dev_pps, 1),
+            "cv2_front_end_pairs_per_s": round(cv2_pps, 2), "front_end_vs_cv2": round(dev_pps / cv2_pps, 1),
+            "stage_ms_per_image": stage_ms, "pyramid_bytes_per_image": pyramid_bytes(h, w, ch),
+            "pyramid_tb_per_s": round(pyr_tbs, 3), "pyramid_share_hbm_peak": round(pyr_tbs / HBM_TBS, 3)}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=8)
+    ap.add_argument("--synthetic-frames", type=int, default=21)
+    ap.add_argument("--out", default=str(ROOT / "profiles" / "h100_sift.json"))
+    a = ap.parse_args()
+
+    from gtsfm_b200 import _lib
+    from gtsfm_b200 import synthetic as syn
+
+    lund = np.load(ROOT / "tests" / "golden" / "lund_door_images.npz")
+    lund_frames = [lund[f"gray_{i}"] for i in range(1, 13)]
+    synth_frames = syn.synthetic_sequence(a.synthetic_frames, 2880, 3840)[0]
+    ctx = _lib.Context(0)
+    cores = os.cpu_count() or 1
+    with mp.get_context("spawn").Pool(cores) as pool:  # fresh processes: cv2's thread pool does not survive a fork
+        rows = [workload("lund_door_loader", lund_frames, a.reps, pool, cores, ctx), workload("synthetic_12mp", synth_frames, a.reps, pool, cores, ctx)]
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
+    name, power = [s.strip() for s in q.stdout.strip().splitlines()[0].split(",")]
+    line = {"workload": "sift", "cv2_cores": cores, "max_keypoints": 5000, "ratio": 0.8, "results": rows, "hbm_peak_tbs": HBM_TBS,
+            "gpu": name, "power_limit": power}
+    s = json.dumps(line)
+    print(s)
+    Path(a.out).parent.mkdir(parents=True, exist_ok=True)
+    Path(a.out).write_text(s + "\n")
+    ctx.close()
+
+
+if __name__ == "__main__":
+    main()
