@@ -93,6 +93,12 @@ SIGNATURES = {
     "b2_netvlad_set_weights": (_i, [_vp, _vp, _sz]),
     "b2_netvlad_describe_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
     "b2_netvlad_describe_host": (_i, [_vp, _vp, _i, _i, _i, _vp]),
+    "b2_megaloc_blob_floats": (_sz, []),
+    "b2_megaloc_set_weights": (_i, [_vp, _vp, _sz]),
+    "b2_megaloc_describe_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),
+    "b2_megaloc_describe_host": (_i, [_vp, _vp, _i, _i, _i, _vp]),
+    "b2_megaloc_describe_u8_dev": (_i, [_vp, _vp, _i, _i, _i, _sz, _vp, _vp]),
+    "b2_megaloc_resize_u8_dev": (_i, [_vp, _vp, _i, _i, _i, _sz, _vp, _vp]),
     "b2_similarity_pairs_host": (_i, [_vp, _vp, _i, _i, _i, _f, _vp, _vp]),
     "b2_ransac_essential_host": (_i, [_vp, _vp, _vp, _i, C.POINTER(RansacParams), _vp, _vp, _ip, _vp, _vp]),
     "b2_ransac_fundamental_host": (_i, [_vp, _vp, _vp, _i, C.POINTER(RansacParams), _vp, _vp, _ip]),

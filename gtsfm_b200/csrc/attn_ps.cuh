@@ -1,7 +1,8 @@
 // Persistent warp-specialised wgmma + TMA flash attention over a BATCH of problems, split-fp16 operands (~fp32 accuracy).
 //
-//   O[Nq][256] = softmax(scale * Q K^T) V per head; q / k / v arrive as fp16 hi / lo planes with UNSCALED lo
-//   (x ~= hi + lo, lo = fp16(x - hi)), the output leaves as hi / lo planes with the usual 2^11-scaled lo.
+//   O[Nq][ldo], columns 64 h .. 64 h + 63 = softmax(scale * Q_h K_h^T) V_h per head h (LightGlue / SuperGlue: 4 heads into
+//   [Nq][256]; MegaLoc's DINOv2: 12 heads into [Nq][768]); q / k / v arrive as head-major [heads][N][64] fp16 hi / lo planes
+//   with UNSCALED lo (x ~= hi + lo, lo = fp16(x - hi)), the output leaves as hi / lo planes with the usual 2^11-scaled lo.
 //
 // One CTA (288 threads, one per SM) owns TWO 128-query tiles of one head at a time and streams 64-key tiles.
 //   warp 8 lane 0 : TMA producer - K and V tiles through one 4-entry ring (128-byte swizzled, zero OOB fill)
@@ -35,13 +36,14 @@ constexpr float AS_RESCALE = 8.0f;  // log2 of the largest P allowed before the 
 constexpr int AP_MAXP = 16;         // problems per launch (2 images x 8 pairs)
 
 struct AttnPsMaps {
-  CUtensorMap kh[AP_MAXP], kl[AP_MAXP], vh[AP_MAXP], vl[AP_MAXP];  // per problem; 2-D views [4 * N rows][64] of the head-major planes
+  CUtensorMap kh[AP_MAXP], kl[AP_MAXP], vh[AP_MAXP], vl[AP_MAXP];  // per problem; 2-D views [heads * N rows][64] of the head-major planes
 };
 
 struct AttnPsProblem {
-  const __half *Qh, *Ql;  // head-major planes [4][Nq][64]
-  __half *Oh, *Ol;        // final output planes [Nq][256]
+  const __half *Qh, *Ql;  // head-major planes [heads][Nq][64]
+  __half *Oh, *Ol;        // final output planes [Nq][ldo]
   int Nq, Nk;
+  int ldo;                // output row pitch in halves (64 x heads when the heads fill the row)
   int qt, tiles;          // 256-query blocks, 64-key tiles
   int w_end;              // running total of (item, key tile) units up to and including this problem
   int item0;              // items (head x query block) of the problems before this one
@@ -269,8 +271,8 @@ static __global__ void __launch_bounds__(AS_THREADS, 1) k_flash_ps(const __grid_
           l_i[sl][h] += __shfl_xor_sync(0xffffffffu, l_i[sl][h], 2);
         }
       auto write_row = [&](const float* v, float inv, int qrow) {  // v[4j + e] scaled by inv -> output dims 8j + c2 + e
-        uint32_t* dh = reinterpret_cast<uint32_t*>(pr.Oh + (size_t)qrow * 256 + sg.h * 64 + c2);
-        uint32_t* dl = reinterpret_cast<uint32_t*>(pr.Ol + (size_t)qrow * 256 + sg.h * 64 + c2);
+        uint32_t* dh = reinterpret_cast<uint32_t*>(pr.Oh + (size_t)qrow * pr.ldo + sg.h * 64 + c2);
+        uint32_t* dl = reinterpret_cast<uint32_t*>(pr.Ol + (size_t)qrow * pr.ldo + sg.h * 64 + c2);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           uint32_t hi, lo;

@@ -88,6 +88,7 @@ struct RetrievalState;
 struct NetVladState;
 struct MnnState;
 struct SiftState;
+struct MegaLocState;
 
 // Device copies of host feature arrays handed to the *_host matcher entry points.  GTSfM matches one image's (keypoints,
 // descriptors) against ~20-40 partners, always passing the same host arrays, so re-uploading 5 MB per image per pair is
@@ -124,6 +125,7 @@ struct b2_context {
   NetVladState* nv = nullptr;
   MnnState* mn = nullptr;
   SiftState* sf = nullptr;
+  MegaLocState* ml = nullptr;
   // staging shared by the *_host entry points
   DevBuf stage_d[8];
   HostBuf stage_h[4];
@@ -189,6 +191,7 @@ void rt_destroy(b2_context* ctx);
 void nv_destroy(b2_context* ctx);
 void mn_destroy(b2_context* ctx);
 void sf_destroy(b2_context* ctx);
+void ml_destroy(b2_context* ctx);
 
 // shared device helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

@@ -24,8 +24,8 @@
 // ptxas cap the kernel at 128 registers and spill the accumulators; with 3 epilogue warps and no rebalance the family took
 // 91-93 ms per vga_lightglue step against 85 ms with 4 (H100 80GB HBM3, three alternated runs each).
 // Shared memory: 2 x 64 KB ring + 68 KB staging (a third ring stage no longer fits).  The epilogue computes exactly what
-// the consumers used to: (fmaf(acc1, 2^-11, acc0) + bias) * scale, ReLU, + residual, then the same split helpers.  Its
-// mode flags (relu, head-major, unscaled lo, which outputs) are read once per tile and are warp-uniform; they are not
+// the consumers used to: (fmaf(acc1, 2^-11, acc0) + bias) * scale, ReLU or GELU, + residual, then the same split helpers.  Its
+// mode flags (relu, gelu, head-major, unscaled lo, which outputs) are read once per tile and are warp-uniform; they are not
 // compile-time specialisations.
 #pragma once
 #include "tma.cuh"
@@ -69,6 +69,7 @@ struct GemmWsArgs {
   int ldch;        // row-major leading dimension of Ch / Cl (ignored when head_major)
   int head_major;  // 1: Ch / Cl (and C) are written as [N/64][M][64] (attention head layout)
   int relu;        // max(., 0) after bias / scale, before the residual
+  int gelu;        // exact (erf) GELU after bias / scale, before the residual
   int lo_unscaled; // split outputs keep lo = fp16(x - hi) (attention operands)
   int* err_flag;   // set to 1 if an mbarrier wait timed out (pipeline bug): results are then invalid
 };
@@ -184,7 +185,7 @@ static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_c
     const int ew = warp - 8;
     const int c = 4 * lane;
     const float scale = g.scale;
-    const int relu = g.relu, hm = g.head_major, lo_unscaled = g.lo_unscaled, ldr = g.ldr, ldch = g.ldch;
+    const int relu = g.relu, gelu = g.gelu, hm = g.head_major, lo_unscaled = g.lo_unscaled, ldr = g.ldr, ldch = g.ldch;
     int it = 0;
     for (int tile = blockIdx.x; tile < g.tiles; tile += gridDim.x, ++it) {
       int z, m0, n0;
@@ -230,6 +231,7 @@ static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_c
             for (int e = 0; e < 4; ++e) {
               v[e] = (v[e] + b4[e]) * scale;
               if (relu) v[e] = fmaxf(v[e], 0.f);
+              if (gelu) v[e] = 0.5f * v[e] * (1.0f + erff(v[e] * 0.70710678118654752440f));
             }
             const size_t off_c = hm ? hm_col + (size_t)row * 64 : (size_t)row * ldc + n;
             const size_t off_s = hm ? hm_col + (size_t)row * 64 : (size_t)row * ldch + n;

@@ -49,6 +49,7 @@ struct LinArgs {
   int head_major = 0;
   bool tc_want_f32 = false;
   int relu = 0;  // max(., 0) after bias / scale, before the residual
+  int gelu = 0;  // exact GELU after bias / scale, before the residual (wgmma path only)
   int lo_unscaled = 0;  // plane output with an unscaled lo plane (attention operands)
   int M = 0, N = 0;
 };
@@ -63,6 +64,7 @@ static int run_linear(b2_context* ctx, cudaStream_t st, const TcWeights& tw, con
     for (int i = 0; i < np; ++i) {
       const LinArgs& x = a[i];
       if (x.M <= 0 || x.N <= 0) continue;
+      if (x.gelu) return b2_fail(ctx, B2_ERR_ARG, "run_linear: the GELU epilogue exists on the wgmma path only");
       GemmArgs g{};
       g.A1 = x.a1f, g.lda1 = x.lda1, g.K1 = x.K1, g.A2 = x.a2f, g.lda2 = x.lda2, g.K2 = x.K2;
       g.B = x.w ? x.w : x.bf, g.ldb = x.ldb, g.C = x.cf, g.ldc = x.ldc, g.M = x.M, g.N = x.N;
@@ -115,31 +117,24 @@ static int run_linear(b2_context* ctx, cudaStream_t st, const TcWeights& tw, con
   if (!ok) return b2_fail(ctx, B2_ERR_CUDA, "cuTensorMapEncodeTiled failed");
   q.nprob = nz, q.tiles = tiles, q.K1 = a0.K1, q.K2 = a0.K2, q.b_per_problem = per_b ? 1 : 0;
   q.bias = a0.bias, q.ldr = a0.ldr, q.scale = a0.scale, q.ldch = a0.ldch;
-  q.head_major = a0.head_major, q.relu = a0.relu, q.lo_unscaled = a0.lo_unscaled, q.err_flag = tw.err;
+  q.head_major = a0.head_major, q.relu = a0.relu, q.gelu = a0.gelu, q.lo_unscaled = a0.lo_unscaled, q.err_flag = tw.err;
   b2_prof_work(ctx, "k_gemm_ws", work);
   B2_LAUNCH(ctx, k_gemm_ws, tiles < tw.sm_count ? tiles : tw.sm_count, GW_THREADS, GW_SMEM, st, maps, q);
   B2_CHECK_LAUNCH(ctx);
   return B2_OK;
 }
 
-// One attention problem of a batched launch.  wgmma path: q / k / v / o buffers hold split fp16 planes (hi, then lo at
-// + cap * 256 halves).
-struct FlashJob {
-  const DevBuf *q, *k, *v, *o;
+// One attention problem of a batched launch, as plane views (wgmma path only): q / k / v head-major [heads][n][64] with
+// unscaled lo planes, o row-major [nq][ldo] (head h in columns 64 h .. 64 h + 63).
+struct FlashPlanes {
+  Pl q, k, v, o;
   int nq, nk;
-  int capq, capk;  // allocated rows of the query-side / key-side buffers (lo plane offset = cap * 256 halves)
+  int heads, ldo;
 };
-static int run_flash(b2_context* ctx, cudaStream_t st, const TcWeights& tw, const FlashJob* jobs, int np, float scale, bool fp16_single = false) {
+static int run_flash_planes(b2_context* ctx, cudaStream_t st, const TcWeights& tw, const FlashPlanes* jobs, int np, float scale,
+                            bool fp16_single = false) {
   if (np <= 0) return B2_OK;
   if (np > AP_MAXP) return b2_fail(ctx, B2_ERR_ARG, "run_flash: too many problems in one launch");
-  if (!tw.use_tc) {
-    for (int i = 0; i < np; ++i) {
-      const FlashJob& j = jobs[i];
-      int rc = launch_flash(ctx, st, j.q->as<float>(), j.k->as<float>(), j.v->as<float>(), j.o->as<float>(), j.nq, j.nk, scale);
-      if (rc) return rc;
-    }
-    return B2_OK;
-  }
   if (!tma_encoder() || !tw.attn_part) return b2_fail(ctx, B2_ERR_CUDA, "wgmma attention needs cuTensorMapEncodeTiled and its scratch buffers");
   static thread_local AttnPsMaps tmaps;
   AttnPsArgs pa{};
@@ -147,21 +142,20 @@ static int run_flash(b2_context* ctx, cudaStream_t st, const TcWeights& tw, cons
   int items = 0, nz = 0, W = 0, tmax = 0;
   double work = 0.0;
   for (int i = 0; i < np; ++i) {
-    const FlashJob& j = jobs[i];
+    const FlashPlanes& j = jobs[i];
     if (j.nq <= 0 || j.nk <= 0) continue;
-    const Pl q = planes_of(*j.q, (size_t)j.capq * 256), k = planes_of(*j.k, (size_t)j.capk * 256), v = planes_of(*j.v, (size_t)j.capk * 256),
-             o = planes_of(*j.o, (size_t)j.capq * 256);
     AttnPsProblem& p = pa.p[nz];
-    p.Qh = q.hi, p.Ql = q.lo, p.Oh = o.hi, p.Ol = o.lo, p.Nq = j.nq, p.Nk = j.nk;
+    p.Qh = j.q.hi, p.Ql = j.q.lo, p.Oh = j.o.hi, p.Ol = j.o.lo, p.Nq = j.nq, p.Nk = j.nk, p.ldo = j.ldo;
     p.qt = cdiv(j.nq, 2 * AW_Q), p.tiles = cdiv(j.nk, AW_KV);
     p.item0 = items;
-    items += p.qt * 4;
-    W += p.qt * 4 * p.tiles;
+    items += p.qt * j.heads;
+    W += p.qt * j.heads * p.tiles;
     p.w_end = W;
     tmax = p.tiles > tmax ? p.tiles : tmax;
-    okm = okm && tma_map_2d(&tmaps.kh[nz], k.hi, (uint64_t)4 * j.nk, 64, 64, AW_KV) && tma_map_2d(&tmaps.kl[nz], k.lo, (uint64_t)4 * j.nk, 64, 64, AW_KV);
-    okm = okm && tma_map_2d(&tmaps.vh[nz], v.hi, (uint64_t)4 * j.nk, 64, 64, AW_KV) && tma_map_2d(&tmaps.vl[nz], v.lo, (uint64_t)4 * j.nk, 64, 64, AW_KV);
-    work += 4.0 * 2.0 * 2.0 * 64 * (double)j.nq * j.nk;  // 4 heads x (QK^T + PV) x 2 FLOP/MAC
+    const uint64_t rows = (uint64_t)j.heads * j.nk;
+    okm = okm && tma_map_2d(&tmaps.kh[nz], j.k.hi, rows, 64, 64, AW_KV) && tma_map_2d(&tmaps.kl[nz], j.k.lo, rows, 64, 64, AW_KV);
+    okm = okm && tma_map_2d(&tmaps.vh[nz], j.v.hi, rows, 64, 64, AW_KV) && tma_map_2d(&tmaps.vl[nz], j.v.lo, rows, 64, 64, AW_KV);
+    work += j.heads * 2.0 * 2.0 * 64 * (double)j.nq * j.nk;  // heads x (QK^T + PV) x 2 FLOP/MAC
     ++nz;
   }
   if (nz == 0) return B2_OK;
@@ -189,4 +183,31 @@ static int run_flash(b2_context* ctx, cudaStream_t st, const TcWeights& tw, cons
   else B2_LAUNCH(ctx, k_flash_ps<false>, ncta, AS_THREADS, AS_SMEM, st, tmaps, pa);
   B2_CHECK_LAUNCH(ctx);
   return B2_OK;
+}
+
+// One 4-head attention problem of a batched launch (LightGlue, SuperGlue).  wgmma path: q / k / v / o buffers hold split
+// fp16 planes (hi, then lo at + cap * 256 halves); the SIMT path reads them as fp32.
+struct FlashJob {
+  const DevBuf *q, *k, *v, *o;
+  int nq, nk;
+  int capq, capk;  // allocated rows of the query-side / key-side buffers (lo plane offset = cap * 256 halves)
+};
+static int run_flash(b2_context* ctx, cudaStream_t st, const TcWeights& tw, const FlashJob* jobs, int np, float scale, bool fp16_single = false) {
+  if (np <= 0) return B2_OK;
+  if (np > AP_MAXP) return b2_fail(ctx, B2_ERR_ARG, "run_flash: too many problems in one launch");
+  if (!tw.use_tc) {
+    for (int i = 0; i < np; ++i) {
+      const FlashJob& j = jobs[i];
+      int rc = launch_flash(ctx, st, j.q->as<float>(), j.k->as<float>(), j.v->as<float>(), j.o->as<float>(), j.nq, j.nk, scale);
+      if (rc) return rc;
+    }
+    return B2_OK;
+  }
+  FlashPlanes fp[AP_MAXP];
+  for (int i = 0; i < np; ++i) {
+    const FlashJob& j = jobs[i];
+    fp[i] = {planes_of(*j.q, (size_t)j.capq * 256), planes_of(*j.k, (size_t)j.capk * 256), planes_of(*j.v, (size_t)j.capk * 256),
+             planes_of(*j.o, (size_t)j.capq * 256), j.nq, j.nk, 4, 256};
+  }
+  return run_flash_planes(ctx, st, tw, fp, np, scale, fp16_single);
 }

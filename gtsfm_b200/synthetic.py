@@ -184,6 +184,53 @@ def netvlad_state_dict(seed: int = 3, whiten_dim: int = 4096) -> Dict[str, np.nd
     return sd
 
 
+def megaloc_state_dict(seed: int = 5) -> Dict[str, np.ndarray]:
+    """Seeded weights with the names and shapes of the reference's MegaLoc checkpoint (190 tensors: DINOv2 ViT-B/14 under
+    `backbone.model.`, SALAD under `aggregator.agg.`, the final `aggregator.linear`).  No checkpoint can be downloaded offline.
+
+    Torch's default init makes every image look alike (cosine 0.9997 between two random images), which would let any
+    parity test pass trivially.  Here the patch embedding is strong (so image content dominates the position table), the
+    residual branches are small (LayerScale 0.1), attention logits are O(1), and the SALAD score head is sharp, so distinct
+    frames land far apart and a shifted view of a frame stays nearest to that frame."""
+    rng = np.random.default_rng(seed)
+    sd: Dict[str, np.ndarray] = {}
+    d, bb, ag = 768, "backbone.model.", "aggregator.agg."
+
+    def lin(name, o, i, gain=1.0, bias_std=0.02, shape=None):
+        w, b = _lin(rng, o, i, gain, bias_std)
+        sd[name + ".weight"] = w.reshape(shape) if shape else w
+        sd[name + ".bias"] = b
+
+    sd[bb + "cls_token"] = (0.5 * rng.standard_normal((1, 1, d))).astype(np.float32)
+    sd[bb + "pos_embed"] = (0.1 * rng.standard_normal((1, 1 + 37 * 37, d))).astype(np.float32)
+    sd[bb + "mask_token"] = np.zeros((1, d), np.float32)
+    lin(bb + "patch_embed.proj", d, 588, gain=3.0, shape=(d, 3, 14, 14))
+    for i in range(12):
+        p = f"{bb}blocks.{i}."
+        sd[p + "norm1.weight"] = (1.0 + 0.1 * rng.standard_normal(d)).astype(np.float32)
+        sd[p + "norm1.bias"] = (0.05 * rng.standard_normal(d)).astype(np.float32)
+        lin(p + "attn.qkv", 3 * d, d, gain=1.0)
+        lin(p + "attn.proj", d, d, gain=1.0)
+        sd[p + "ls1.gamma"] = (0.1 * (1.0 + 0.2 * rng.standard_normal(d))).astype(np.float32)
+        sd[p + "norm2.weight"] = (1.0 + 0.1 * rng.standard_normal(d)).astype(np.float32)
+        sd[p + "norm2.bias"] = (0.05 * rng.standard_normal(d)).astype(np.float32)
+        lin(p + "mlp.fc1", 4 * d, d, gain=1.4)
+        lin(p + "mlp.fc2", d, 4 * d, gain=1.0)
+        sd[p + "ls2.gamma"] = (0.1 * (1.0 + 0.2 * rng.standard_normal(d))).astype(np.float32)
+    sd[bb + "norm.weight"] = (1.0 + 0.1 * rng.standard_normal(d)).astype(np.float32)
+    sd[bb + "norm.bias"] = (0.05 * rng.standard_normal(d)).astype(np.float32)
+    lin(ag + "token_features.0", 512, d, gain=1.4)
+    lin(ag + "token_features.2", 256, 512, gain=1.0)
+    lin(ag + "cluster_features.0", 512, d, gain=1.4, shape=(512, d, 1, 1))
+    lin(ag + "cluster_features.3", 256, 512, gain=2.0, shape=(256, 512, 1, 1))
+    lin(ag + "score.0", 512, d, gain=1.4, shape=(512, d, 1, 1))
+    lin(ag + "score.3", 64, 512, gain=8.0, shape=(64, 512, 1, 1))
+    sd[ag + "dust_bin"] = np.array(1.0, np.float32)
+    sd["aggregator.linear.weight"] = (rng.standard_normal((8448, 16640), dtype=np.float32) * np.float32(1.0 / np.sqrt(16640.0)))
+    sd["aggregator.linear.bias"] = (0.002 * rng.standard_normal(8448)).astype(np.float32)
+    return sd
+
+
 def save_pth(state: Dict[str, np.ndarray], path) -> None:
     """Write a state dict in the reference's checkpoint format (torch.save of name -> tensor)."""
     import torch

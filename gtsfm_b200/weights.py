@@ -168,3 +168,31 @@ def pack_netvlad(sd: StateDict) -> np.ndarray:
     blob = _pack(sd, NETVLAD_ORDER)
     assert blob.size == 14714688 + 2 * 64 * 512 + 4096 * 32768 + 4096 + 3, blob.size
     return blob
+
+
+# ---- MegaLoc (thirdparty/megaloc/megaloc.py: DINOv2 ViT-B/14 backbone + SALAD aggregator + Linear(16640, 8448)) ---------------------
+MEGALOC_BLOCKS = 12
+_ML_BB = "backbone.model."
+_ML_AGG = "aggregator.agg."
+MEGALOC_ORDER: List[str] = (
+    [_ML_BB + n for n in ("cls_token", "pos_embed", "patch_embed.proj.weight", "patch_embed.proj.bias")]
+    + [f"{_ML_BB}blocks.{i}.{n}" for i in range(MEGALOC_BLOCKS)
+       for n in ("norm1.weight", "norm1.bias", "attn.qkv.weight", "attn.qkv.bias", "attn.proj.weight", "attn.proj.bias", "ls1.gamma",
+                 "norm2.weight", "norm2.bias", "mlp.fc1.weight", "mlp.fc1.bias", "mlp.fc2.weight", "mlp.fc2.bias", "ls2.gamma")]
+    + [_ML_BB + "norm.weight", _ML_BB + "norm.bias"]
+    + [_ML_AGG + f"{m}.{i}.{p}" for m, idx in (("cluster_features", (0, 3)), ("score", (0, 3)), ("token_features", (0, 2)))
+       for i in idx for p in ("weight", "bias")]
+    + [_ML_AGG + "dust_bin", "aggregator.linear.weight", "aggregator.linear.bias"]
+)
+MEGALOC_BLOB_FLOATS = 228640321 - 768  # the checkpoint's parameters without mask_token (unused at inference)
+
+
+def load_megaloc(src: Union[str, Path, StateDict]) -> StateDict:
+    """The reference's `megaloc.torch` (a torch.save state dict, megaloc.py:52-62) or an in-memory dict."""
+    return load_state_dict(src)
+
+
+def pack_megaloc(sd: StateDict) -> np.ndarray:
+    blob = _pack(sd, MEGALOC_ORDER)
+    assert blob.size == MEGALOC_BLOB_FLOATS, blob.size
+    return blob

@@ -230,6 +230,32 @@ int b2_netvlad_set_weights(b2_context* ctx, const float* blob, size_t n_floats);
 int b2_netvlad_describe_dev(b2_context* ctx, const float* images, int batch, int height, int width, float* out, void* stream);
 int b2_netvlad_describe_host(b2_context* ctx, const float* images, int batch, int height, int width, float* out);
 
+/* ---- MegaLoc global descriptor (gtsfm/frontend/global_descriptor/megaloc_global_descriptor.py:18-77,
+ * thirdparty/megaloc/megaloc.py:25-257: DINOv2 ViT-B/14 + SALAD + Linear(16640 -> 8448)) ------------------------------------ */
+/* blob = cls_token [768], pos_embed [1370][768], patch_embed.proj weight [768][3][14][14] and bias; 12 x (norm1 weight, bias,
+ * attn.qkv weight [2304][768], bias, attn.proj weight [768][768], bias, ls1.gamma, norm2 weight, bias, mlp.fc1 weight
+ * [3072][768], bias, mlp.fc2 weight [768][3072], bias, ls2.gamma); norm weight, bias; SALAD cluster_features.0 weight
+ * [512][768], bias, .3 weight [256][512], bias; score.0 weight [512][768], bias, .3 weight [64][512], bias; token_features.0
+ * weight [512][768], bias, .2 weight [256][512], bias; dust_bin; aggregator.linear weight [8448][16640], bias:
+ * b2_megaloc_blob_floats() floats (the checkpoint's tensors without mask_token, in gtsfm_b200.weights.MEGALOC_ORDER).
+ * MegaLoc runs on the tensor-core path only: with the "force_simt" option set every b2_megaloc_* call returns -3. */
+size_t b2_megaloc_blob_floats(void);
+int b2_megaloc_set_weights(b2_context* ctx, const float* blob, size_t n_floats);
+/* images: DEVICE [B][3][H][W] fp32, normalised as the plugin's batch transform does ((x / 255 - mean) / std, ImageNet); H and W
+ * multiples of 14 with more than 64 patches (H / 14) (W / 14), otherwise -2.  out: DEVICE [B][8448] unit-norm descriptors.
+ * Any B: the backbone runs in chunks of 16 images, the final Linear over all B at once.  Synchronises `stream`. */
+int b2_megaloc_describe_dev(b2_context* ctx, const float* images, int batch, int height, int width, float* out, void* stream);
+int b2_megaloc_describe_host(b2_context* ctx, const float* images, int batch, int height, int width, float* out);
+/* The plugin's whole preprocessing on the device: images = HOST array of n DEVICE pointers to uint8 H x W x 3 (RGB) images of
+ * one shape and row pitch (bytes), e.g. the frames already uploaded for b2_sift_detect_batched_dev.  torchvision's
+ * Resize((322, 322), antialias=True) on uint8 (torch's integer path, bit for bit), then / 255 and the ImageNet normalisation,
+ * then the network.  out: DEVICE [n][8448].  Synchronises `stream`. */
+int b2_megaloc_describe_u8_dev(b2_context* ctx, const uint8_t* const* images, int n, int height, int width, size_t pitch, float* out,
+                               void* stream);
+/* The resize alone: out = DEVICE uint8 [n][3][322][322] (what the plugin's resize transform returns).  Synchronises `stream`. */
+int b2_megaloc_resize_u8_dev(b2_context* ctx, const uint8_t* const* images, int n, int height, int width, size_t pitch, uint8_t* out,
+                             void* stream);
+
 /* ---- retrieval front (SURVEY.md section 8f rank 4) ---------------------------------------------------------------- */
 /* gtsfm/retriever/similarity_retriever.py:86-260: sim = G G^T of the global image descriptors (desc: HOST [n][dim] fp32,
  * dim a multiple of 64), then per query image i its `num_matched` best partners among j > i with sim >= min_score, best
