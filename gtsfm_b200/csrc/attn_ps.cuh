@@ -4,12 +4,23 @@
 //   [Nq][256]; MegaLoc's DINOv2: 12 heads into [Nq][768]); q / k / v arrive as head-major [heads][N][64] fp16 hi / lo planes
 //   with UNSCALED lo (x ~= hi + lo, lo = fp16(x - hi)), the output leaves as hi / lo planes with the usual 2^11-scaled lo.
 //
-// One CTA (288 threads, one per SM) owns TWO 128-query tiles of one head at a time and streams 64-key tiles.
-//   warp 8 lane 0 : TMA producer - K and V tiles through one 4-entry ring (128-byte swizzled, zero OOB fill)
-//   warps 0-3 / 4-7: consumer warpgroup of query tile 0 / 1, Q hi / lo in shared memory.  Per key tile and 64-row slab:
-//                   S = Qh Kh^T + Qh Kl^T + Ql Kh^T (wgmma from shared memory); base-2 online softmax on the fragment with a
+// One CTA (384 threads, one per SM) owns TWO 128-query tiles of one head at a time and streams 64-key tiles.
+//   warp 8 lane 0 : TMA producer - K and V tiles through one 4-entry ring (128-byte swizzled, zero OOB fill); warps 9-11
+//                   only exist so that the producer has a warpgroup of its own for setmaxnreg
+//   warps 0-3 / 4-7: consumer warpgroup of query tile 0 / 1, Q lo in shared memory and Q hi in registers.  Per key tile
+//                   and 64-row slab: S = Qh Kh^T + Qh Kl^T + Ql Kh^T (the Qh products take A from registers, so they read
+//                   only K from shared memory: with 64-wide tiles these MMAs are paced by shared-memory reads, and this
+//                   removes a third of the QK traffic); base-2 online softmax on the fragment with a
 //                   LAZY reference maximum (rescale only when the row maximum grew by more than 2^8: P <= 256 stays exact
 //                   in the hi / lo split); O += Ph Vh + Ph Vl + Pl Vh (P from registers, V MN-major), O kept in registers.
+// Software pipeline inside a consumer warpgroup: the softmax of one slab runs while the tensor core works on the other
+// slab's MMAs.  Per key tile i:
+//     QK(i, 0) QK(i, 1) | wait QK(i, 0) | softmax 0 | PV(i, 0) | wait QK(i, 1) | softmax 1 | PV(i, 1) | wait PV(i, *)
+// While one warpgroup waits for its last PV, the other warpgroup's MMAs keep the tensor core busy.
+// Every accumulator still receives the same MMAs in the same order, so the result is bit-identical to running the slabs one
+// after the other.  Registers: 384 threads start at 168 each; setmaxnreg moves them to the consumers (240) and leaves the
+// producer 24, which holds both O accumulators, Q hi of both slabs, one S being produced while the other is softmaxed, and
+// the P planes that an in-flight PV MMA still reads, without spilling.
 //
 // Schedule ("stream-K" over the key dimension): the whole launch - every problem of the batch, i.e. the self- or
 // cross-attention of all images of up to 8 pairs - is ONE linear space of (item, key tile) units, item = (problem, head,
@@ -31,7 +42,7 @@ constexpr int AS_TILE_BYTES = AS_NS * AS_STAGE;
 constexpr int AS_Q_PLANE = AW_Q * AW_D * 2;  // 16 KB: one plane of a 128-query tile
 constexpr int AS_Q_BYTES = 2 * 2 * AS_Q_PLANE;  // hi + lo planes of both query tiles
 constexpr size_t AS_SMEM = AS_TILE_BYTES + AS_Q_BYTES + 1024 + 512;
-constexpr int AS_THREADS = 256 + 32;  // 2 consumer warpgroups + TMA producer warp
+constexpr int AS_THREADS = 256 + 128;  // 2 consumer warpgroups + TMA producer warpgroup (one thread works)
 constexpr float AS_RESCALE = 8.0f;  // log2 of the largest P allowed before the reference maximum is refreshed
 constexpr int AP_MAXP = 16;         // problems per launch (2 images x 8 pairs)
 
@@ -110,8 +121,9 @@ static __global__ void __launch_bounds__(AS_THREADS, 1) k_flash_ps(const __grid_
   __syncthreads();
   bool ok = true;
 
-  if (warp == 8) {
-    if (lane == 0) {
+  if (warp >= 8) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n" ::: "memory");
+    if (warp == 8 && lane == 0) {
       // ===== TMA producer: ring entry e of a segment = K tile e (if any) + V tile e - 2 (if any) =====
       int ge = 0;
       for (int w = w_begin; w < w_end;) {
@@ -140,6 +152,7 @@ static __global__ void __launch_bounds__(AS_THREADS, 1) k_flash_ps(const __grid_
       }
     }
   } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 240;\n" ::: "memory");
     // ===== consumer warpgroup q: query rows q * 128 + slab * 64 + rq (+ 8) =====
     const int q = warp >> 2;
     const int r = t & 127;
@@ -172,93 +185,128 @@ static __global__ void __launch_bounds__(AS_THREADS, 1) k_flash_ps(const __grid_
         tc::fence_proxy_async();  // generic-proxy stores -> visible to the tensor core
         wg_bar();
       }
+      // Q hi of slab 0 / 1 also as register A fragments (k step ks: registers 4 ks .. 4 ks + 3): the QK products with Qh
+      // then read only K from shared memory
+      uint32_t qf[2][16];
+#pragma unroll
+      for (int sl = 0; sl < 2; ++sl)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int qrow = sg.q0 + q * AW_Q + sl * 64 + rq + 8 * h;
+          const uint32_t* src = reinterpret_cast<const uint32_t*>(pr.Qh + ((size_t)sg.h * pr.Nq + qrow) * 64 + c2);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) qf[sl][4 * (j >> 1) + 2 * (j & 1) + h] = qrow < pr.Nq ? __ldg(src + 4 * j) : 0u;
+        }
       float o[2][32];
       float m_ref[2][2], l_i[2][2];
 #pragma unroll
       for (int sl = 0; sl < 2; ++sl)
 #pragma unroll
         for (int h = 0; h < 2; ++h) m_ref[sl][h] = -INFINITY, l_i[sl][h] = 0.f;
+      float s[2][32];                 // S of slab 0 / 1
+      uint32_t ph[2][16], pl[2][16];  // P hi / lo planes of slab 0 / 1: register A operands of the PV MMAs
+      // S(sl) = Q(sl) K(i)^T: one commit group
+      auto qk = [&](int i, int sl) {
+        const uint32_t sK = smem0 + ((ge + i) % AS_NS) * AS_STAGE;
+        const uint64_t dKh = tc::wg_desc_sw128(sK), dKl = tc::wg_desc_sw128(sK + AW_KV_BYTES);
+        const uint64_t dQl = tc::wg_desc_sw128(sQ + AS_Q_PLANE + sl * (64 * 128));
+        tc::wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+          const uint64_t adv = (uint64_t)(ks * 2);
+          tc::wg_rs_n64(s[sl], qf[sl] + 4 * ks, dKh + adv, ks ? 1u : 0u);
+          if (!SINGLE) {
+            tc::wg_rs_n64(s[sl], qf[sl] + 4 * ks, dKl + adv, 1u);
+            tc::wg_ss_n64(s[sl], dQl + adv, dKh + adv, 1u);
+          }
+        }
+        tc::wg_commit();
+      };
+      // online softmax of S(sl) of key tile i -> P(sl), rescaling O(sl) when the reference maximum moves
+      auto softmax = [&](int i, int sl) {
+        float* a = s[sl];
+        const int k0 = (sg.tile0 + i) * AW_KV;
+        if (k0 + AW_KV > Nk) {
+#pragma unroll
+          for (int jj = 0; jj < 32; ++jj)
+            if (k0 + 8 * (jj >> 2) + c2 + (jj & 1) >= Nk) a[jj] = -INFINITY;  // 2^(-inf) = 0
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {  // fragment row rq + 8h: a[4j + 2h + e]
+          float mx = a[2 * h];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) mx = fmaxf(mx, fmaxf(a[4 * j + 2 * h], a[4 * j + 2 * h + 1]));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          const float m_new = fmaxf(m_ref[sl][h], mx * c2s);
+          if (m_new - m_ref[sl][h] > AS_RESCALE) {  // also true on the first tile (m_ref = -inf); uniform over the quad
+            const float corr = tc::ex2(m_ref[sl][h] - m_new);
+            l_i[sl][h] *= corr;
+            if (i > 0) {
+#pragma unroll
+              for (int j = 0; j < 8; ++j) o[sl][4 * j + 2 * h] *= corr, o[sl][4 * j + 2 * h + 1] *= corr;
+            }
+            m_ref[sl][h] = m_new;
+          }
+          float rs = 0.f;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float p0 = tc::ex2(fmaf(a[4 * j + 2 * h], c2s, -m_ref[sl][h]));
+            const float p1 = tc::ex2(fmaf(a[4 * j + 2 * h + 1], c2s, -m_ref[sl][h]));
+            rs += p0 + p1;
+            const __half2 hh = __floats2half2_rn(p0, p1);
+            // A fragment of k step j / 2: registers (row rq, k 2c), (row rq + 8, k 2c), (row rq, k 2c + 8), (row rq + 8, ...)
+            const int ri = 4 * (j >> 1) + 2 * (j & 1) + h;
+            ph[sl][ri] = *reinterpret_cast<const uint32_t*>(&hh);
+            if (!SINGLE) {
+              const float2 hf = __half22float2(hh);
+              const __half2 ll = __floats2half2_rn(p0 - hf.x, p1 - hf.y);  // p - hi, exact
+              pl[sl][ri] = *reinterpret_cast<const uint32_t*>(&ll);
+            }
+          }
+          l_i[sl][h] += rs;
+        }
+      };
+      // O(sl) += P(sl) V(i): one commit group
+      auto pv = [&](int i, int sl) {
+        const uint32_t sV = smem0 + ((ge + i + 2) % AS_NS) * AS_STAGE + AS_HALF;
+        const uint64_t dVh = tc::wg_desc_sw128(sV), dVl = tc::wg_desc_sw128(sV + AW_KV_BYTES);
+        tc::wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+          const uint64_t advV = (uint64_t)(ks * 128);  // 16 key rows of 128 bytes
+          tc::wg_rs_n64_bt(o[sl], ph[sl] + 4 * ks, dVh + advV, (i | ks) ? 1u : 0u);
+          if (!SINGLE) {
+            tc::wg_rs_n64_bt(o[sl], ph[sl] + 4 * ks, dVl + advV, 1u);
+            tc::wg_rs_n64_bt(o[sl], pl[sl] + 4 * ks, dVh + advV, 1u);
+          }
+        }
+        tc::wg_commit();
+      };
+
+      // Ring entry ge + e holds K tile e (e < T) and V tile e - 2 (e >= 2); every entry is released exactly once, after all
+      // MMAs that read it have completed.  Key tiles i - 1 and i share no MMA in flight: ptxas cannot count commit groups
+      // across the loop's back edge and, if any were left in flight there, would serialise every MMA of the loop.
       for (int j = 0; j < 2; ++j) ok = tc::mbar_wait(&kv_full[(ge + j) % AS_NS], ((ge + j) / AS_NS) & 1) && ok;
       if (T == 1) release(ge + 1);  // ring entry 1 of a one-tile segment is empty but still cycles through the ring
       for (int i = 0; i < T; ++i) {
+        // K tile i sits in an entry already waited for (the prologue, or V tile i - 2's entry)
+        qk(i, 0);
+        qk(i, 1);
+        tc::wg_wait<1>();  // QK(i, 0) has completed; softmax 0 overlaps QK(i, 1)
+        tc::fence_regs(s[0]);
+        softmax(i, 0);
         const int gv = ge + i + 2;  // ring entry: V tile i and (if any) K tile i + 2
         ok = tc::mbar_wait(&kv_full[gv % AS_NS], (gv / AS_NS) & 1) && ok;
-        const uint32_t sK = smem0 + ((ge + i) % AS_NS) * AS_STAGE, sV = smem0 + (gv % AS_NS) * AS_STAGE + AS_HALF;
-        const uint64_t dKh = tc::wg_desc_sw128(sK), dKl = tc::wg_desc_sw128(sK + AW_KV_BYTES);
-        const uint64_t dVh = tc::wg_desc_sw128(sV), dVl = tc::wg_desc_sw128(sV + AW_KV_BYTES);
-        const int k0 = (sg.tile0 + i) * AW_KV;
-#pragma unroll
-        for (int sl = 0; sl < 2; ++sl) {
-          const uint64_t dQh = tc::wg_desc_sw128(sQ + sl * (64 * 128)), dQl = tc::wg_desc_sw128(sQ + AS_Q_PLANE + sl * (64 * 128));
-          float a[32];
-          tc::wg_fence();
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t adv = (uint64_t)(ks * 2);
-            tc::wg_ss_n64(a, dQh + adv, dKh + adv, ks ? 1u : 0u);
-            if (!SINGLE) {
-              tc::wg_ss_n64(a, dQh + adv, dKl + adv, 1u);
-              tc::wg_ss_n64(a, dQl + adv, dKh + adv, 1u);
-            }
-          }
-          tc::wg_commit();
-          tc::wg_wait<0>();
-          if (k0 + AW_KV > Nk) {
-#pragma unroll
-            for (int jj = 0; jj < 32; ++jj)
-              if (k0 + 8 * (jj >> 2) + c2 + (jj & 1) >= Nk) a[jj] = -INFINITY;  // 2^(-inf) = 0
-          }
-          uint32_t ph[16], pl[16];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {  // fragment row rq + 8h: a[4j + 2h + e]
-            float mx = a[2 * h];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) mx = fmaxf(mx, fmaxf(a[4 * j + 2 * h], a[4 * j + 2 * h + 1]));
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-            const float m_new = fmaxf(m_ref[sl][h], mx * c2s);
-            if (m_new - m_ref[sl][h] > AS_RESCALE) {  // also true on the first tile (m_ref = -inf); uniform over the quad
-              const float corr = tc::ex2(m_ref[sl][h] - m_new);
-              l_i[sl][h] *= corr;
-              if (i > 0) {
-#pragma unroll
-                for (int j = 0; j < 8; ++j) o[sl][4 * j + 2 * h] *= corr, o[sl][4 * j + 2 * h + 1] *= corr;
-              }
-              m_ref[sl][h] = m_new;
-            }
-            float rs = 0.f;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float p0 = tc::ex2(fmaf(a[4 * j + 2 * h], c2s, -m_ref[sl][h]));
-              const float p1 = tc::ex2(fmaf(a[4 * j + 2 * h + 1], c2s, -m_ref[sl][h]));
-              rs += p0 + p1;
-              const __half2 hh = __floats2half2_rn(p0, p1);
-              // A fragment of k step j / 2: registers (row rq, k 2c), (row rq + 8, k 2c), (row rq, k 2c + 8), (row rq + 8, ...)
-              const int ri = 4 * (j >> 1) + 2 * (j & 1) + h;
-              ph[ri] = *reinterpret_cast<const uint32_t*>(&hh);
-              if (!SINGLE) {
-                const float2 hf = __half22float2(hh);
-                const __half2 ll = __floats2half2_rn(p0 - hf.x, p1 - hf.y);  // p - hi, exact
-                pl[ri] = *reinterpret_cast<const uint32_t*>(&ll);
-              }
-            }
-            l_i[sl][h] += rs;
-          }
-          tc::wg_fence();
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t advV = (uint64_t)(ks * 128);  // 16 key rows of 128 bytes
-            tc::wg_rs_n64_bt(o[sl], ph + 4 * ks, dVh + advV, (i | ks) ? 1u : 0u);
-            if (!SINGLE) {
-              tc::wg_rs_n64_bt(o[sl], ph + 4 * ks, dVl + advV, 1u);
-              tc::wg_rs_n64_bt(o[sl], pl + 4 * ks, dVh + advV, 1u);
-            }
-          }
-          tc::wg_commit();
-          tc::wg_wait<0>();
-        }
-        release(ge + i);                // K tile i (and V tile i - 2)
-        if (i + 2 >= T) release(gv);   // an entry without a K tile: V tile i was its only content
+        pv(i, 0);
+        tc::wg_wait<1>();  // QK(i, 1) has completed; softmax 1 overlaps PV(i, 0)
+        tc::fence_regs(s[1]);
+        release(ge + i);  // K tile i (and V tile i - 2)
+        softmax(i, 1);
+        pv(i, 1);
+        tc::wg_wait<0>();
+        tc::fence_regs(o[0]), tc::fence_regs(o[1]);
+        if (i + 2 >= T) release(gv);  // an entry without a K tile: V tile i was its only content
       }
       ge += T + 2;
       w += T;

@@ -1,8 +1,17 @@
-// Test-only entry points: run one GEMM through the SIMT fp32 kernel or the wgmma split-fp16 kernel (parity tests).
+// Test-only entry points: run one GEMM through the SIMT fp32 kernel or the wgmma split-fp16 kernel (parity tests), and one
+// batched launch of the split-fp16 flash attention kernel.
 #include <stdlib.h>
+
+#include <vector>
 
 #include "common.cuh"
 #include "linear.cuh"
+
+// fp32 -> fp16 hi plane and UNSCALED lo plane (the operand format of the attention kernel)
+static __global__ void k_split_unscaled_f32(const float* __restrict__ x, size_t n, __half* __restrict__ hi, __half* __restrict__ lo) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) tc::split_h_unscaled(x[i], hi[i], lo[i]);
+}
 
 extern "C" int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, const float* B, const float* bias, float* C,
                                   int M, int N, int K) {
@@ -54,5 +63,56 @@ extern "C" int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, con
   }
   dA.release(), dB.release(), dC.release(), dBias.release(), dBh.release(), dBl.release(), dErr.release();
   if (rc == B2_OK && err) rc = b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
+  return rc;
+}
+
+extern "C" int b2_debug_attention_host(b2_context* ctx, int np, const int* nq, const int* nk, int heads, float scale, int single,
+                                       const float* q, const float* k, const float* v, float* o) {
+  if (!ctx || !nq || !nk || !q || !k || !v || !o || np <= 0 || np > AP_MAXP || heads <= 0) return B2_ERR_ARG;
+  size_t eq = 0, ek = 0;  // elements of q (and o), of k (and v)
+  for (int z = 0; z < np; ++z) {
+    if (nq[z] <= 0 || nk[z] <= 0) return B2_ERR_ARG;
+    eq += (size_t)nq[z] * heads * 64, ek += (size_t)nk[z] * heads * 64;
+  }
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  const size_t n = eq + 2 * ek;  // q, k, v back to back
+  DevBuf dIn, dPl, dO, dErr, part, ml, cnt;
+  B2_CUDA(ctx, dIn.ensure(n * 4));
+  B2_CUDA(ctx, dPl.ensure(n * 2 * 2));
+  B2_CUDA(ctx, dO.ensure(eq * 2 * 2));
+  B2_CUDA(ctx, dErr.ensure(16));
+  float* in = dIn.as<float>();
+  B2_CUDA(ctx, cudaMemcpyAsync(in, q, eq * 4, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(in + eq, k, ek * 4, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(in + eq + ek, v, ek * 4, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemsetAsync(dErr.p, 0, 16, st));
+  __half *hi = dPl.as<__half>(), *lo = hi + n, *oh = dO.as<__half>(), *ol = oh + eq;
+  B2_LAUNCH(ctx, k_split_unscaled_f32, (unsigned)((n + 255) / 256), 256, 0, st, in, n, hi, lo);
+  B2_CUDA(ctx, cudaFuncSetAttribute(k_flash_ps<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AS_SMEM));
+  B2_CUDA(ctx, cudaFuncSetAttribute(k_flash_ps<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AS_SMEM));
+  FlashPlanes fp[AP_MAXP];
+  size_t qo = 0, ko = eq;
+  for (int z = 0; z < np; ++z) {
+    const size_t vo = ko + ek;
+    fp[z] = {{hi + qo, lo + qo}, {hi + ko, lo + ko}, {hi + vo, lo + vo}, {oh + qo, ol + qo}, nq[z], nk[z], heads, 64 * heads};
+    qo += (size_t)nq[z] * heads * 64, ko += (size_t)nk[z] * heads * 64;
+  }
+  TcWeights tw{nullptr, nullptr, nullptr, dErr.as<int>(), true};
+  tw.attn_part = &part, tw.attn_ml = &ml, tw.attn_cnt = &cnt, tw.sm_count = ctx->sm_count;
+  int rc = run_flash_planes(ctx, st, tw, fp, np, scale, single != 0);
+  std::vector<__half> ho(2 * eq);
+  int err = 0;
+  if (rc == B2_OK) {
+    cudaError_t e = cudaMemcpyAsync(ho.data(), oh, eq * 2 * 2, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&err, dErr.p, 4, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) rc = b2_fail(ctx, B2_ERR_CUDA, std::string("debug attention: ") + cudaGetErrorString(e));
+  }
+  if (rc == B2_OK)  // o = hi + lo * 2^-11 (the SINGLE variant writes lo = 0)
+    for (size_t i = 0; i < eq; ++i) o[i] = __half2float(ho[i]) + __half2float(ho[eq + i]) * tc::LO_INV;
+  dIn.release(), dPl.release(), dO.release(), dErr.release(), part.release(), ml.release(), cnt.release();
+  if (rc == B2_OK && err) rc = b2_fail(ctx, B2_ERR_STATE, "wgmma attention timed out on an mbarrier (kernel bug)");
   return rc;
 }

@@ -69,6 +69,12 @@ int64_t b2_debug_fetch(b2_context* ctx, const char* name, float* host_out, int64
  * kernel with fp32 B converted in-kernel, 2 = wgmma split-fp16 kernel with pre-split fp16 B.  K must be a multiple of 64. */
 int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, const float* B, const float* bias, float* C, int M, int N,
                        int K);
+/* Test-only: one batched launch of the wgmma flash attention on HOST fp32 buffers.  Problem z (0 <= z < np <= 16) has
+ * nq[z] queries, nk[z] keys and `heads` heads of 64: q as [heads][nq[z]][64], k and v as [heads][nk[z]][64] (head-major),
+ * each concatenated over z; o receives softmax(scale * q k^T) v as [nq[z]][64 * heads] per problem, concatenated over z.
+ * The operands are split into fp16 hi / lo planes on the device; single = 1 runs the fp16 variant (hi planes only). */
+int b2_debug_attention_host(b2_context* ctx, int np, const int* nq, const int* nk, int heads, float scale, int single,
+                            const float* q, const float* k, const float* v, float* o);
 
 /* ---- SuperPoint -------------------------------------------------------------------------------------------------- */
 /* `blob`: the 24 state-dict tensors in reference order (conv1a.weight, conv1a.bias, conv1b.weight, ... convDb.bias;
