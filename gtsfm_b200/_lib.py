@@ -49,6 +49,11 @@ class SiftImage(C.Structure):
                 ("out_desc", C.c_void_p), ("out_n", C.c_int), ("out_total", C.c_int)]
 
 
+class D2NetImage(C.Structure):
+    _fields_ = [("image", C.c_void_p), ("max_keypoints", C.c_int), ("out_xy", C.c_void_p), ("out_scores", C.c_void_p),
+                ("out_desc", C.c_void_p), ("out_n", C.c_int), ("out_total", C.c_int)]
+
+
 SIFT_CAPACITY = -5  # b2_sift_detect_host: more keypoints than the capacity; *out_n holds the count needed
 
 
@@ -109,6 +114,14 @@ SIGNATURES = {
     "b2_mnn_match_host": (_i, [_vp, _vp, _i, _vp, _i, _i, _i, C.c_double, _vp, _vp, _ip]),
     "b2_sift_detect_batched_dev": (_i, [_vp, C.POINTER(SiftImage), _i, _i, _i, _i, _sz, _vp]),
     "b2_sift_detect_host": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _ip]),
+    "b2_d2net_blob_floats": (_sz, []),
+    "b2_d2net_norm_table": (_i, [_vp]),
+    "b2_d2net_set_weights": (_i, [_vp, _vp, _sz]),
+    "b2_d2net_detect_batched_dev": (_i, [_vp, C.POINTER(D2NetImage), _i, _i, _i, _i, _sz, _vp]),
+    "b2_d2net_detect_host": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _ip, _ip]),
+    "b2_debug_conv_ps_host": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
+    "b2_debug_d2net_avgpool_host": (_i, [_vp, _vp, _i, _i, _vp]),
+    "b2_debug_d2net_rank_host": (_i, [_vp, _vp, _vp, _i, _i, _vp]),
 }
 
 

@@ -38,6 +38,7 @@ extern "C" void b2_destroy(b2_context* ctx) {
   mn_destroy(ctx);
   sf_destroy(ctx);
   ml_destroy(ctx);
+  d2_destroy(ctx);
   for (auto& b : ctx->stage_d) b.release();
   for (auto& b : ctx->stage_h) b.release();
   for (auto& e : ctx->fcache) e.buf.release();

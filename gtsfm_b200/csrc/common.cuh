@@ -89,6 +89,7 @@ struct NetVladState;
 struct MnnState;
 struct SiftState;
 struct MegaLocState;
+struct D2NetState;
 
 // Device copies of host feature arrays handed to the *_host matcher entry points.  GTSfM matches one image's (keypoints,
 // descriptors) against ~20-40 partners, always passing the same host arrays, so re-uploading 5 MB per image per pair is
@@ -126,6 +127,7 @@ struct b2_context {
   MnnState* mn = nullptr;
   SiftState* sf = nullptr;
   MegaLocState* ml = nullptr;
+  D2NetState* d2 = nullptr;
   // staging shared by the *_host entry points
   DevBuf stage_d[8];
   HostBuf stage_h[4];
@@ -192,6 +194,7 @@ void nv_destroy(b2_context* ctx);
 void mn_destroy(b2_context* ctx);
 void sf_destroy(b2_context* ctx);
 void ml_destroy(b2_context* ctx);
+void d2_destroy(b2_context* ctx);
 
 // shared device helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

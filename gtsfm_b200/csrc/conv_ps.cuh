@@ -18,22 +18,41 @@
 //     (columns 0-63: Ah Bh, 64-127: Ah Bl); Al x Bh^T (N = 64) goes to a third accumulator.
 //   * Warp 8 = TMA producer (3 plane buffers); warpgroup w (warps 4w .. 4w + 3) owns pixels 64w .. 64w + 63: MMAs, then
 //     hh + (hl + lh) * 2^-11, 2x2 max-pool (partners: row + 8 in the fragment, lane ^ 4), bias, ReLU, planes and / or fp32.
+//
+// DILATION (k_conv_ps<2>: D2-Net's conv4_x, 3x3 with dilation 2 and padding 2).  The template parameter D is the dilation
+// and the padding.  The halo box becomes {64, 8 + 2D, 16 + 2D}, the tap offsets are D pixels apart and the 8-row group stride
+// is (8 + 2D) x 128 bytes.  At D = 2 a box is 30 KiB: the 144 KiB weight block plus three of them would be 241 152 bytes, over
+// the 232 448-byte per-block limit, so the dilated instance keeps TWO activation buffers (210 432 bytes).  The producer then
+// runs at most one plane ahead of the consumers.  Measured effect (profiles/h100_d2net.json, H100 80GB HBM3 at a 400 W power
+// limit): one 512 -> 512 layer at 282 x 189 takes 1.659 ms on k_conv_ps<2> (two buffers, 20 x 12 halo) against 1.653 ms on
+// k_conv_ps<1> (three buffers, 18 x 10 halo), 151.6 vs 152.1 TFLOP/s: with Cin >= 256 every 64-channel chunk reloads its
+// 144 KiB of weights, and that wait, not the third activation buffer, sets the pace.  The alternative, a smaller tile, would
+// re-read more halo per output pixel.  D = 1 is the shipped SuperPoint / NetVLAD instance: every expression reduces to the
+// former constants and it compiles to the same SASS.
 #pragma once
 #include "common.cuh"
 #include "tma.cuh"
 
-constexpr int CP_TH = 16, CP_TW = 8;                 // output tile (pixels)
-constexpr int CP_HH = CP_TH + 2, CP_HW = CP_TW + 2;  // halo tile
-constexpr int CP_A_LOAD = CP_HH * CP_HW * 128;       // 23040 bytes per plane box
-constexpr int CP_A_BYTES = 23 * 1024;                // buffer pitch (1024-aligned)
-constexpr int CP_NA = 3;                             // activation plane buffers
-constexpr int CP_B_TAP = 128 * 128;                  // [Bh; Bl] x 64 K halves
+constexpr int CP_TH = 16, CP_TW = 8;  // output tile (pixels)
+constexpr int CP_B_TAP = 128 * 128;   // [Bh; Bl] x 64 K halves
 constexpr int CP_B_BYTES = 9 * CP_B_TAP;
 constexpr int CP_THREADS = 256 + 32;
-constexpr size_t CP_SMEM = (size_t)CP_B_BYTES + CP_NA * CP_A_BYTES + 1024 + 512;
+
+template <int D>  // dilation = padding
+struct CpGeom {
+  static constexpr int HH = CP_TH + 2 * D, HW = CP_TW + 2 * D;  // halo tile
+  static constexpr int A_LOAD = HH * HW * 128;                  // bytes per plane box (D = 1: 23040)
+  static constexpr int A_BYTES = (A_LOAD + 1023) / 1024 * 1024;  // buffer pitch (1024-aligned)
+  static constexpr int NA = D == 1 ? 3 : 2;                     // activation plane buffers
+  static constexpr size_t SMEM = (size_t)CP_B_BYTES + NA * A_BYTES + 1024 + 512;
+};
+constexpr int CP_HH = CpGeom<1>::HH, CP_HW = CpGeom<1>::HW;
+constexpr int CP_A_LOAD = CpGeom<1>::A_LOAD, CP_A_BYTES = CpGeom<1>::A_BYTES, CP_NA = CpGeom<1>::NA;
+constexpr size_t CP_SMEM = CpGeom<1>::SMEM;
+static_assert(CP_A_BYTES == 23 * 1024 && CpGeom<2>::SMEM <= 232448, "conv_ps shared-memory plan");
 
 struct ConvPsMaps {
-  CUtensorMap ah, al;  // activations: 3-D {C, W, H}, box {64, 10, 18}
+  CUtensorMap ah, al;  // activations: 3-D {C, W, H}, box {64, 8 + 2D, 16 + 2D}
   CUtensorMap wh, wl;  // weights: 2-D {9 * Cin, Cout}, box {64, 64}
 };
 struct ConvPsArgs {
@@ -63,16 +82,19 @@ __device__ __forceinline__ void cp_stamp(float* dbg, int slot) {
   dbg[blockIdx.x * 8 + slot] = (float)(tns & 0xFFFFFFull);
 }
 
+template <int D = 1>
 static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_constant__ ConvPsMaps maps, ConvPsArgs g) {
+  using Geo = CpGeom<D>;
+  constexpr int HW = Geo::HW, A_BYTES = Geo::A_BYTES, NA = Geo::NA;
   extern __shared__ unsigned char cp_raw[];
   const uint32_t raw = tc::smem_u32(cp_raw);
   const uint32_t smem0 = (raw + 1023u) & ~1023u;
   unsigned char* sm = cp_raw + (smem0 - raw);
   const uint32_t sB = smem0, sA = smem0 + CP_B_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + CP_B_BYTES + CP_NA * CP_A_BYTES);
-  uint64_t* fullA = bars;               // [CP_NA]
-  uint64_t* emptyA = fullA + CP_NA;     // [CP_NA] one arrival per consumer warp
-  uint64_t* fullB = emptyA + CP_NA;     // [9]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sm + CP_B_BYTES + NA * A_BYTES);
+  uint64_t* fullA = bars;               // [NA]
+  uint64_t* emptyA = fullA + NA;        // [NA] one arrival per consumer warp
+  uint64_t* fullB = emptyA + NA;        // [9]
   uint64_t* emptyB = fullB + 9;         // [9] one arrival per consumer warp
 
   const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
@@ -83,7 +105,7 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
 
   if (t == 0) {
     cp_stamp(g.dbg, 0);
-    for (int i = 0; i < CP_NA; ++i) tc::mbar_init(&fullA[i], 1), tc::mbar_init(&emptyA[i], 8);
+    for (int i = 0; i < NA; ++i) tc::mbar_init(&fullA[i], 1), tc::mbar_init(&emptyA[i], 8);
     for (int i = 0; i < 9; ++i) tc::mbar_init(&fullB[i], 1), tc::mbar_init(&emptyB[i], 8);
     tc::fence_mbar_init();
     tc::tma_prefetch_desc(&maps.ah);
@@ -112,10 +134,10 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
             ++bver;
           }
           for (int plane = 0; plane < 2; ++plane, ++a_cnt) {
-            const uint32_t buf = a_cnt % CP_NA, use = a_cnt / CP_NA;
+            const uint32_t buf = a_cnt % NA, use = a_cnt / NA;
             if (use > 0) ok = tc::mbar_wait(&emptyA[buf], (use - 1) & 1) && ok;
-            tc::mbar_expect_tx(&fullA[buf], CP_A_LOAD);
-            tc::tma_load_3d(sA + buf * CP_A_BYTES, plane ? &maps.al : &maps.ah, &fullA[buf], c * 64, x0 - 1, y0 - 1);
+            tc::mbar_expect_tx(&fullA[buf], Geo::A_LOAD);
+            tc::tma_load_3d(sA + buf * A_BYTES, plane ? &maps.al : &maps.ah, &fullA[buf], c * 64, x0 - D, y0 - D);
           }
         }
       }
@@ -134,14 +156,14 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
         const bool new_b = nchunk > 1 || bver == 0;
         if (new_b) ++bver;
         {  // hi plane: Ah x [Bh; Bl]^T
-          const uint32_t buf = a_cnt % CP_NA;
-          ok = tc::mbar_wait(&fullA[buf], (a_cnt / CP_NA) & 1) && ok;
-          const uint32_t base = sA + buf * CP_A_BYTES;
+          const uint32_t buf = a_cnt % NA;
+          ok = tc::mbar_wait(&fullA[buf], (a_cnt / NA) & 1) && ok;
+          const uint32_t base = sA + buf * A_BYTES;
           if (a_cnt == 0 && t == 0) cp_stamp(g.dbg, 2);
 #pragma unroll 1
           for (int tap = 0; tap < 9; ++tap) {
             if (new_b) ok = tc::mbar_wait(&fullB[tap], (bver - 1) & 1) && ok;
-            const uint64_t dA = tc::wg_desc_sw128(base + ((tap / 3 + wg * 8) * CP_HW + tap % 3) * 128, CP_HW * 128);
+            const uint64_t dA = tc::wg_desc_sw128(base + ((D * (tap / 3) + wg * 8) * HW + D * (tap % 3)) * 128, HW * 128);
             const uint64_t dB = tc::wg_desc_sw128(sB + tap * CP_B_TAP);
             tc::wg_fence();
 #pragma unroll
@@ -154,12 +176,12 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
           ++a_cnt;
         }
         {  // lo plane: Al x Bh^T into accl
-          const uint32_t buf = a_cnt % CP_NA;
-          ok = tc::mbar_wait(&fullA[buf], (a_cnt / CP_NA) & 1) && ok;
-          const uint32_t base = sA + buf * CP_A_BYTES;
+          const uint32_t buf = a_cnt % NA;
+          ok = tc::mbar_wait(&fullA[buf], (a_cnt / NA) & 1) && ok;
+          const uint32_t base = sA + buf * A_BYTES;
 #pragma unroll 1
           for (int tap = 0; tap < 9; ++tap) {
-            const uint64_t dA = tc::wg_desc_sw128(base + ((tap / 3 + wg * 8) * CP_HW + tap % 3) * 128, CP_HW * 128);
+            const uint64_t dA = tc::wg_desc_sw128(base + ((D * (tap / 3) + wg * 8) * HW + D * (tap % 3)) * 128, HW * 128);
             const uint64_t dB = tc::wg_desc_sw128(sB + tap * CP_B_TAP);
             tc::wg_fence();
 #pragma unroll
@@ -241,14 +263,88 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
   if (t == 0) cp_stamp(g.dbg, 6);
 }
 
-// NHWC fp16 activation plane [H][W][C] -> 3-D map {C, W, H}, box {64, CP_HW, CP_HH}, 128-byte swizzle, zero OOB fill
-static inline bool tma_map_nhwc_halo(CUtensorMap* out, const __half* base, int H, int W, int C) {
+// NHWC fp16 activation plane [H][W][C] -> 3-D map {C, W, H}, box {64, 8 + 2 dil, 16 + 2 dil}, 128-byte swizzle, zero OOB fill
+static inline bool tma_map_nhwc_halo(CUtensorMap* out, const __half* base, int H, int W, int C, int dil = 1) {
   PFN_encodeTiled enc = tma_encoder();
   if (!enc || !base) return false;
   cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H};
   cuuint64_t strides[2] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2};
-  cuuint32_t box[3] = {64, CP_HW, CP_HH};
+  cuuint32_t box[3] = {64, (cuuint32_t)(CP_TW + 2 * dil), (cuuint32_t)(CP_TH + 2 * dil)};
   cuuint32_t estr[3] = {1, 1, 1};
   return enc(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<__half*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+// ---- host helpers shared by the VGG-style networks on this kernel (NetVLAD, D2-Net) ----------------------------------------
+
+// Walks n layers of (OIHW 3x3 weight, bias) from `blob`: layer 0 (3 input channels, run by a SIMT kernel) -> w0 fp32
+// [tap][ci][co]; layers >= 1 -> `stage` at woff[l] as [co][tap * Cin + ci] (the implicit GEMM's K order); biases concatenated
+// at boff[l].  Returns the number of floats read.
+static size_t conv_ps_repack(const float* blob, int n, const int* CI, const int* CO, std::vector<float>& stage, std::vector<float>& bias,
+                             std::vector<float>& w0, size_t* woff, size_t* boff) {
+  size_t wtot = 0, btot = 0;
+  for (int l = 0; l < n; ++l) {
+    woff[l] = wtot, boff[l] = btot;
+    if (l) wtot += (size_t)CO[l] * 9 * CI[l];
+    btot += CO[l];
+  }
+  stage.assign(wtot, 0.f), bias.assign(btot, 0.f), w0.assign((size_t)27 * CO[0], 0.f);
+  size_t src = 0;
+  for (int l = 0; l < n; ++l) {
+    const int co = CO[l], ci = CI[l];
+    const float* w = blob + src;
+    if (l == 0) {
+      for (int o = 0; o < co; ++o)
+        for (int i = 0; i < ci; ++i)
+          for (int tp = 0; tp < 9; ++tp) w0[((size_t)tp * 3 + i) * co + o] = w[((size_t)o * ci + i) * 9 + tp];
+    } else {
+      float* d = stage.data() + woff[l];
+      for (int o = 0; o < co; ++o)
+        for (int tp = 0; tp < 9; ++tp)
+          for (int i = 0; i < ci; ++i) d[(size_t)o * 9 * ci + (size_t)tp * ci + i] = w[((size_t)o * ci + i) * 9 + tp];
+    }
+    src += (size_t)co * ci * 9;
+    std::copy(blob + src, blob + src + co, bias.begin() + boff[l]);
+    src += co;
+  }
+  return src;
+}
+
+// host fp32 [n] -> device split planes h / l (k_split_f32), staged through `tmp` in pieces of `piece` floats; synchronous
+static cudaError_t conv_ps_upload_planes(const float* host, size_t n, DevBuf& h, DevBuf& l, DevBuf& tmp, size_t piece) {
+  cudaError_t e;
+  if ((e = h.ensure(n * sizeof(__half))) != cudaSuccess || (e = l.ensure(n * sizeof(__half))) != cudaSuccess) return e;
+  for (size_t o = 0; o < n; o += piece) {
+    const size_t m = n - o < piece ? n - o : piece;
+    if ((e = cudaMemcpy(tmp.p, host + o, m * sizeof(float), cudaMemcpyHostToDevice)) != cudaSuccess) return e;
+    k_split_f32<<<(unsigned)((m + 255) / 256), 256>>>(tmp.as<float>(), m, h.as<__half>() + o, l.as<__half>() + o);
+    if ((e = cudaDeviceSynchronize()) != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
+
+// One layer on k_conv_ps<dil> (dil = padding, 1 or 2): input planes `ih` [H][W][Cin] with the lo plane right after the hi one,
+// weight planes wh / wl [Cout][9 Cin] -> output planes `oh` (lo after hi) and / or fp32 `of`, NHWC.  The caller has set the
+// kernel's dynamic shared-memory attribute (CP_SMEM / CpGeom<2>::SMEM).
+static int conv_ps_run(b2_context* ctx, cudaStream_t st, const __half* ih, int H, int W, int Cin, int Cout, int pool, int relu, int dil,
+                       const __half* wh, const __half* wl, const float* bias, __half* oh, float* of, int* err_flag, const char* model) {
+  if (dil != 1 && dil != 2) return b2_fail(ctx, B2_ERR_ARG, "conv_ps: dilation must be 1 or 2");
+  const int OH = pool ? H / 2 : H, OW = pool ? W / 2 : W;
+  ConvPsMaps maps;
+  const __half* il = ih + (size_t)H * W * Cin;
+  bool ok = tma_map_nhwc_halo(&maps.ah, ih, H, W, Cin, dil) && tma_map_nhwc_halo(&maps.al, il, H, W, Cin, dil) &&
+            tma_map_2d(&maps.wh, wh, Cout, 9 * Cin, 9 * Cin, 64) && tma_map_2d(&maps.wl, wl, Cout, 9 * Cin, 9 * Cin, 64);
+  if (!ok) return b2_fail(ctx, B2_ERR_CUDA, std::string("cuTensorMapEncodeTiled failed (") + model + " conv)");
+  ConvPsArgs a{};
+  a.H = H, a.W = W, a.Cin = Cin, a.Cout = Cout, a.pool = pool, a.relu = relu, a.bias = bias;
+  if (oh) a.Oh = oh, a.Ol = oh + (size_t)OH * OW * Cout;
+  a.Of = of, a.err_flag = err_flag;
+  const int nblk = Cout / 64, units = cdiv(W, CP_TW) * cdiv(H, CP_TH) * nblk;
+  int grid = ctx->sm_count < units ? ctx->sm_count : units;
+  grid -= grid % nblk;
+  b2_prof_work(ctx, dil == 1 ? "k_conv_ps<1>" : "k_conv_ps<2>", 2.0 * 9.0 * H * W * Cin * Cout);
+  if (dil == 1) B2_LAUNCH(ctx, k_conv_ps<1>, grid, CP_THREADS, CP_SMEM, st, maps, a);
+  else B2_LAUNCH(ctx, k_conv_ps<2>, grid, CP_THREADS, CpGeom<2>::SMEM, st, maps, a);
+  B2_CHECK_LAUNCH(ctx);
+  return B2_OK;
 }

@@ -183,46 +183,14 @@ extern "C" int b2_netvlad_set_weights(b2_context* ctx, const float* blob, size_t
   if (!ctx->nv) ctx->nv = new NetVladState();
   NetVladState* s = ctx->nv;
   // convolution weights: layer 0 as fp32 [tap][ci][co]; layers 1..12 as [co][tap * Cin + ci] planes; biases concatenated
-  size_t wtot = 0, btot = 0;
-  for (int l = 0; l < NV_NCONV; ++l) {
-    s->woff[l] = wtot, s->boff[l] = btot;
-    if (l) wtot += (size_t)NV_CO[l] * 9 * NV_CI[l];
-    btot += NV_CO[l];
-  }
-  std::vector<float> stage(wtot), b(btot), w0(27 * 64);
-  size_t src = 0;
-  for (int l = 0; l < NV_NCONV; ++l) {
-    const int co = NV_CO[l], ci = NV_CI[l];
-    const float* w = blob + src;
-    if (l == 0) {
-      for (int o = 0; o < co; ++o)
-        for (int i = 0; i < ci; ++i)
-          for (int tp = 0; tp < 9; ++tp) w0[((size_t)tp * 3 + i) * 64 + o] = w[((size_t)o * ci + i) * 9 + tp];
-    } else {
-      float* d = stage.data() + s->woff[l];
-      for (int o = 0; o < co; ++o)
-        for (int tp = 0; tp < 9; ++tp)
-          for (int i = 0; i < ci; ++i) d[(size_t)o * 9 * ci + (size_t)tp * ci + i] = w[((size_t)o * ci + i) * 9 + tp];
-    }
-    src += (size_t)co * ci * 9;
-    std::copy(blob + src, blob + src + co, b.begin() + s->boff[l]);
-    src += co;
-  }
+  std::vector<float> stage, b, w0;
+  size_t src = conv_ps_repack(blob, NV_NCONV, NV_CI, NV_CO, stage, b, w0, s->woff, s->boff);
+  const size_t btot = b.size();
   DevBuf tmp;
   const size_t piece = (size_t)64 << 20;  // floats per staging piece of the device-side split
   B2_CUDA(ctx, tmp.ensure(piece * sizeof(float)));
-  auto split_to = [&](const float* host, size_t n, DevBuf& h, DevBuf& l) -> cudaError_t {
-    cudaError_t e;
-    if ((e = h.ensure(n * sizeof(__half))) != cudaSuccess || (e = l.ensure(n * sizeof(__half))) != cudaSuccess) return e;
-    for (size_t o = 0; o < n; o += piece) {
-      const size_t m = n - o < piece ? n - o : piece;
-      if ((e = cudaMemcpy(tmp.p, host + o, m * sizeof(float), cudaMemcpyHostToDevice)) != cudaSuccess) return e;
-      k_split_f32<<<(unsigned)((m + 255) / 256), 256>>>(tmp.as<float>(), m, h.as<__half>() + o, l.as<__half>() + o);
-      if ((e = cudaDeviceSynchronize()) != cudaSuccess) return e;
-    }
-    return cudaSuccess;
-  };
-  B2_CUDA(ctx, split_to(stage.data(), wtot, s->wh, s->wl));
+  auto split_to = [&](const float* host, size_t n, DevBuf& h, DevBuf& l) { return conv_ps_upload_planes(host, n, h, l, tmp, piece); };
+  B2_CUDA(ctx, split_to(stage.data(), stage.size(), s->wh, s->wl));
   B2_CUDA(ctx, s->w0.ensure(w0.size() * sizeof(float)));
   B2_CUDA(ctx, cudaMemcpy(s->w0.p, w0.data(), w0.size() * sizeof(float), cudaMemcpyHostToDevice));
   B2_CUDA(ctx, s->bias.ensure(btot * sizeof(float)));
@@ -241,7 +209,7 @@ extern "C" int b2_netvlad_set_weights(b2_context* ctx, const float* blob, size_t
   tmp.release();
   B2_CUDA(ctx, s->errflag.ensure(16));
   B2_CUDA(ctx, cudaMemset(s->errflag.p, 0, 16));
-  B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CP_SMEM));
+  B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CP_SMEM));
   B2_CUDA(ctx, cudaFuncSetAttribute(k_gemm_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GW_SMEM));
   s->loaded = true;
   return B2_OK;
@@ -249,27 +217,9 @@ extern "C" int b2_netvlad_set_weights(b2_context* ctx, const float* blob, size_t
 
 static int nv_conv(b2_context* ctx, cudaStream_t st, const DevBuf& in, int l, int H, int W, DevBuf* out_planes, float* out_f32) {
   NetVladState* s = ctx->nv;
-  const int Cin = NV_CI[l], Cout = NV_CO[l], pool = NV_POOL[l];
-  const int OH = pool ? H / 2 : H, OW = pool ? W / 2 : W;
-  ConvPsMaps maps;
-  const __half* ih = in.as<__half>();
-  const __half* il = ih + (size_t)H * W * Cin;
-  const __half* wh = s->wh.as<__half>() + s->woff[l];
-  const __half* wl = s->wl.as<__half>() + s->woff[l];
-  bool ok = tma_map_nhwc_halo(&maps.ah, ih, H, W, Cin) && tma_map_nhwc_halo(&maps.al, il, H, W, Cin) &&
-            tma_map_2d(&maps.wh, wh, Cout, 9 * Cin, 9 * Cin, 64) && tma_map_2d(&maps.wl, wl, Cout, 9 * Cin, 9 * Cin, 64);
-  if (!ok) return b2_fail(ctx, B2_ERR_CUDA, "cuTensorMapEncodeTiled failed (netvlad conv)");
-  ConvPsArgs a{};
-  a.H = H, a.W = W, a.Cin = Cin, a.Cout = Cout, a.pool = pool, a.relu = l != NV_NCONV - 1, a.bias = s->bias.as<float>() + s->boff[l];
-  if (out_planes) a.Oh = out_planes->as<__half>(), a.Ol = a.Oh + (size_t)OH * OW * Cout;
-  a.Of = out_f32, a.err_flag = s->errflag.as<int>();
-  const int nblk = Cout / 64, units = cdiv(W, CP_TW) * cdiv(H, CP_TH) * nblk;
-  int grid = ctx->sm_count < units ? ctx->sm_count : units;
-  grid -= grid % nblk;
-  b2_prof_work(ctx, "k_conv_ps", 2.0 * 9.0 * H * W * Cin * Cout);
-  B2_LAUNCH(ctx, k_conv_ps, grid, CP_THREADS, CP_SMEM, st, maps, a);
-  B2_CHECK_LAUNCH(ctx);
-  return B2_OK;
+  return conv_ps_run(ctx, st, in.as<__half>(), H, W, NV_CI[l], NV_CO[l], NV_POOL[l], l != NV_NCONV - 1, 1, s->wh.as<__half>() + s->woff[l],
+                     s->wl.as<__half>() + s->woff[l], s->bias.as<float>() + s->boff[l], out_planes ? out_planes->as<__half>() : nullptr, out_f32,
+                     s->errflag.as<int>(), "netvlad");
 }
 
 // images: DEVICE [B][3][H][W] fp32 in [0, 1] (what the reference's batch transform produces); out: DEVICE [B][4096] fp32

@@ -651,7 +651,7 @@ static int sp_conv3x3_tc(b2_context* ctx, cudaStream_t st, const DevBuf& in, int
   int grid = ctx->sm_count < units ? ctx->sm_count : units;
   grid -= grid % nblk;  // a CTA keeps one 64-channel block of the weights resident: CTA c serves block c % nblk
   b2_prof_work(ctx, "k_conv_ps", 2.0 * 9.0 * H * W * Cin * Cout);
-  B2_LAUNCH(ctx, k_conv_ps, grid, CP_THREADS, CP_SMEM, st, maps, a);
+  B2_LAUNCH(ctx, k_conv_ps<1>, grid, CP_THREADS, CP_SMEM, st, maps, a);
   B2_CHECK_LAUNCH(ctx);
   return B2_OK;
 }
@@ -751,7 +751,7 @@ extern "C" int b2_superpoint_set_weights(b2_context* ctx, const float* blob, siz
     B2_CHECK_LAUNCH(ctx);
     B2_CUDA(ctx, cudaDeviceSynchronize());
     tmp.release();
-    B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CP_SMEM));
+    B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CP_SMEM));
     B2_CUDA(ctx, cudaFuncSetAttribute(k_gemm_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GW_SMEM));
     s->use_tc = !b2_force_simt(ctx) && tma_encoder() != nullptr;
   }

@@ -1,4 +1,4 @@
-"""SuperPoint and SIFT detector-descriptor plugins.
+"""SuperPoint, SIFT and D2-Net detector-descriptor plugins.
 
 Drop-in for gtsfm/frontend/detector_descriptor/superpoint.py:32-93 (`SuperPointDetectorDescriptor`): same constructor
 arguments, same `detect_and_describe(image) -> (Keypoints, (N, 256) float32)` contract, same post-processing order
@@ -13,6 +13,9 @@ survive the host-side mask / top-k selection, instead of for every detection (id
 `B200SIFTDetectorDescriptor` is the drop-in for gtsfm/frontend/detector_descriptor/sift.py:24-55 (`SIFTDetectorDescriptor`):
 cv2.SIFT_create() with its defaults, restated in csrc/sift.cu.  Its one deliberate difference: an image without keypoints
 gives (empty Keypoints, (0, 128) float32) where the reference raises a TypeError.
+
+`B200D2NetDetectorDescriptor` is the drop-in for gtsfm/frontend/detector_descriptor/d2net.py (`D2NetDetDesc`), single scale, restated
+in csrc/d2net.cu.
 """
 from __future__ import annotations
 
@@ -252,3 +255,143 @@ class B200SIFTDetectorDescriptor(DetectorDescriptorBase):
                               responses=kp["response"].astype(np.float64))
         keypoints, sel = keypoints.get_top_k(self.max_keypoints)  # gtsfm/.../sift.py:53-54
         return keypoints, desc[sel].astype(np.float32)
+
+
+D2NET_DESC_DIM = 512
+D2NET_MAX_EDGE_PX, D2NET_MAX_SUM_EDGES_PX = 1600, 2800  # gtsfm/.../d2net.py:22-23
+D2NET_MODEL_SUBPATH = Path("thirdparty") / "d2net" / "weights" / "d2_tf.pth"
+
+
+def default_d2net_model_path() -> Path:
+    """The reference's default (gtsfm/.../d2net.py:29): thirdparty/d2net/weights/d2_tf.pth under the root of the GTSfM checkout,
+    found from the importable `gtsfm` package.  Without one, the same relative path under the working directory."""
+    try:
+        import importlib.util
+
+        spec = importlib.util.find_spec("gtsfm")
+    except (ImportError, ValueError):
+        spec = None
+    if spec is not None and spec.origin:
+        return Path(spec.origin).resolve().parent.parent / D2NET_MODEL_SUBPATH
+    return Path.cwd() / D2NET_MODEL_SUBPATH
+
+
+class D2NetEngine:
+    """Single-scale D2-Net on csrc/d2net.cu: host calls and batched device calls (descriptors left on the GPU for
+    TwoWayEngine.match_batched_dev)."""
+
+    def __init__(self, state_dict, device: int = 0, ctx: Optional[_lib.Context] = None):
+        self.ctx = ctx or _lib.Context(device)
+        blob = weights.pack_d2net(weights.load_d2net(state_dict))
+        self.ctx.check(self.ctx.lib.b2_d2net_set_weights(self.ctx.handle, _lib.ptr(blob), blob.size), "d2net_set_weights")
+        self.lock = threading.RLock()
+
+    @staticmethod
+    def check_image(img: np.ndarray) -> np.ndarray:
+        img = np.ascontiguousarray(img)
+        if img.dtype != np.uint8:
+            raise ValueError("D2-Net takes uint8 images")
+        if img.ndim not in (2, 3) or (img.ndim == 3 and img.shape[2] not in (1, 3)):
+            raise ValueError("D2-Net takes gray (H, W) / (H, W, 1) or RGB (H, W, 3) images")
+        h, w = img.shape[:2]
+        if max(h, w) > D2NET_MAX_EDGE_PX or h + w > D2NET_MAX_SUM_EDGES_PX:
+            raise ValueError(f"image {h}x{w} is over D2-Net's size limits (longer edge 1600, edges summing to 2800): the reference "
+                             "resizes such images with scipy.misc.imresize, which current scipy no longer has")
+        if min(h, w) < 8:
+            raise ValueError("D2-Net needs images of at least 8 x 8 pixels")
+        return img
+
+    def detect_and_describe(self, image: np.ndarray, max_keypoints: int = 5000):
+        """Host uint8 image -> ((K, 2) float32 (x, y), (K,) float32 scores, (K, 512) float32 descriptors), score-ordered."""
+        img = self.check_image(image)
+        h, w = img.shape[:2]
+        ch = 1 if img.ndim == 2 else img.shape[2]
+        xy = np.empty((max_keypoints, 2), np.float32)
+        sc = np.empty(max_keypoints, np.float32)
+        desc = np.empty((max_keypoints, D2NET_DESC_DIM), np.float32)
+        n, total = _lib.C.c_int(0), _lib.C.c_int(0)
+        with self.lock:
+            rc = self.ctx.lib.b2_d2net_detect_host(self.ctx.handle, _lib.ptr(img), h, w, ch, int(max_keypoints), _lib.ptr(xy), _lib.ptr(sc),
+                                                   _lib.ptr(desc), _lib.C.byref(n), _lib.C.byref(total))
+        self.ctx.check(rc, "d2net_detect_host")
+        k = n.value
+        return xy[:k].copy(), sc[:k].copy(), desc[:k].copy()
+
+    def extract_many(self, images, max_keypoints: int = 5000):
+        """images: same-shape CUDA uint8 tensors (H, W) / (H, W, 1) / (H, W, 3), rows may be pitched.  -> list of
+        ((n, 2) xy, (n,) scores, (n, 512) descriptors) CUDA float32 tensors and the count before the top-k."""
+        import torch
+
+        if len(images) == 0:
+            return []
+        shape = tuple(images[0].shape)
+        if any(tuple(x.shape) != shape for x in images):
+            raise ValueError("extract_many takes images of one shape")
+        h, w = shape[:2]
+        ch = 1 if len(shape) == 2 else shape[2]
+        self.check_image(np.empty((h, w, ch), np.uint8))  # the size limits, before any device work
+        dev = images[0].device
+        out = []
+        with self.lock:
+            for c0 in range(0, len(images), 64):
+                idx = range(c0, min(len(images), c0 + 64))
+                st = (_lib.D2NetImage * len(idx))()
+                keep, pitch = [], None
+                for s, i in enumerate(idx):
+                    x = images[i]
+                    if x.dtype != torch.uint8:
+                        raise ValueError("images must be uint8")
+                    if x.stride(-1) != 1 or (x.dim() == 3 and x.stride(1) != ch):
+                        x = x.contiguous()
+                    if pitch is None:
+                        pitch = x.stride(0)
+                    elif x.stride(0) != pitch:
+                        x = x.contiguous()
+                        if x.stride(0) != pitch:
+                            raise ValueError("images of one call must share a row pitch")
+                    xy = torch.empty((max_keypoints, 2), dtype=torch.float32, device=dev)
+                    sc = torch.empty(max_keypoints, dtype=torch.float32, device=dev)
+                    desc = torch.empty((max_keypoints, D2NET_DESC_DIM), dtype=torch.float32, device=dev)
+                    keep.append((x, xy, sc, desc))
+                    st[s] = _lib.D2NetImage(x.data_ptr(), int(max_keypoints), xy.data_ptr(), sc.data_ptr(), desc.data_ptr(), 0, 0)
+                stream = torch.cuda.current_stream(dev).cuda_stream
+                rc = self.ctx.lib.b2_d2net_detect_batched_dev(self.ctx.handle, st, len(idx), h, w, ch, int(pitch), _lib.C.c_void_p(stream))
+                self.ctx.check(rc, "d2net_detect_batched_dev")
+                for s, (_, xy, sc, desc) in enumerate(keep):
+                    n = st[s].out_n
+                    out.append((xy[:n], sc[:n], desc[:n], st[s].out_total))
+        return out
+
+
+class B200D2NetDetectorDescriptor(DetectorDescriptorBase):
+    """Single-scale D2-Net on hand-written sm_90a kernels: the drop-in for gtsfm/.../d2net.py `D2NetDetDesc`.
+
+    Same outputs: float32 (x, y) coordinates and responses (no scales), (K, 512) float32 descriptors, the max_keypoints best
+    scores first.  Like the reference it ignores `image.mask` and runs single-scale only.  Images whose longer edge is over
+    1600 pixels or whose edges sum to over 2800 raise ValueError: the reference resizes them with scipy.misc.imresize, which
+    its pinned scipy no longer has, so it cannot process them either.  RGBA and non-uint8 input raise ValueError."""
+
+    def __init__(self, max_keypoints: int = 5000, model_path: Union[Path, str, dict, None] = None, device: int = 0) -> None:
+        super().__init__(max_keypoints=max_keypoints)
+        model_path = default_d2net_model_path() if model_path is None else model_path
+        if not isinstance(model_path, dict) and not Path(model_path).exists():
+            raise FileNotFoundError(  # same failure as gtsfm/.../d2net.py:46-50
+                f"D2-Net weights not found at {model_path}. Please run 'bash scripts/download_model_weights.sh' from the repo root.")
+        self._model_path = model_path
+        self._device = device
+        self._engine: Optional[D2NetEngine] = None  # lazy, never pickled
+
+    def __getstate__(self):
+        st = dict(self.__dict__)
+        st["_engine"] = None
+        return st
+
+    def _ensure_engine(self) -> D2NetEngine:
+        if self._engine is None:
+            self._engine = D2NetEngine(self._model_path, self._device)
+        return self._engine
+
+    def detect_and_describe(self, image: Image) -> Tuple[Keypoints, np.ndarray]:
+        arr = D2NetEngine.check_image(image.value_array)
+        xy, sc, desc = self._ensure_engine().detect_and_describe(arr, self.max_keypoints)
+        return Keypoints(coordinates=xy, responses=sc), desc

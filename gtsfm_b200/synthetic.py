@@ -231,6 +231,21 @@ def megaloc_state_dict(seed: int = 5) -> Dict[str, np.ndarray]:
     return sd
 
 
+D2NET_CONVS = [(0, 3, 64), (2, 64, 64), (5, 64, 128), (7, 128, 128), (10, 128, 256), (12, 256, 256), (14, 256, 256), (17, 256, 512),
+               (19, 512, 512), (21, 512, 512)]  # (index in dense_feature_extraction.model, Cin, Cout)
+
+
+def d2net_state_dict(seed: int = 7) -> Dict[str, np.ndarray]:
+    """Seeded He-normal weights with small biases, named as the reference's d2_tf.pth `model` state dict
+    (thirdparty/d2net/lib/model_test.py: dense_feature_extraction.model.{0,2,...,21}).  No checkpoint can be downloaded offline."""
+    rng = np.random.default_rng(seed)
+    sd: Dict[str, np.ndarray] = {}
+    for idx, ci, co in D2NET_CONVS:
+        sd[f"dense_feature_extraction.model.{idx}.weight"] = (rng.standard_normal((co, ci, 3, 3)) * np.sqrt(2.0 / (9 * ci))).astype(np.float32)
+        sd[f"dense_feature_extraction.model.{idx}.bias"] = (0.01 * rng.standard_normal(co)).astype(np.float32)
+    return sd
+
+
 def save_pth(state: Dict[str, np.ndarray], path) -> None:
     """Write a state dict in the reference's checkpoint format (torch.save of name -> tensor)."""
     import torch

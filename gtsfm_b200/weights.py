@@ -196,3 +196,28 @@ def pack_megaloc(sd: StateDict) -> np.ndarray:
     blob = _pack(sd, MEGALOC_ORDER)
     assert blob.size == MEGALOC_BLOB_FLOATS, blob.size
     return blob
+
+
+# ---- D2-Net (thirdparty/d2net/lib/model_test.py: DenseFeatureExtractionModule, VGG16 up to conv4_3, the last block dilated) --------
+D2NET_CONV_IDX = [0, 2, 5, 7, 10, 12, 14, 17, 19, 21]  # Conv2d modules of dense_feature_extraction.model
+D2NET_ORDER: List[str] = [f"dense_feature_extraction.model.{i}.{p}" for i in D2NET_CONV_IDX for p in ("weight", "bias")]
+D2NET_BLOB_FLOATS = 7635264
+
+
+def load_d2net(src: Union[str, Path, StateDict]) -> StateDict:
+    """The reference's `d2_tf.pth` (torch.save of {"model": state dict}, model_test.py:73-77) or an in-memory state dict."""
+    if isinstance(src, dict):
+        return load_state_dict(src.get("model", src))
+    path = Path(src)
+    if not path.exists():
+        raise FileNotFoundError(f"weights not found at {path}")
+    import torch
+
+    ck = torch.load(str(path), map_location="cpu")
+    return {k: v.detach().cpu().numpy() for k, v in ck["model"].items()}
+
+
+def pack_d2net(sd: StateDict) -> np.ndarray:
+    blob = _pack(sd, D2NET_ORDER)
+    assert blob.size == D2NET_BLOB_FLOATS, blob.size
+    return blob

@@ -327,6 +327,45 @@ int b2_sift_detect_batched_dev(b2_context* ctx, b2_sift_image* images, int n_ima
 int b2_sift_detect_host(b2_context* ctx, const uint8_t* image, int height, int width, int channels, const uint8_t* mask,
                         b2_sift_keypoint* out_keypoints, uint8_t* out_desc, int capacity, int* out_n);
 
+/* ---- D2-Net detector-descriptor (gtsfm/frontend/detector_descriptor/d2net.py, thirdparty/d2net/lib/{model_test,pyramid,utils}.py)
+ * Single scale, use_relu, 'torch' preprocessing: VGG16 conv1_1 .. conv3_3, AvgPool2d(2, stride=1), conv4_1 .. conv4_3 with
+ * dilation 2 -> dense map (H/4 - 1) x (W/4 - 1) x 512; HardDetectionModule (edge threshold 5), HandcraftedLocalizationModule,
+ * bilinear descriptors, F.normalize.  Keypoints come ordered by score descending, ties in the reference's torch.nonzero order
+ * (channel, row, column); the first max_keypoints are kept.  Images are uint8 H x W x {1, 3} interleaved (gray is used for all three
+ * channels, as the reference repeats it); 8 <= H, W, max(H, W) <= 1600 and H + W <= 2800 (the reference resizes larger
+ * images, which its scipy no longer can), otherwise -2.  With the "force_simt" option set every b2_d2net_* call that uses the
+ * GPU returns -3. */
+/* Floats of the weight blob: the 20 tensors dense_feature_extraction.model.{0,2,5,7,10,12,14,17,19,21}.{weight,bias} of the
+ * d2_tf.pth checkpoint, in that order, each in its checkpoint layout (gtsfm_b200.weights.D2NET_ORDER). */
+size_t b2_d2net_blob_floats(void);
+/* HOST [3][256]: the float32 value the reference's preprocess_image('torch') gives byte u of channel c, at [c][u]. */
+int b2_d2net_norm_table(float* out);
+int b2_d2net_set_weights(b2_context* ctx, const float* blob, size_t n_floats);
+typedef struct b2_d2net_image {
+  const uint8_t* image; /* DEVICE image, row pitch as passed to the call */
+  int max_keypoints;    /* >= 0: keypoints kept (capacity of the outputs) */
+  float* out_xy;        /* DEVICE [max_keypoints][2] (x, y) in input pixels */
+  float* out_scores;    /* DEVICE [max_keypoints] */
+  float* out_desc;      /* DEVICE [max_keypoints][512], unit length */
+  int out_n;            /* written on the HOST struct: keypoints written */
+  int out_total;        /* written on the HOST struct: keypoints before the top-k */
+} b2_d2net_image;
+/* Up to 64 same-shape images, one after another through the network; counts stay on the device and `stream` is synchronised once. */
+int b2_d2net_detect_batched_dev(b2_context* ctx, b2_d2net_image* images, int n_images, int height, int width, int channels,
+                                size_t pitch, void* stream);
+/* HOST pointers, dense image: the max_keypoints best keypoints, ordered; out_total (may be NULL) = the count before the top-k. */
+int b2_d2net_detect_host(b2_context* ctx, const uint8_t* image, int height, int width, int channels, int max_keypoints,
+                         float* out_xy, float* out_scores, float* out_desc, int* out_n, int* out_total);
+/* Test-only entry points (tests/test_d2net_kernels_gpu.py), HOST pointers:
+ *  b2_debug_conv_ps_host: one k_conv_ps<dilation> layer (dilation 1 or 2, padding = dilation, Cin and Cout multiples of 64) on fp32 NHWC
+ *    [H][W][Cin] with OIHW weights [Cout][Cin][3][3] and bias, optional ReLU -> fp32 NHWC [H][W][Cout];
+ *  b2_debug_d2net_avgpool_host: the AvgPool2d(2, stride=1) kernel on fp32 NHWC [H][W][256] -> [H - 1][W - 1][256] (hi + lo planes);
+ *  b2_debug_d2net_rank_host: the keypoint ordering on n candidates (score, c, i, j) -> order[r] = candidate of rank r < min(n, max_k). */
+int b2_debug_conv_ps_host(b2_context* ctx, int dilation, const float* in, int height, int width, int cin, int cout, const float* weight,
+                          const float* bias, int relu, float* out);
+int b2_debug_d2net_avgpool_host(b2_context* ctx, const float* in, int height, int width, float* out);
+int b2_debug_d2net_rank_host(b2_context* ctx, const float* scores, const int* cij, int n, int max_k, int* order);
+
 #ifdef __cplusplus
 }
 #endif
