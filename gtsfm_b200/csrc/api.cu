@@ -39,9 +39,6 @@ extern "C" void b2_destroy(b2_context* ctx) {
   sf_destroy(ctx);
   ml_destroy(ctx);
   d2_destroy(ctx);
-  for (auto& b : ctx->stage_d) b.release();
-  for (auto& b : ctx->stage_h) b.release();
-  for (auto& e : ctx->fcache) e.buf.release();
   for (cudaEvent_t e : ctx->prof.ev) cudaEventDestroy(e);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   delete ctx;

@@ -20,9 +20,15 @@
 #define B2_ERR_MNN_RATIO -4  // ratio test requested with fewer than 2 descriptors on one side (include/gtsfm_b200.h)
 #define B2_SIFT_CAPACITY -5  // b2_sift_detect_host: more keypoints than the caller's capacity, *out_n = the count needed
 
+// DevBuf / HostBuf own their allocation: the destructor frees it, so a buffer in a model state is freed when the state is
+// deleted and a local one on every return path.  Not copyable (two owners would free twice).
 struct DevBuf {  // grow-only device allocation
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { release(); }
   cudaError_t ensure(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
     if (p) cudaFree(p);
@@ -45,6 +51,10 @@ struct DevBuf {  // grow-only device allocation
 struct HostBuf {  // grow-only pinned host allocation
   void* p = nullptr;
   size_t cap = 0;
+  HostBuf() = default;
+  HostBuf(const HostBuf&) = delete;
+  HostBuf& operator=(const HostBuf&) = delete;
+  ~HostBuf() { release(); }
   cudaError_t ensure(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
     if (p) cudaFreeHost(p);
@@ -132,6 +142,7 @@ struct b2_context {
   DevBuf stage_d[8];
   HostBuf stage_h[4];
   FeatCacheEntry fcache[B2_FEAT_CACHE_SLOTS];
+  DevBuf resize_taps;  // b2_image_resize_dev: x then y cubic tap tables of the call in flight
   uint64_t fstamp = 0;
   int fcache_on = -1;          // -1 = read B2_FEATURE_CACHE on first use
   uint64_t h2d_bytes = 0;      // bytes the *_host entry points that track them actually copied

@@ -50,12 +50,7 @@ struct D2NetState {
 };
 
 void d2_destroy(b2_context* ctx) {
-  if (!ctx->d2) return;
-  D2NetState* s = ctx->d2;
-  DevBuf* bufs[] = {&s->w0, &s->bias, &s->wh, &s->wl, &s->table, &s->errflag, &s->actA, &s->actB, &s->f3, &s->dense, &s->cand,
-                    &s->order, &s->counts};
-  for (DevBuf* b : bufs) b->release();
-  delete s;
+  delete ctx->d2;
   ctx->d2 = nullptr;
 }
 
@@ -412,24 +407,19 @@ extern "C" int b2_d2net_detect_host(b2_context* ctx, const uint8_t* image, int h
   B2_CUDA(ctx, xy_d.ensure(k * 2 * sizeof(float)));
   B2_CUDA(ctx, sc_d.ensure(k * sizeof(float)));
   B2_CUDA(ctx, de_d.ensure(k * D2_D * sizeof(float)));
-  int rc = B2_ERR_CUDA;
   b2_d2net_image im{img_d.as<uint8_t>(), max_keypoints, xy_d.as<float>(), sc_d.as<float>(), de_d.as<float>(), 0, 0};
-  if (cudaMemcpy(img_d.p, image, nin, cudaMemcpyHostToDevice) == cudaSuccess) {
-    rc = b2_d2net_detect_batched_dev(ctx, &im, 1, height, width, channels, (size_t)width * channels, ctx->stream);
-    if (rc == B2_OK) {
-      const size_t n = (size_t)im.out_n;
-      if (n && (cudaMemcpy(out_xy, xy_d.p, n * 2 * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess ||
-          cudaMemcpy(out_scores, sc_d.p, n * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess ||
-          cudaMemcpy(out_desc, de_d.p, n * D2_D * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess))
-        rc = b2_fail(ctx, B2_ERR_CUDA, "copy of the keypoints failed");
-      *out_n = im.out_n;
-      if (out_total) *out_total = im.out_total;
-    }
-  } else {
-    b2_fail(ctx, B2_ERR_CUDA, "copy of the image failed");
+  B2_CUDA(ctx, cudaMemcpy(img_d.p, image, nin, cudaMemcpyHostToDevice));
+  const int rc = b2_d2net_detect_batched_dev(ctx, &im, 1, height, width, channels, (size_t)width * channels, ctx->stream);
+  if (rc != B2_OK) return rc;
+  const size_t n = (size_t)im.out_n;
+  if (n) {
+    B2_CUDA(ctx, cudaMemcpy(out_xy, xy_d.p, n * 2 * sizeof(float), cudaMemcpyDeviceToHost));
+    B2_CUDA(ctx, cudaMemcpy(out_scores, sc_d.p, n * sizeof(float), cudaMemcpyDeviceToHost));
+    B2_CUDA(ctx, cudaMemcpy(out_desc, de_d.p, n * D2_D * sizeof(float), cudaMemcpyDeviceToHost));
   }
-  img_d.release(), xy_d.release(), sc_d.release(), de_d.release();
-  return rc;
+  *out_n = im.out_n;
+  if (out_total) *out_total = im.out_total;
+  return B2_OK;
 }
 
 // ---- test-only entry points: the dilated convolution, the average pool and the ordering, each on its own ---------------------
@@ -455,31 +445,30 @@ extern "C" int b2_debug_conv_ps_host(b2_context* ctx, int dilation, const float*
       for (int i = 0; i < Cin; ++i) wk[(size_t)o * 9 * Cin + (size_t)tp * Cin + i] = weight[((size_t)o * Cin + i) * 9 + tp];
   const size_t nin = (size_t)H * W * Cin, nout = (size_t)H * W * Cout;
   DevBuf tmp, wh, wl, ip, il, b, o, err;
-  auto done = [&](int rc) {
-    DevBuf* bufs[] = {&tmp, &wh, &wl, &ip, &il, &b, &o, &err};
-    for (DevBuf* x : bufs) x->release();
-    return rc;
-  };
   const size_t big = nin > wk.size() ? nin : wk.size();
   // ip holds both planes (hi, then lo): allocated at full size first, so the upload below does not reallocate it
-  if (ip.ensure(2 * nin * sizeof(__half)) || tmp.ensure(big * sizeof(float)) || conv_ps_upload_planes(wk.data(), wk.size(), wh, wl, tmp, big) ||
-      conv_ps_upload_planes(in, nin, ip, il, tmp, big) || b.ensure(Cout * sizeof(float)) || o.ensure(nout * sizeof(float)) || err.ensure(16) ||
-      cudaMemcpy(b.p, bias, Cout * sizeof(float), cudaMemcpyHostToDevice) || cudaMemset(err.p, 0, 16))
-    return done(b2_fail(ctx, B2_ERR_CUDA, "debug conv: allocation or copy failed"));
+  B2_CUDA(ctx, ip.ensure(2 * nin * sizeof(__half)));
+  B2_CUDA(ctx, tmp.ensure(big * sizeof(float)));
+  B2_CUDA(ctx, conv_ps_upload_planes(wk.data(), wk.size(), wh, wl, tmp, big));
+  B2_CUDA(ctx, conv_ps_upload_planes(in, nin, ip, il, tmp, big));
+  B2_CUDA(ctx, b.ensure(Cout * sizeof(float)));
+  B2_CUDA(ctx, o.ensure(nout * sizeof(float)));
+  B2_CUDA(ctx, err.ensure(16));
+  B2_CUDA(ctx, cudaMemcpy(b.p, bias, Cout * sizeof(float), cudaMemcpyHostToDevice));
+  B2_CUDA(ctx, cudaMemset(err.p, 0, 16));
   // the kernel reads the lo plane right after the hi one
-  if (cudaMemcpy(ip.as<__half>() + nin, il.p, nin * sizeof(__half), cudaMemcpyDeviceToDevice))
-    return done(b2_fail(ctx, B2_ERR_CUDA, "debug conv: plane copy failed"));
-  if (cudaFuncSetAttribute(k_conv_ps<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CP_SMEM) ||
-      cudaFuncSetAttribute(k_conv_ps<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CpGeom<2>::SMEM))
-    return done(b2_fail(ctx, B2_ERR_CUDA, "debug conv: shared-memory attribute"));
-  int rc = conv_ps_run(ctx, ctx->stream, ip.as<__half>(), H, W, Cin, Cout, 0, relu, dilation, wh.as<__half>(), wl.as<__half>(), b.as<float>(),
-                       nullptr, o.as<float>(), err.as<int>(), "debug");
-  if (rc) return done(rc);
+  B2_CUDA(ctx, cudaMemcpy(ip.as<__half>() + nin, il.p, nin * sizeof(__half), cudaMemcpyDeviceToDevice));
+  B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CP_SMEM));
+  B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CpGeom<2>::SMEM));
+  const int rc = conv_ps_run(ctx, ctx->stream, ip.as<__half>(), H, W, Cin, Cout, 0, relu, dilation, wh.as<__half>(), wl.as<__half>(), b.as<float>(),
+                             nullptr, o.as<float>(), err.as<int>(), "debug");
+  if (rc) return rc;
   int e = 0;
-  if (cudaStreamSynchronize(ctx->stream) || cudaMemcpy(&e, err.p, sizeof(int), cudaMemcpyDeviceToHost) ||
-      cudaMemcpy(out, o.p, nout * sizeof(float), cudaMemcpyDeviceToHost))
-    return done(b2_fail(ctx, B2_ERR_CUDA, std::string("debug conv: ") + cudaGetErrorString(cudaGetLastError())));
-  return done(e ? b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)") : B2_OK);
+  B2_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  B2_CUDA(ctx, cudaMemcpy(&e, err.p, sizeof(int), cudaMemcpyDeviceToHost));
+  B2_CUDA(ctx, cudaMemcpy(out, o.p, nout * sizeof(float), cudaMemcpyDeviceToHost));
+  if (e) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
+  return B2_OK;
 }
 
 extern "C" int b2_debug_d2net_avgpool_host(b2_context* ctx, const float* in, int H, int W, float* out) {
@@ -497,7 +486,6 @@ extern "C" int b2_debug_d2net_avgpool_host(b2_context* ctx, const float* in, int
   B2_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   B2_CUDA(ctx, cudaMemcpy(hl.data(), p.p, 2 * nout * sizeof(__half), cudaMemcpyDeviceToHost));
   for (size_t k = 0; k < nout; ++k) out[k] = __half2float(hl[k]) + __half2float(hl[nout + k]) * (1.0f / 2048.0f);  // hi + lo 2^-11
-  i.release(), p.release();
   return B2_OK;
 }
 
@@ -521,6 +509,5 @@ extern "C" int b2_debug_d2net_rank_host(b2_context* ctx, const float* scores, co
   B2_CHECK_LAUNCH(ctx);
   B2_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   B2_CUDA(ctx, cudaMemcpy(order, ord.p, (size_t)(max_k < n ? max_k : n) * sizeof(int), cudaMemcpyDeviceToHost));
-  sc.release(), ij.release(), cand.release(), cnt.release(), ord.release();
   return B2_OK;
 }

@@ -19,7 +19,7 @@ extern "C" int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, con
   std::lock_guard<std::mutex> lk(ctx->mu);
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
-  DevBuf dA, dB, dC, dBias, dBh, dBl, dErr;
+  DevBuf dA, dB, dC, dBias, dErr;
   B2_CUDA(ctx, dA.ensure((size_t)M * K * 4));
   B2_CUDA(ctx, dB.ensure((size_t)N * K * 4));
   B2_CUDA(ctx, dC.ensure((size_t)M * N * 4));
@@ -29,12 +29,12 @@ extern "C" int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, con
   B2_CUDA(ctx, cudaMemcpyAsync(dB.p, B, (size_t)N * K * 4, cudaMemcpyHostToDevice, st));
   if (bias) B2_CUDA(ctx, cudaMemcpyAsync(dBias.p, bias, (size_t)N * 4, cudaMemcpyHostToDevice, st));
   B2_CUDA(ctx, cudaMemsetAsync(dErr.p, 0, 16, st));
-  int rc = B2_OK;
   if (mode == 0) {
-    rc = launch_gemm(ctx, st, gemm_linear(dA.as<float>(), K, K, dB.as<float>(), bias ? dBias.as<float>() : nullptr, dC.as<float>(), N, M, N));
+    const int rc = launch_gemm(ctx, st, gemm_linear(dA.as<float>(), K, K, dB.as<float>(), bias ? dBias.as<float>() : nullptr, dC.as<float>(), N, M, N));
+    if (rc != B2_OK) return rc;
   } else {
     // modes 1 and 2 both run the wgmma kernel on operands split here (A and B as fp16 hi / lo planes)
-    DevBuf dAh, dAl;
+    DevBuf dAh, dAl, dBh, dBl;
     B2_CUDA(ctx, dAh.ensure((size_t)M * K * 2));
     B2_CUDA(ctx, dAl.ensure((size_t)M * K * 2));
     B2_CUDA(ctx, dBh.ensure((size_t)N * K * 2));
@@ -47,23 +47,16 @@ extern "C" int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, con
     LinArgs a;
     a.a1p = {dAh.as<__half>(), dAl.as<__half>()}, a.lda1 = K, a.K1 = K, a.bp = {dBh.as<__half>(), dBl.as<__half>()}, a.ldb = K;
     a.bias = bias ? dBias.as<float>() : nullptr, a.cf = dC.as<float>(), a.ldc = N, a.tc_want_f32 = true, a.M = M, a.N = N;
-    rc = run_linear(ctx, st, tw, &a, 1);
-    if (rc == B2_OK) {
-      cudaError_t e = cudaStreamSynchronize(st);
-      if (e != cudaSuccess) rc = b2_fail(ctx, B2_ERR_CUDA, std::string("debug gemm: ") + cudaGetErrorString(e));
-    }
-    dAh.release(), dAl.release();
+    const int rc = run_linear(ctx, st, tw, &a, 1);
+    if (rc != B2_OK) return rc;
+    B2_CUDA(ctx, cudaStreamSynchronize(st));
   }
   int err = 0;
-  if (rc == B2_OK) {
-    cudaError_t e = cudaMemcpyAsync(C, dC.p, (size_t)M * N * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&err, dErr.p, 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) rc = b2_fail(ctx, B2_ERR_CUDA, std::string("debug gemm: ") + cudaGetErrorString(e));
-  }
-  dA.release(), dB.release(), dC.release(), dBias.release(), dBh.release(), dBl.release(), dErr.release();
-  if (rc == B2_OK && err) rc = b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
-  return rc;
+  B2_CUDA(ctx, cudaMemcpyAsync(C, dC.p, (size_t)M * N * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(&err, dErr.p, 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  if (err) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
+  return B2_OK;
 }
 
 extern "C" int b2_debug_attention_host(b2_context* ctx, int np, const int* nq, const int* nk, int heads, float scale, int single,
@@ -101,18 +94,15 @@ extern "C" int b2_debug_attention_host(b2_context* ctx, int np, const int* nq, c
   }
   TcWeights tw{nullptr, nullptr, nullptr, dErr.as<int>(), true};
   tw.attn_part = &part, tw.attn_ml = &ml, tw.attn_cnt = &cnt, tw.sm_count = ctx->sm_count;
-  int rc = run_flash_planes(ctx, st, tw, fp, np, scale, single != 0);
+  const int rc = run_flash_planes(ctx, st, tw, fp, np, scale, single != 0);
+  if (rc != B2_OK) return rc;
   std::vector<__half> ho(2 * eq);
   int err = 0;
-  if (rc == B2_OK) {
-    cudaError_t e = cudaMemcpyAsync(ho.data(), oh, eq * 2 * 2, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&err, dErr.p, 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) rc = b2_fail(ctx, B2_ERR_CUDA, std::string("debug attention: ") + cudaGetErrorString(e));
-  }
-  if (rc == B2_OK)  // o = hi + lo * 2^-11 (the SINGLE variant writes lo = 0)
-    for (size_t i = 0; i < eq; ++i) o[i] = __half2float(ho[i]) + __half2float(ho[eq + i]) * tc::LO_INV;
-  dIn.release(), dPl.release(), dO.release(), dErr.release(), part.release(), ml.release(), cnt.release();
-  if (rc == B2_OK && err) rc = b2_fail(ctx, B2_ERR_STATE, "wgmma attention timed out on an mbarrier (kernel bug)");
-  return rc;
+  B2_CUDA(ctx, cudaMemcpyAsync(ho.data(), oh, eq * 2 * 2, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(&err, dErr.p, 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  // o = hi + lo * 2^-11 (the SINGLE variant writes lo = 0)
+  for (size_t i = 0; i < eq; ++i) o[i] = __half2float(ho[i]) + __half2float(ho[eq + i]) * tc::LO_INV;
+  if (err) return b2_fail(ctx, B2_ERR_STATE, "wgmma attention timed out on an mbarrier (kernel bug)");
+  return B2_OK;
 }

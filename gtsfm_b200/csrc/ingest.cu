@@ -6,12 +6,7 @@
 // HBM-bound byte work: one thread per output pixel, all channels, 16 clamped source reads per channel served by L1/L2.
 #include "common.cuh"
 
-namespace {
-struct IngestState {
-  DevBuf xtab, ytab;  // per destination index: int32 first source index, 4 x int16 weights (12 bytes, padded to 16)
-};
-}  // namespace
-
+// per destination index: int32 first source index, 4 x int16 weights (12 bytes, padded to 16)
 struct CubicTap {
   int s0;
   short w[4];
@@ -85,9 +80,8 @@ extern "C" int b2_image_resize_dev(b2_context* ctx, const uint8_t* src, int heig
   std::lock_guard<std::mutex> lk(ctx->mu);
   cudaSetDevice(ctx->device);
   cudaStream_t st = (cudaStream_t)stream;
-  static thread_local DevBuf tabs;  // (per host thread: the tap tables of the call in flight on `st`)
-  B2_CUDA(ctx, tabs.ensure((size_t)(new_width + new_height) * sizeof(CubicTap)));
-  CubicTap* xt = tabs.as<CubicTap>();
+  B2_CUDA(ctx, ctx->resize_taps.ensure((size_t)(new_width + new_height) * sizeof(CubicTap)));
+  CubicTap* xt = ctx->resize_taps.as<CubicTap>();
   CubicTap* yt = xt + new_width;
   B2_LAUNCH(ctx, k_cubic_taps, cdiv(new_width, 128), 128, 0, st, xt, new_width, width);
   B2_LAUNCH(ctx, k_cubic_taps, cdiv(new_height, 128), 128, 0, st, yt, new_height, height);

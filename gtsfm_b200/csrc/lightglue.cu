@@ -75,23 +75,7 @@ struct JobList {  // per-problem arguments of one batched launch; blockIdx.y (or
 };
 
 void lg_destroy(b2_context* ctx) {
-  if (!ctx->lg) return;
-  LightGlueState* s = ctx->lg;
-  s->wblob.release();
-  s->wblob_h.release();
-  s->wblob_l.release();
-  s->errflag.release();
-  for (auto& sd : s->side) {
-    DevBuf* bufs[] = {&sd.x[0], &sd.x[1], &sd.xs[0], &sd.xs[1], &sd.hs, &sd.qkv, &sd.q, &sd.k, &sd.v, &sd.ctx, &sd.msg, &sd.h, &sd.cs[0], &sd.cs[1],
-                      &sd.sn[0], &sd.sn[1], &sd.ind[0], &sd.ind[1], &sd.conf, &sd.mat, &sd.src, &sd.md, &sd.rmax,
-                      &sd.rlog, &sd.ls, &sd.lsg, &sd.amax, &sd.aidx};
-    for (DevBuf* b : bufs) b->release();
-  }
-  for (auto& b : s->sim) b.release();
-  s->attn_part.release(), s->attn_ml.release(), s->attn_cnt.release(), s->as_part.release(), s->as_bar.release();
-  s->counters.release();
-  s->hread.release();
-  delete s;
+  delete ctx->lg;
   ctx->lg = nullptr;
 }
 

@@ -55,13 +55,8 @@ struct MegaLocState {
 
 void ml_destroy(b2_context* ctx) {
   if (!ctx->ml) return;
-  MegaLocState* s = ctx->ml;
-  DevBuf* bufs[] = {&s->wh, &s->wl, &s->small, &s->errflag, &s->attn_part, &s->attn_ml, &s->attn_cnt, &s->postab, &s->rh.w, &s->rh.x0,
-                    &s->rv.w, &s->rv.x0, &s->col, &s->x, &s->lnp, &s->qkv, &s->att, &s->hid, &s->h1, &s->fcl, &s->sco, &s->t1,
-                    &s->tfe, &s->vsc, &s->pm, &s->agg, &s->dph, &s->dpl, &s->hout, &s->imgs, &s->rsz, &s->rtmp};
-  for (DevBuf* b : bufs) b->release();
   ctx->debug.erase("megaloc_tokens");
-  delete s;
+  delete ctx->ml;
   ctx->ml = nullptr;
 }
 
@@ -843,14 +838,9 @@ extern "C" int b2_megaloc_describe_host(b2_context* ctx, const float* images, in
   cudaSetDevice(ctx->device);
   B2_CUDA(ctx, in_d.ensure(nin));
   B2_CUDA(ctx, out_d.ensure(nout));
-  int rc = B2_ERR_CUDA;
-  if (cudaMemcpy(in_d.p, images, nin, cudaMemcpyHostToDevice) == cudaSuccess) {
-    rc = b2_megaloc_describe_dev(ctx, in_d.as<float>(), B, H, W, out_d.as<float>(), ctx->stream);
-    if (rc == B2_OK && cudaMemcpy(out, out_d.p, nout, cudaMemcpyDeviceToHost) != cudaSuccess) rc = b2_fail(ctx, B2_ERR_CUDA, "copy of the descriptors failed");
-  } else {
-    b2_fail(ctx, B2_ERR_CUDA, "copy of the images failed");
-  }
-  in_d.release();
-  out_d.release();
-  return rc;
+  B2_CUDA(ctx, cudaMemcpy(in_d.p, images, nin, cudaMemcpyHostToDevice));
+  const int rc = b2_megaloc_describe_dev(ctx, in_d.as<float>(), B, H, W, out_d.as<float>(), ctx->stream);
+  if (rc != B2_OK) return rc;
+  B2_CUDA(ctx, cudaMemcpy(out, out_d.p, nout, cudaMemcpyDeviceToHost));
+  return B2_OK;
 }

@@ -80,12 +80,7 @@ struct MnnState {
 };
 
 void mn_destroy(b2_context* ctx) {
-  if (!ctx->mn) return;
-  MnnState* s = ctx->mn;
-  DevBuf* bufs[] = {&s->u8, &s->hi, &s->lo, &s->norm_i, &s->norm_f, &s->best, &s->d1, &s->d2, &s->seg_ok,
-                    &s->table, &s->out_k, &s->sort, &s->err, &s->in0, &s->in1, &s->om, &s->od};
-  for (DevBuf* b : bufs) b->release();
-  delete s;
+  delete ctx->mn;
   ctx->mn = nullptr;
 }
 

@@ -29,12 +29,7 @@ struct NetVladState {
 };
 
 void nv_destroy(b2_context* ctx) {
-  if (!ctx->nv) return;
-  NetVladState* s = ctx->nv;
-  DevBuf* bufs[] = {&s->w0, &s->bias, &s->wh, &s->wl, &s->sh, &s->sl, &s->centers, &s->whh, &s->whl, &s->wbias, &s->errflag,
-                    &s->actA, &s->actB, &s->feat, &s->xn, &s->xnp, &s->scores, &s->vlad, &s->vh, &s->vl, &s->out};
-  for (DevBuf* b : bufs) b->release();
-  delete s;
+  delete ctx->nv;
   ctx->nv = nullptr;
 }
 
@@ -309,14 +304,9 @@ extern "C" int b2_netvlad_describe_host(b2_context* ctx, const float* images, in
   cudaSetDevice(ctx->device);
   B2_CUDA(ctx, in_d.ensure(nin));
   B2_CUDA(ctx, out_d.ensure(nout));
-  int rc = B2_ERR_CUDA;
-  if (cudaMemcpy(in_d.p, images, nin, cudaMemcpyHostToDevice) == cudaSuccess) {
-    rc = b2_netvlad_describe_dev(ctx, in_d.as<float>(), B, H, W, out_d.as<float>(), ctx->stream);
-    if (rc == B2_OK && cudaMemcpy(out, out_d.p, nout, cudaMemcpyDeviceToHost) != cudaSuccess) rc = b2_fail(ctx, B2_ERR_CUDA, "copy of the descriptors failed");
-  } else {
-    b2_fail(ctx, B2_ERR_CUDA, "copy of the images failed");
-  }
-  in_d.release();
-  out_d.release();
-  return rc;
+  B2_CUDA(ctx, cudaMemcpy(in_d.p, images, nin, cudaMemcpyHostToDevice));
+  const int rc = b2_netvlad_describe_dev(ctx, in_d.as<float>(), B, H, W, out_d.as<float>(), ctx->stream);
+  if (rc != B2_OK) return rc;
+  B2_CUDA(ctx, cudaMemcpy(out, out_d.p, nout, cudaMemcpyDeviceToHost));
+  return B2_OK;
 }

@@ -30,12 +30,7 @@ struct RansacState {
 };
 
 void rs_destroy(b2_context* ctx) {
-  if (!ctx->rs) return;
-  RansacState* s = ctx->rs;
-  DevBuf* bufs[] = {&s->x1, &s->x2, &s->models, &s->nsol, &s->cost, &s->ninl, &s->best, &s->mask, &s->pose};
-  for (DevBuf* b : bufs) b->release();
-  s->hbuf.release();
-  delete s;
+  delete ctx->rs;
   ctx->rs = nullptr;
 }
 

@@ -17,11 +17,7 @@ struct RetrievalState {
 };
 
 void rt_destroy(b2_context* ctx) {
-  if (!ctx->rt) return;
-  RetrievalState* s = ctx->rt;
-  DevBuf* bufs[] = {&s->g, &s->gh, &s->gl, &s->sim, &s->pairs, &s->count, &s->err};
-  for (DevBuf* b : bufs) b->release();
-  delete s;
+  delete ctx->rt;
   ctx->rt = nullptr;
 }
 

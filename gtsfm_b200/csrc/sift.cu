@@ -76,11 +76,7 @@ struct SiftState {
 };
 
 void sf_destroy(b2_context* ctx) {
-  SiftState* s = ctx->sf;
-  if (!s) return;
-  DevBuf* bufs[] = {&s->pyr, &s->cand, &s->raw, &s->sorted, &s->fin, &s->fresp, &s->sel, &s->counts, &s->table, &s->img, &s->mask, &s->okp, &s->odesc};
-  for (DevBuf* b : bufs) b->release();
-  delete s;
+  delete ctx->sf;
   ctx->sf = nullptr;
 }
 

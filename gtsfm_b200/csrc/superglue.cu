@@ -42,15 +42,7 @@ struct SuperGlueState {
 };
 
 void sg_destroy(b2_context* ctx) {
-  if (!ctx->sg) return;
-  SuperGlueState* s = ctx->sg;
-  DevBuf* top[] = {&s->wblob, &s->wblob_h, &s->wblob_l, &s->errflag, &s->sim, &s->counters, &s->attn_part, &s->attn_ml, &s->attn_cnt, &s->sk_part, &s->sk_bar};
-  for (DevBuf* b : top) b->release();
-  for (auto& sd : s->side) {
-    DevBuf* bufs[] = {&sd.x, &sd.xs, &sd.q, &sd.k, &sd.v, &sd.ctx, &sd.msg, &sd.h, &sd.hs, &sd.md, &sd.u, &sd.vv, &sd.best, &sd.arg};
-    for (DevBuf* b : bufs) b->release();
-  }
-  delete s;
+  delete ctx->sg;
   ctx->sg = nullptr;
 }
 

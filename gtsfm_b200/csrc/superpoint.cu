@@ -69,9 +69,6 @@ static inline uint32_t __float_as_uint_host(float f) {
 void sp_destroy(b2_context* ctx) {
   if (!ctx->sp) return;
   SuperPointState* s = ctx->sp;
-  DevBuf* bufs[] = {&s->wblob, &s->wsplit_h, &s->wsplit_l, &s->errflag, &s->conv_dbg, &s->logits, &s->gray, &s->a0, &s->a1, &s->feat, &s->head, &s->heat, &s->nms,
-                    &s->rowcnt, &s->rowoff, &s->dense, &s->kpxy, &s->kpsc, &s->sel_idx, &s->sel_cnt};
-  for (DevBuf* b : bufs) b->release();
   for (auto& g : s->gslot)
     if (g.exec) cudaGraphExecDestroy(g.exec);
   if (s->cap_stream) cudaStreamDestroy(s->cap_stream);
@@ -750,7 +747,6 @@ extern "C" int b2_superpoint_set_weights(b2_context* ctx, const float* blob, siz
               s->wsplit_l.as<__half>());
     B2_CHECK_LAUNCH(ctx);
     B2_CUDA(ctx, cudaDeviceSynchronize());
-    tmp.release();
     B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CP_SMEM));
     B2_CUDA(ctx, cudaFuncSetAttribute(k_gemm_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GW_SMEM));
     s->use_tc = !b2_force_simt(ctx) && tma_encoder() != nullptr;
