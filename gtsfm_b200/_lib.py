@@ -77,6 +77,7 @@ SIGNATURES = {
     "b2_profile_stop": (_i, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.POINTER(C.c_double)]),
     "b2_debug_fetch": (C.c_int64, [_vp, C.c_char_p, _vp, C.c_int64]),
     "b2_debug_gemm_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i]),
+    "b2_debug_gemm_segments_host": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "b2_debug_attention_host": (_i, [_vp, _i, _ip, _ip, _i, _f, _i, _vp, _vp, _vp, _vp]),
     "b2_superpoint_set_weights": (_i, [_vp, _vp, _sz]),
     "b2_superpoint_detect_dev": (_i, [_vp, _vp, _i, _i, _i, _sz, _f, _i, _i, _vp, _vp, _i, _ip, C.POINTER(C.c_uint64), _vp]),
@@ -89,6 +90,7 @@ SIGNATURES = {
     "b2_superpoint_describe_host": (_i, [_vp, C.c_uint64, _vp, _i, _vp]),
     "b2_image_resize_dev": (_i, [_vp, _vp, _i, _i, _i, _sz, _vp, _i, _i, _vp]),
     "b2_lightglue_set_weights": (_i, [_vp, _vp, _sz]),
+    "b2_lightglue_qkv_rows": (_i, [_vp]),
     "b2_lightglue_match_dev": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, C.POINTER(LightGlueParams), _vp, _vp, _ip, _ip, _vp]),
     "b2_lightglue_match_host": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, C.POINTER(LightGlueParams), _vp, _vp, _ip, _ip]),
     "b2_lightglue_match_batched_dev": (_i, [_vp, C.POINTER(LightGluePair), _i, C.POINTER(LightGlueParams), _vp]),

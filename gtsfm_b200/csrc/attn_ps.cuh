@@ -40,7 +40,7 @@ constexpr int AS_HALF = 2 * AW_KV_BYTES;     // hi + lo plane of one 64 x 64 til
 constexpr int AS_STAGE = 2 * AS_HALF;        // K part at +0, V part at +AS_HALF
 constexpr int AS_TILE_BYTES = AS_NS * AS_STAGE;
 constexpr int AS_Q_PLANE = AW_Q * AW_D * 2;  // 16 KB: one plane of a 128-query tile
-constexpr int AS_Q_BYTES = 2 * 2 * AS_Q_PLANE;  // hi + lo planes of both query tiles
+constexpr int AS_Q_BYTES = 2 * AS_Q_PLANE;  // lo plane of both query tiles (Q hi is read into registers)
 constexpr size_t AS_SMEM = AS_TILE_BYTES + AS_Q_BYTES + 1024 + 512;
 constexpr int AS_THREADS = 256 + 128;  // 2 consumer warpgroups + TMA producer warpgroup (one thread works)
 constexpr float AS_RESCALE = 8.0f;  // log2 of the largest P allowed before the reference maximum is refreshed
@@ -158,7 +158,7 @@ static __global__ void __launch_bounds__(AS_THREADS, 1) k_flash_ps(const __grid_
     const int r = t & 127;
     const int rq = (warp & 3) * 16 + (lane >> 2);  // fragment rows rq, rq + 8 of a slab
     const int c2 = (lane & 3) * 2;                 // fragment columns 8j + c2, + 1
-    const uint32_t sQ = smem0 + AS_TILE_BYTES + q * 2 * AS_Q_PLANE;
+    const uint32_t sQl = smem0 + AS_TILE_BYTES + q * AS_Q_PLANE;
     const float c2s = args.scale * 1.4426950408889634f;
     auto wg_bar = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + q) : "memory"); };
     auto release = [&](int g) { if (lane == 0) tc::mbar_arrive(&kv_empty[g % AS_NS]); };
@@ -168,19 +168,16 @@ static __global__ void __launch_bounds__(AS_THREADS, 1) k_flash_ps(const __grid_
       const AttnPsSeg sg = attn_ps_decode(args, w, w_end);
       const AttnPsProblem& pr = args.p[sg.z];
       const int T = sg.T, Nk = pr.Nk;
-      {  // this thread's query row -> shared memory, 128-byte swizzled (zero rows past the end)
+      if (!SINGLE) {  // this thread's query row of the lo plane -> shared memory, 128-byte swizzled (zero rows past the end)
         const int qrow = sg.q0 + q * AW_Q + r;
-        wg_bar();  // the previous segment's MMAs of every warp of the group have read Q
+        wg_bar();  // the previous segment's MMAs of every warp of the group have read Q lo
+        const __half* src = pr.Ql + ((size_t)sg.h * pr.Nq + qrow) * 64;
+        unsigned char* dst = sm + AS_TILE_BYTES + q * AS_Q_PLANE + r * 128;
 #pragma unroll
-        for (int pl = 0; pl < (SINGLE ? 1 : 2); ++pl) {
-          const __half* src = (pl ? pr.Ql : pr.Qh) + ((size_t)sg.h * pr.Nq + qrow) * 64;
-          unsigned char* dst = sm + AS_TILE_BYTES + q * 2 * AS_Q_PLANE + pl * AS_Q_PLANE + r * 128;
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            uint4 v = make_uint4(0u, 0u, 0u, 0u);
-            if (qrow < pr.Nq) v = __ldg(reinterpret_cast<const uint4*>(src) + c);
-            *reinterpret_cast<uint4*>(dst + ((c ^ (r & 7)) << 4)) = v;
-          }
+        for (int c = 0; c < 8; ++c) {
+          uint4 v = make_uint4(0u, 0u, 0u, 0u);
+          if (qrow < pr.Nq) v = __ldg(reinterpret_cast<const uint4*>(src) + c);
+          *reinterpret_cast<uint4*>(dst + ((c ^ (r & 7)) << 4)) = v;
         }
         tc::fence_proxy_async();  // generic-proxy stores -> visible to the tensor core
         wg_bar();
@@ -209,7 +206,7 @@ static __global__ void __launch_bounds__(AS_THREADS, 1) k_flash_ps(const __grid_
       auto qk = [&](int i, int sl) {
         const uint32_t sK = smem0 + ((ge + i) % AS_NS) * AS_STAGE;
         const uint64_t dKh = tc::wg_desc_sw128(sK), dKl = tc::wg_desc_sw128(sK + AW_KV_BYTES);
-        const uint64_t dQl = tc::wg_desc_sw128(sQ + AS_Q_PLANE + sl * (64 * 128));
+        const uint64_t dQl = tc::wg_desc_sw128(sQl + sl * (64 * 128));
         tc::wg_fence();
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) {

@@ -182,14 +182,17 @@ inline void b2_prof_work(b2_context* ctx, const char* kernel, double work) {
   if (ctx->prof.match(kernel)) ctx->prof.work += work;
 }
 
-#define B2_LAUNCH(ctx, kernel, grid, block, smem, stream, ...)  \
-  do {                                                          \
-    const bool _prof = (ctx)->prof.match(#kernel);              \
-    if (_prof) b2_prof_mark((ctx), (stream));                   \
-    kernel<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__); \
-    if (_prof) b2_prof_mark((ctx), (stream));                   \
-    (ctx)->launches++;                                          \
+// `name` is what the profiler matches against: the kernel's own name, or that name followed by a call-site label
+// ("k_gemm_ws/lg_self_qkv") so that one call site of a shared kernel can be timed on its own
+#define B2_LAUNCH_NAMED(ctx, name, kernel, grid, block, smem, stream, ...) \
+  do {                                                                     \
+    const bool _prof = (ctx)->prof.match(name);                            \
+    if (_prof) b2_prof_mark((ctx), (stream));                              \
+    kernel<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__);            \
+    if (_prof) b2_prof_mark((ctx), (stream));                              \
+    (ctx)->launches++;                                                     \
   } while (0)
+#define B2_LAUNCH(ctx, kernel, grid, block, smem, stream, ...) B2_LAUNCH_NAMED(ctx, #kernel, kernel, grid, block, smem, stream, __VA_ARGS__)
 
 #define B2_CHECK_LAUNCH(ctx) B2_CUDA(ctx, cudaGetLastError())
 

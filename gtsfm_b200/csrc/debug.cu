@@ -1,5 +1,5 @@
-// Test-only entry points: run one GEMM through the SIMT fp32 kernel or the wgmma split-fp16 kernel (parity tests), and one
-// batched launch of the split-fp16 flash attention kernel.
+// Test-only entry points: run one GEMM through the SIMT fp32 kernel or the wgmma split-fp16 kernel (parity tests), the
+// wgmma kernel's column-segment / rotary epilogue, and one batched launch of the split-fp16 flash attention kernel.
 #include <stdlib.h>
 
 #include <vector>
@@ -53,6 +53,66 @@ extern "C" int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, con
   }
   int err = 0;
   B2_CUDA(ctx, cudaMemcpyAsync(C, dC.p, (size_t)M * N * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(&err, dErr.p, 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  if (err) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
+  return B2_OK;
+}
+
+extern "C" int b2_debug_gemm_segments_host(b2_context* ctx, const float* A, const float* B, const float* bias, int M, int K, int nseg,
+                                           int rot_mask, const float* cs, const float* sn, int separate, uint16_t* out_hi, uint16_t* out_lo) {
+  if (!ctx || !A || !B || !bias || !out_hi || !out_lo || M <= 0 || K <= 0 || (K % 64) || nseg < 1 || nseg > GW_SEGS ||
+      (rot_mask && (!cs || !sn || separate)))
+    return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  const int N = 256 * nseg;
+  const size_t ep = (size_t)M * 256;  // halves of one segment's plane
+  DevBuf dA, dB, dBias, dCs, dSn, dErr, dAh, dAl, dBh, dBl, dH, dL;
+  B2_CUDA(ctx, dA.ensure((size_t)M * K * 4));
+  B2_CUDA(ctx, dB.ensure((size_t)N * K * 4));
+  B2_CUDA(ctx, dBias.ensure((size_t)N * 4));
+  B2_CUDA(ctx, dCs.ensure((size_t)M * 32 * 4));
+  B2_CUDA(ctx, dSn.ensure((size_t)M * 32 * 4));
+  B2_CUDA(ctx, dErr.ensure(16));
+  B2_CUDA(ctx, dAh.ensure((size_t)M * K * 2));
+  B2_CUDA(ctx, dAl.ensure((size_t)M * K * 2));
+  B2_CUDA(ctx, dBh.ensure((size_t)N * K * 2));
+  B2_CUDA(ctx, dBl.ensure((size_t)N * K * 2));
+  B2_CUDA(ctx, dH.ensure(nseg * ep * 2));
+  B2_CUDA(ctx, dL.ensure(nseg * ep * 2));
+  B2_CUDA(ctx, cudaMemcpyAsync(dA.p, A, (size_t)M * K * 4, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(dB.p, B, (size_t)N * K * 4, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(dBias.p, bias, (size_t)N * 4, cudaMemcpyHostToDevice, st));
+  if (rot_mask) {
+    B2_CUDA(ctx, cudaMemcpyAsync(dCs.p, cs, (size_t)M * 32 * 4, cudaMemcpyHostToDevice, st));
+    B2_CUDA(ctx, cudaMemcpyAsync(dSn.p, sn, (size_t)M * 32 * 4, cudaMemcpyHostToDevice, st));
+  }
+  B2_CUDA(ctx, cudaMemsetAsync(dErr.p, 0, 16, st));
+  B2_LAUNCH(ctx, k_split_f32, (unsigned)(((size_t)M * K + 255) / 256), 256, 0, st, dA.as<float>(), (size_t)M * K, dAh.as<__half>(), dAl.as<__half>());
+  B2_LAUNCH(ctx, k_split_f32, (unsigned)(((size_t)N * K + 255) / 256), 256, 0, st, dB.as<float>(), (size_t)N * K, dBh.as<__half>(), dBl.as<__half>());
+  B2_CUDA(ctx, cudaFuncSetAttribute(k_gemm_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GW_SMEM));
+  TcWeights tw{nullptr, nullptr, nullptr, dErr.as<int>(), true};
+  tw.sm_count = ctx->sm_count;
+  __half *H = dH.as<__half>(), *L = dL.as<__half>(), *Bh = dBh.as<__half>(), *Bl = dBl.as<__half>();
+  LinArgs a;
+  a.a1p = {dAh.as<__half>(), dAl.as<__half>()}, a.lda1 = K, a.K1 = K, a.ldb = K, a.M = M, a.head_major = 1, a.lo_unscaled = 1;
+  for (int s = 0; s < (separate ? nseg : 1); ++s) {
+    if (separate) {  // segment s as a linear of its own: its 256 rows of B and of the bias
+      a.bp = {Bh + (size_t)s * 256 * K, Bl + (size_t)s * 256 * K}, a.bias = dBias.as<float>() + s * 256, a.N = 256;
+      a.cp = {H + s * ep, L + s * ep};
+    } else {
+      a.bp = {Bh, Bl}, a.bias = dBias.as<float>(), a.N = N, a.seg_n = 256;
+      for (int j = 0; j < nseg; ++j) a.seg_p[j] = {H + j * ep, L + j * ep};
+      a.rot_mask = rot_mask, a.cs = dCs.as<float>(), a.sn = dSn.as<float>();
+    }
+    const int rc = run_linear(ctx, st, tw, &a, 1);
+    if (rc != B2_OK) return rc;
+  }
+  int err = 0;
+  B2_CUDA(ctx, cudaMemcpyAsync(out_hi, H, nseg * ep * 2, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(out_lo, L, nseg * ep * 2, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaMemcpyAsync(&err, dErr.p, 4, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
   if (err) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");

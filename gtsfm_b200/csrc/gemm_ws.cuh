@@ -27,6 +27,11 @@
 // the consumers used to: (fmaf(acc1, 2^-11, acc0) + bias) * scale, ReLU or GELU, + residual, then the same split helpers.  Its
 // mode flags (relu, gelu, head-major, unscaled lo, which outputs) are read once per tile and are warp-uniform; they are not
 // compile-time specialisations.
+// Column segments (seg_n > 0): output columns s * seg_n .. (s + 1) * seg_n - 1 go to their own head-major planes Ch[s] / Cl[s],
+// so one launch can write several attention operands (LightGlue's q | k | v, or the cross block's q | v).  A segment whose
+// bit is set in rot_mask gets the rotary encoding of lightglue.py:58-65 from the problem's cos / sin table [M][32] before
+// the split: an epilogue lane's 4 columns are two whole (2p, 2p + 1) pairs, and the product / sum sequence is the one of
+// k_lg_split_rotary, so the planes are bit-identical to an fp32 GEMM output rotated and split in a second kernel.
 #pragma once
 #include "tma.cuh"
 
@@ -43,11 +48,13 @@ constexpr int GW_RB = 8;  // epilogue rows per warp whose residual loads are in 
 constexpr int GW_EW = 4;  // epilogue warps
 constexpr int GW_THREADS = 512;  // two consumer warpgroups, the epilogue warpgroup, the producer warpgroup (one thread works)
 constexpr size_t GW_SMEM = GW_STAGES * GW_STAGE_BYTES + GW_STG_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int GW_SEGS = 3;  // column segments per problem
 
 struct GemmProblem {
   const float* resid;  // [M][ldr] fp32 or null, added after bias / scale
   float* C;            // optional fp32 output, row-major [M][ldc]
-  __half *Ch, *Cl;     // optional split output planes
+  __half *Ch[GW_SEGS], *Cl[GW_SEGS];  // optional split output planes; [0] unless the launch has column segments
+  const float *cs, *sn;               // rotary table [M][32] (segments with a rot_mask bit)
   int M, N, ldc;
   int vec4;      // outputs / residual may be accessed 4 columns at a time (host checks 16-byte alignment of bases and lds)
   int tiles_n;   // ceil(N / 128)
@@ -71,8 +78,13 @@ struct GemmWsArgs {
   int relu;        // max(., 0) after bias / scale, before the residual
   int gelu;        // exact (erf) GELU after bias / scale, before the residual
   int lo_unscaled; // split outputs keep lo = fp16(x - hi) (attention operands)
+  int seg_n;       // > 0: columns per segment (a multiple of GW_N; head_major, plane outputs only, every access 4-wide)
+  int rot_mask;    // bit s: rotary on segment s
   int* err_flag;   // set to 1 if an mbarrier wait timed out (pipeline bug): results are then invalid
 };
+
+// exact (erf) GELU; out of line, so that the epilogue's unrolled row loop does not carry eight inlined copies of erff
+static __device__ __noinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
 static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_constant__ GemmWsMaps maps, const __grid_constant__ GemmWsArgs g) {
   extern __shared__ unsigned char gw_raw[];
@@ -193,7 +205,9 @@ static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_c
       const GemmProblem& pb = g.p[z];
       const float* resid = pb.resid;
       float* C = pb.C;
-      __half *Ch = pb.Ch, *Cl = pb.Cl;
+      const int sg = g.seg_n ? n0 / g.seg_n : 0;  // column segment of this tile
+      __half *Ch = pb.Ch[sg], *Cl = pb.Cl[sg];
+      const bool rot = (g.rot_mask >> sg) & 1;
       const int M = pb.M, ldc = pb.ldc;
       const int n = n0 + c;
       const int ncols = min(4, pb.N - n);  // this thread's valid columns (<= 0 past the end)
@@ -204,66 +218,97 @@ static __global__ void __launch_bounds__(GW_THREADS, 1) k_gemm_ws(const __grid_c
 #pragma unroll
         for (int e = 0; e < 4; ++e)
           if (e < ncols) b4[e] = __ldg(g.bias + n + e);
-      const size_t hm_col = (size_t)(n >> 6) * M * 64 + (n & 63);  // head-major: [N / 64][M][64] (4 columns stay in one head)
+      const int ns = n - sg * g.seg_n;  // column inside the segment
+      const size_t hm_col = (size_t)(ns >> 6) * M * 64 + (ns & 63);  // head-major: [N / 64][M][64] (4 columns stay in one head)
       // Rows go in batches of GW_RB per warp with the batch's residual loads issued together (the first batch's before the
       // staging wait), so the residual's DRAM latency is paid once per batch rather than once per row.  In-place use
-      // (resid == C) stays safe: every element is read and then written by this thread alone.
+      // (resid == C) stays safe: every element is read and then written by this thread alone.  A rotary segment has no
+      // residual and loads its rows' (cos, cos, sin, sin) of pairs p, p + 1 into the same registers.
       const bool vres = resid && vec;
+      const int rp = (ns & 63) >> 1;  // first rotary pair of this thread's columns
       float4 rr[GW_RB];
-      auto load_resid = [&](int rb) {
+      auto load_rows = [&](int rb) {  // the branch stays outside the loops: each batch's loads go out back to back
+        if (rot) {
 #pragma unroll
-        for (int i = 0; i < GW_RB; ++i)
-          if (rb + GW_EW * i < rows) rr[i] = *reinterpret_cast<const float4*>(resid + (size_t)(m0 + rb + GW_EW * i) * ldr + n);
+          for (int i = 0; i < GW_RB; ++i)
+            if (rb + GW_EW * i < rows) {
+              const size_t o = (size_t)(m0 + rb + GW_EW * i) * 32 + rp;
+              const float2 cc = __ldg(reinterpret_cast<const float2*>(pb.cs + o)), ss = __ldg(reinterpret_cast<const float2*>(pb.sn + o));
+              rr[i] = make_float4(cc.x, cc.y, ss.x, ss.y);
+            }
+        } else {
+#pragma unroll
+          for (int i = 0; i < GW_RB; ++i)
+            if (rb + GW_EW * i < rows) rr[i] = *reinterpret_cast<const float4*>(resid + (size_t)(m0 + rb + GW_EW * i) * ldr + n);
+        }
       };
-      if (vres) load_resid(ew);
+      if (vres || rot) load_rows(ew);
       ok = tc::mbar_wait(sfull, it & 1) && ok;
-      if (ncols > 0) {
+      auto pre = [&](int r, float* v) {  // staged accumulators -> (. + bias) * scale, ReLU / GELU
+        const float4 a = *reinterpret_cast<const float4*>(stg + r * GW_PITCH + c);
+        v[0] = a.x, v[1] = a.y, v[2] = a.z, v[3] = a.w;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          v[e] = (v[e] + b4[e]) * scale;
+          if (relu) v[e] = fmaxf(v[e], 0.f);
+          if (gelu) v[e] = gelu_erf(v[e]);
+        }
+      };
+      if (ncols > 0 && vec) {
         for (int rb = ew; rb < rows; rb += GW_EW * GW_RB) {
-          if (vres && rb != ew) load_resid(rb);
+          if ((vres || rot) && rb != ew) load_rows(rb);
 #pragma unroll
           for (int i = 0; i < GW_RB; ++i) {
             const int r = rb + GW_EW * i;
             if (r >= rows) break;
             const int row = m0 + r;
-            const float4 a = *reinterpret_cast<const float4*>(stg + r * GW_PITCH + c);
-            float v[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              v[e] = (v[e] + b4[e]) * scale;
-              if (relu) v[e] = fmaxf(v[e], 0.f);
-              if (gelu) v[e] = 0.5f * v[e] * (1.0f + erff(v[e] * 0.70710678118654752440f));
+            float v[4];
+            pre(r, v);
+            if (resid) v[0] += rr[i].x, v[1] += rr[i].y, v[2] += rr[i].z, v[3] += rr[i].w;
+            if (rot) {  // (t * cos) + (rotate_half(t) * sin), rotate_half: (x1, x2) -> (-x2, x1)
+              const float c0 = rr[i].x, c1 = rr[i].y, s0 = rr[i].z, s1 = rr[i].w;
+              const float a0 = __fadd_rn(__fmul_rn(v[0], c0), __fmul_rn(-v[1], s0)), a1 = __fadd_rn(__fmul_rn(v[1], c0), __fmul_rn(v[0], s0));
+              const float a2 = __fadd_rn(__fmul_rn(v[2], c1), __fmul_rn(-v[3], s1)), a3 = __fadd_rn(__fmul_rn(v[3], c1), __fmul_rn(v[2], s1));
+              v[0] = a0, v[1] = a1, v[2] = a2, v[3] = a3;
             }
-            const size_t off_c = hm ? hm_col + (size_t)row * 64 : (size_t)row * ldc + n;
-            const size_t off_s = hm ? hm_col + (size_t)row * 64 : (size_t)row * ldch + n;
-            if (vec) {
-              if (resid) v[0] += rr[i].x, v[1] += rr[i].y, v[2] += rr[i].z, v[3] += rr[i].w;
-              if (C) *reinterpret_cast<float4*>(C + off_c) = make_float4(v[0], v[1], v[2], v[3]);
-              if (Ch) {
-                uint32_t h01, l01, h23, l23;
-                if (lo_unscaled) {
-                  tc::split2_unscaled_clamped(v[0], v[1], h01, l01);
-                  tc::split2_unscaled_clamped(v[2], v[3], h23, l23);
-                } else {
-                  tc::split2(v[0], v[1], h01, l01);
-                  tc::split2(v[2], v[3], h23, l23);
-                }
-                *reinterpret_cast<uint2*>(Ch + off_s) = make_uint2(h01, h23);
-                *reinterpret_cast<uint2*>(Cl + off_s) = make_uint2(l01, l23);
+            const size_t off = hm ? hm_col + (size_t)row * 64 : (size_t)row * ldc + n;
+            if (C) *reinterpret_cast<float4*>(C + off) = make_float4(v[0], v[1], v[2], v[3]);
+            if (Ch) {
+              const size_t off_s = hm ? off : (size_t)row * ldch + n;
+              uint32_t h01, l01, h23, l23;
+              if (lo_unscaled) {
+                tc::split2_unscaled_clamped(v[0], v[1], h01, l01);
+                tc::split2_unscaled_clamped(v[2], v[3], h23, l23);
+              } else {
+                tc::split2(v[0], v[1], h01, l01);
+                tc::split2(v[2], v[3], h23, l23);
               }
-            } else {
+              *reinterpret_cast<uint2*>(Ch + off_s) = make_uint2(h01, h23);
+              *reinterpret_cast<uint2*>(Cl + off_s) = make_uint2(l01, l23);
+            }
+          }
+        }
+      } else if (ncols > 0) {
+        // the cold path (a ragged last column tile, or outputs without 16-byte alignment): element by element, one row at a
+        // time, kept out of the unrolled loop above so that the hot loop's code stays small
+#pragma unroll 1
+        for (int r = ew; r < rows; r += GW_EW) {
+          const int row = m0 + r;
+          float v[4];
+          pre(r, v);
+          const size_t off_c = hm ? hm_col + (size_t)row * 64 : (size_t)row * ldc + n;
+          const size_t off_s = hm ? hm_col + (size_t)row * 64 : (size_t)row * ldch + n;
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                if (e >= ncols) break;
-                if (resid) v[e] += resid[(size_t)row * ldr + n + e];
-                if (C) C[off_c + e] = v[e];
-                if (Ch) {
-                  __half hh, ll;
-                  if (lo_unscaled) tc::split_h_unscaled(v[e], hh, ll);
-                  else tc::split_h(v[e], hh, ll);
-                  Ch[off_s + e] = hh;
-                  Cl[off_s + e] = ll;
-                }
-              }
+          for (int e = 0; e < 4; ++e) {
+            if (e >= ncols) break;
+            if (resid) v[e] += resid[(size_t)row * ldr + n + e];
+            if (C) C[off_c + e] = v[e];
+            if (Ch) {
+              __half hh, ll;
+              if (lo_unscaled) tc::split_h_unscaled(v[e], hh, ll);
+              else tc::split_h(v[e], hh, ll);
+              Ch[off_s + e] = hh;
+              Cl[off_s + e] = ll;
             }
           }
         }

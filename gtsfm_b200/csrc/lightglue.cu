@@ -20,10 +20,10 @@ constexpr size_t LG_NFLOATS = 11851601;
 constexpr int D = 256;
 
 struct SelfW {
-  float *wqkv, *bqkv, *wout, *bout, *w0, *b0, *lng, *lnb, *w3, *b3;
+  float *wqkv, *bqkv, *wout, *bout, *w0, *b0, *lng, *lnb, *w3, *b3;  // wqkv / bqkv rows in b2_lightglue_qkv_rows order
 };
 struct CrossW {
-  float *wqk, *bqk, *wv, *bv, *wout, *bout, *w0, *b0, *lng, *lnb, *w3, *b3;
+  float *wqv, *bqv, *wout, *bout, *w0, *b0, *lng, *lnb, *w3, *b3;  // wqv [512][256] = [to_qk; to_v], bqv [512] likewise
 };
 struct AssignW {
   float *wm, *bm, *wf, *bf;
@@ -152,55 +152,33 @@ __global__ void __launch_bounds__(256) k_lg_load_desc(const __grid_constant__ Jo
   }
 }
 
-// qkv [N][768] with feature (h*64 + j)*3 + {q,k,v} (lightglue.py:166-167) -> rotary on q,k (:58-65) -> [4][N][64],
-// either as fp32 (SIMT attention) or split into fp16 hi / lo planes (wgmma attention; plane stride = 4*N*64 halves).
+// SIMT path: qkv [N][768] as [q | k | v] (b2_lightglue_qkv_rows) -> rotary on q,k (lightglue.py:58-65) -> fp32 [4][N][64].
+// The wgmma path does the same in the projection's epilogue (gemm_ws.cuh, column segments).
 struct RotJob {  // one image's share of a two-image launch (blockIdx.y)
   const float *qkv, *cs, *sn;
   int n;
-  size_t plane;
-  void *qo, *ko, *vo;
+  float *qo, *ko, *vo;
 };
-template <bool SPLIT>
-__global__ void __launch_bounds__(256) k_lg_split_rotary(const __grid_constant__ JobList<RotJob> jobs, int qk_unscaled) {
+__global__ void __launch_bounds__(256) k_lg_split_rotary(const __grid_constant__ JobList<RotJob> jobs) {
   const RotJob& jb = jobs.j[blockIdx.y];
   const float* __restrict__ qkv = jb.qkv;
   const float* __restrict__ cs = jb.cs;
   const float* __restrict__ sn = jb.sn;
   const int n = jb.n;
-  const size_t plane = jb.plane;
-  void* __restrict__ qo = jb.qo;
-  void* __restrict__ ko = jb.ko;
-  void* __restrict__ vo = jb.vo;
+  float* __restrict__ q = jb.qo;
+  float* __restrict__ k = jb.ko;
+  float* __restrict__ v = jb.vo;
   int i = blockIdx.x * blockDim.x + threadIdx.x;  // over n * 4 * 32 pairs
   if (i >= n * 128) return;
   int p = i & 31, h = (i >> 5) & 3, r = i >> 7;
-  const float* src = qkv + (size_t)r * 768 + (h * 64 + 2 * p) * 3;
-  float q0 = src[0], k0 = src[1], v0 = src[2], q1 = src[3], k1 = src[4], v1 = src[5];
+  const float* src = qkv + (size_t)r * 768 + h * 64 + 2 * p;
+  float q0 = src[0], q1 = src[1], k0 = src[256], k1 = src[257], v0 = src[512], v1 = src[513];
   float c = cs[r * 32 + p], s = sn[r * 32 + p];
   size_t o = ((size_t)h * n + r) * 64 + 2 * p;
   // (t * cos) + (rotate_half(t) * sin), rotate_half: (x1, x2) -> (-x2, x1)
   const float qa = __fadd_rn(__fmul_rn(q0, c), __fmul_rn(-q1, s)), qb = __fadd_rn(__fmul_rn(q1, c), __fmul_rn(q0, s));
   const float ka = __fadd_rn(__fmul_rn(k0, c), __fmul_rn(-k1, s)), kb = __fadd_rn(__fmul_rn(k1, c), __fmul_rn(k0, s));
-  if (SPLIT) {
-    __half* outs[3] = {static_cast<__half*>(qo), static_cast<__half*>(ko), static_cast<__half*>(vo)};
-    const float va[3] = {qa, ka, v0}, vb[3] = {qb, kb, v1};
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      __half ha, la, hb, lb;
-      if ((qk_unscaled >> (j < 2 ? 0 : 1)) & 1) {  // bit 0: q, k (single-accumulator logits); bit 1: v (k_flash_ts)
-        tc::split_h_unscaled(va[j], ha, la);
-        tc::split_h_unscaled(vb[j], hb, lb);
-      } else {
-        tc::split_h(va[j], ha, la);
-        tc::split_h(vb[j], hb, lb);
-      }
-      *reinterpret_cast<__half2*>(outs[j] + o) = __halves2half2(ha, hb);
-      *reinterpret_cast<__half2*>(outs[j] + plane + o) = __halves2half2(la, lb);
-    }
-  } else {
-    float *q = static_cast<float*>(qo), *k = static_cast<float*>(ko), *v = static_cast<float*>(vo);
-    q[o] = qa, q[o + 1] = qb, k[o] = ka, k[o + 1] = kb, v[o] = v0, v[o + 1] = v1;
-  }
+  q[o] = qa, q[o + 1] = qb, k[o] = ka, k[o + 1] = kb, v[o] = v0, v[o + 1] = v1;
 }
 
 // LayerNorm(512, eps 1e-5, affine) + exact GELU in place (lightglue.py:152-157). one warp per row.
@@ -570,6 +548,16 @@ __global__ void __launch_bounds__(1024) k_lg_filter(const float* __restrict__ be
 // host side
 // ------------------------------------------------------------------------------------------------------------------
 
+// Row r of the device copy of a self block's QKV projection (weight and bias) is row out[r] of the checkpoint's.  The
+// checkpoint interleaves q, k, v per feature, (h * 64 + j) * 3 + {q, k, v} (lightglue.py:166-167); the device copy is
+// [q | k | v], each 256 rows in head-major order h * 64 + j, so the rotary pair (2p, 2p + 1) of a head is two adjacent
+// output columns and each of q, k, v is one column segment of the GEMM.  Every output is the same dot product as before.
+extern "C" int b2_lightglue_qkv_rows(int* out) {
+  if (!out) return B2_ERR_ARG;
+  for (int r = 0; r < 3 * D; ++r) out[r] = (r % D) * 3 + r / D;
+  return B2_OK;
+}
+
 extern "C" int b2_lightglue_set_weights(b2_context* ctx, const float* blob, size_t n_floats) {
   if (!ctx || !blob) return B2_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
@@ -592,19 +580,30 @@ extern "C" int b2_lightglue_set_weights(b2_context* ctx, const float* blob, size
     for (size_t z : asz) sizes.push_back(z);
   }
   for (int i = 0; i < LG_LAYERS - 1; ++i) sizes.push_back(256), sizes.push_back(1);
+  // device placement: the blob order, except that each cross block's to_v weight goes right after its to_qk weight (and
+  // the biases likewise), so that [to_qk; to_v] is one [512][256] operand (a 256 x 256 tensor fills whole 64-float slots)
+  constexpr int SELF_T = 10, LAYER_T = 22;  // tensors per self block, per layer (self + cross)
+  std::vector<size_t> order(sizes.size());
+  for (size_t i = 0; i < order.size(); ++i) order[i] = i;
+  for (int i = 0; i < LG_LAYERS; ++i) std::swap(order[1 + LAYER_T * i + SELF_T + 1], order[1 + LAYER_T * i + SELF_T + 2]);
   size_t total = 0, src_total = 0;
-  std::vector<size_t> doff;
-  for (size_t z : sizes) {
-    doff.push_back(total);
-    total += (z + 63) / 64 * 64;
-    src_total += z;
+  std::vector<size_t> doff(sizes.size()), soff(sizes.size());
+  for (size_t k : order) {
+    doff[k] = total;
+    total += (sizes[k] + 63) / 64 * 64;
   }
+  for (size_t i = 0; i < sizes.size(); ++i) soff[i] = src_total, src_total += sizes[i];
   if (src_total != LG_NFLOATS) return b2_fail(ctx, B2_ERR_STATE, "internal lightglue layout mismatch");
   std::vector<float> host(total, 0.f);
-  size_t so = 0;
-  for (size_t i = 0; i < sizes.size(); ++i) {
-    memcpy(host.data() + doff[i], blob + so, sizes[i] * sizeof(float));
-    so += sizes[i];
+  for (size_t i = 0; i < sizes.size(); ++i) memcpy(host.data() + doff[i], blob + soff[i], sizes[i] * sizeof(float));
+  int qkv_rows[3 * D];
+  b2_lightglue_qkv_rows(qkv_rows);
+  for (int i = 0; i < LG_LAYERS; ++i) {  // self QKV weight and bias rows -> [q | k | v]
+    const size_t tw = 1 + LAYER_T * i, tb = tw + 1;
+    for (int r = 0; r < 3 * D; ++r) {
+      memcpy(host.data() + doff[tw] + (size_t)r * D, blob + soff[tw] + (size_t)qkv_rows[r] * D, D * sizeof(float));
+      host[doff[tb] + r] = blob[soff[tb] + qkv_rows[r]];
+    }
   }
   B2_CUDA(ctx, s->wblob.ensure(total * sizeof(float)));
   B2_CUDA(ctx, cudaMemcpy(s->wblob.p, host.data(), total * sizeof(float), cudaMemcpyHostToDevice));
@@ -617,8 +616,8 @@ extern "C" int b2_lightglue_set_weights(b2_context* ctx, const float* blob, size
     a.wqkv = next(), a.bqkv = next(), a.wout = next(), a.bout = next(), a.w0 = next(), a.b0 = next(), a.lng = next(),
     a.lnb = next(), a.w3 = next(), a.b3 = next();
     CrossW& c = s->cw[i];
-    c.wqk = next(), c.bqk = next(), c.wv = next(), c.bv = next(), c.wout = next(), c.bout = next(), c.w0 = next(),
-    c.b0 = next(), c.lng = next(), c.lnb = next(), c.w3 = next(), c.b3 = next();
+    c.wqv = next(), c.bqv = next(), next(), next();  // to_v's weight and bias sit right behind to_qk's
+    c.wout = next(), c.bout = next(), c.w0 = next(), c.b0 = next(), c.lng = next(), c.lnb = next(), c.w3 = next(), c.b3 = next();
   }
   for (int i = 0; i < LG_LAYERS; ++i) {
     AssignW& a = s->aw[i];
@@ -657,7 +656,7 @@ static inline TcWeights lg_tw(LightGlueState* s) {
   return t;
 }
 
-static int lg_side_alloc(b2_context* ctx, LgSide& sd, int n) {
+static int lg_side_alloc(b2_context* ctx, LgSide& sd, int n, bool use_tc) {
   const size_t N = (size_t)(n > 0 ? n : 1);
   for (int i = 0; i < 2; ++i) {
     B2_CUDA(ctx, sd.x[i].ensure(N * 256 * 4));
@@ -666,7 +665,7 @@ static int lg_side_alloc(b2_context* ctx, LgSide& sd, int n) {
     B2_CUDA(ctx, sd.sn[i].ensure(N * 32 * 4));
     B2_CUDA(ctx, sd.ind[i].ensure(N * 4));
   }
-  B2_CUDA(ctx, sd.qkv.ensure(N * 768 * 4));
+  if (!use_tc) B2_CUDA(ctx, sd.qkv.ensure(N * 768 * 4));  // the wgmma path writes q / k / v from the projection directly
   B2_CUDA(ctx, sd.q.ensure(N * 256 * 4));
   B2_CUDA(ctx, sd.k.ensure(N * 256 * 4));
   B2_CUDA(ctx, sd.v.ensure(N * 256 * 4));
@@ -702,8 +701,10 @@ static int lg_max_n(const LightGlueState* s, const LgActive& act) {
 
 // x + ffn(cat[x, msg])  (lightglue.py:152-157,172,228-229): Linear(512,512) -> LN -> GELU -> Linear(512,256) + x, preceded
 // by the attention output projection (out_proj / to_out); every image of the batch goes through each GEMM together.
-static int lg_out_and_ffn(b2_context* ctx, cudaStream_t st, LightGlueState* s, const LgActive& act, const float* wout, const float* bout,
-                          const float* w0, const float* b0, const float* lng, const float* lnb, const float* w3, const float* b3) {
+// `blk` ("lg_self" / "lg_cross") prefixes the profiler labels of the three GEMM call sites.
+static int lg_out_and_ffn(b2_context* ctx, cudaStream_t st, LightGlueState* s, const LgActive& act, const char* blk, const float* wout,
+                          const float* bout, const float* w0, const float* b0, const float* lng, const float* lnb, const float* w3,
+                          const float* b3) {
   int rc;
   const TcWeights tw = lg_tw(s);
   LinArgs o[LG_MAX_SIDES], f0[LG_MAX_SIDES], f3[LG_MAX_SIDES];
@@ -723,8 +724,9 @@ static int lg_out_and_ffn(b2_context* ctx, cudaStream_t st, LightGlueState* s, c
     c.resid = x, c.ldr = 256;  // in place: every element is read (as residual) and written by the same thread
     c.cf = x, c.ldc = 256, c.tc_want_f32 = true, c.cp = planes_of(sd.xs[sd.cur], e), c.ldch = 256, c.M = sd.n, c.N = 256;
   }
-  if ((rc = run_linear(ctx, st, tw, o, act.n))) return rc;
-  if ((rc = run_linear(ctx, st, tw, f0, act.n))) return rc;
+  const std::string site(blk);
+  if ((rc = run_linear(ctx, st, tw, o, act.n, (site + "_out").c_str()))) return rc;
+  if ((rc = run_linear(ctx, st, tw, f0, act.n, (site + "_ffn0").c_str()))) return rc;
   {
     JobList<LnJob> lj{};
     for (int i = 0; i < act.n; ++i) {
@@ -738,35 +740,40 @@ static int lg_out_and_ffn(b2_context* ctx, cudaStream_t st, LightGlueState* s, c
       B2_CHECK_LAUNCH(ctx);
     }
   }
-  return run_linear(ctx, st, tw, f3, act.n);
+  return run_linear(ctx, st, tw, f3, act.n, (site + "_ffn3").c_str());
 }
 
 static int lg_self_layer(b2_context* ctx, cudaStream_t st, LightGlueState* s, const LgActive& act, int layer, bool fp16_attn) {
   const SelfW& w = s->sw[layer];
   const TcWeights tw = lg_tw(s);
   int rc;
+  // wgmma path: one launch writes rotated q, k and unrotated v as head-major planes with unscaled lo (attention operands);
+  // SIMT path: qkv fp32 [N][768], then the rotary kernel
   LinArgs q[LG_MAX_SIDES];
   for (int i = 0; i < act.n; ++i) {
     LgSide& sd = s->side[act.side[i]];
+    const size_t e = (size_t)sd.cap * 256;
     LinArgs& a = q[i];
-    a.a1f = sd.x[sd.cur].as<float>(), a.a1p = planes_of(sd.xs[sd.cur], (size_t)sd.cap * 256), a.lda1 = 256, a.K1 = 256;
-    a.w = w.wqkv, a.ldb = 256, a.bias = w.bqkv, a.cf = sd.qkv.as<float>(), a.ldc = 768, a.tc_want_f32 = true, a.M = sd.n, a.N = 768;
+    a.a1f = sd.x[sd.cur].as<float>(), a.a1p = planes_of(sd.xs[sd.cur], e), a.lda1 = 256, a.K1 = 256;
+    a.w = w.wqkv, a.ldb = 256, a.bias = w.bqkv, a.M = sd.n, a.N = 768;
+    if (s->use_tc) {
+      a.seg_n = 256, a.seg_p[0] = planes_of(sd.q, e), a.seg_p[1] = planes_of(sd.k, e), a.seg_p[2] = planes_of(sd.v, e);
+      a.rot_mask = 3, a.cs = sd.cs[sd.cur].as<float>(), a.sn = sd.sn[sd.cur].as<float>();
+      a.head_major = 1, a.lo_unscaled = 1;
+    } else {
+      a.cf = sd.qkv.as<float>(), a.ldc = 768;
+    }
   }
-  if ((rc = run_linear(ctx, st, tw, q, act.n))) return rc;
-  {
+  if ((rc = run_linear(ctx, st, tw, q, act.n, "lg_self_qkv"))) return rc;
+  const int mx = lg_max_n(s, act);
+  if (!s->use_tc && mx > 0) {
     JobList<RotJob> rj{};
     for (int i = 0; i < act.n; ++i) {
       LgSide& sd = s->side[act.side[i]];
-      rj.j[i] = {sd.qkv.as<float>(), sd.cs[sd.cur].as<float>(), sd.sn[sd.cur].as<float>(), sd.n, (size_t)sd.cap * 256, sd.q.p, sd.k.p, sd.v.p};
+      rj.j[i] = {sd.qkv.as<float>(), sd.cs[sd.cur].as<float>(), sd.sn[sd.cur].as<float>(), sd.n, sd.q.as<float>(), sd.k.as<float>(), sd.v.as<float>()};
     }
-    const int mx = lg_max_n(s, act);
-    if (mx > 0) {
-      if (s->use_tc)  // q, k, v all feed the wgmma attention: unscaled lo planes (bits 0 and 1)
-        B2_LAUNCH(ctx, k_lg_split_rotary<true>, dim3(cdiv(mx * 128, 256), act.n), 256, 0, st, rj, 3);
-      else
-        B2_LAUNCH(ctx, k_lg_split_rotary<false>, dim3(cdiv(mx * 128, 256), act.n), 256, 0, st, rj, 0);
-      B2_CHECK_LAUNCH(ctx);
-    }
+    B2_LAUNCH(ctx, k_lg_split_rotary, dim3(cdiv(mx * 128, 256), act.n), 256, 0, st, rj);
+    B2_CHECK_LAUNCH(ctx);
   }
   FlashJob fj[LG_MAX_SIDES];
   for (int i = 0; i < act.n; ++i) {
@@ -774,27 +781,24 @@ static int lg_self_layer(b2_context* ctx, cudaStream_t st, LightGlueState* s, co
     fj[i] = {&a.q, &a.k, &a.v, &a.ctx, a.n, a.n, a.cap, a.cap};
   }
   if ((rc = run_flash(ctx, st, tw, fj, act.n, 0.125f, fp16_attn))) return rc;
-  return lg_out_and_ffn(ctx, st, s, act, w.wout, w.bout, w.w0, w.b0, w.lng, w.lnb, w.w3, w.b3);
+  return lg_out_and_ffn(ctx, st, s, act, "lg_self", w.wout, w.bout, w.w0, w.b0, w.lng, w.lnb, w.w3, w.b3);
 }
 
 static int lg_cross_block(b2_context* ctx, cudaStream_t st, LightGlueState* s, const LgActive& act, int layer, bool fp16_attn) {
   const CrossW& w = s->cw[layer];
   const TcWeights tw = lg_tw(s);
   int rc;
-  for (int which = 0; which < 2; ++which) {  // to_qk -> sd.q, to_v -> sd.v, both head-major [4][n][64]
-    LinArgs p[LG_MAX_SIDES];
-    for (int i = 0; i < act.n; ++i) {
-      LgSide& sd = s->side[act.side[i]];
-      const size_t e = (size_t)sd.cap * 256;
-      LinArgs& a = p[i];
-      a.a1f = sd.x[sd.cur].as<float>(), a.a1p = planes_of(sd.xs[sd.cur], e), a.lda1 = 256, a.K1 = 256;
-      a.w = which ? w.wv : w.wqk, a.ldb = 256, a.bias = which ? w.bv : w.bqk;
-      DevBuf& dst = which ? sd.v : sd.q;
-      a.cf = dst.as<float>(), a.cp = planes_of(dst, e), a.head_major = 1, a.M = sd.n, a.N = 256;
-      a.lo_unscaled = s->use_tc ? 1 : 0;  // attention operands
-    }
-    if ((rc = run_linear(ctx, st, tw, p, act.n))) return rc;
+  LinArgs p[LG_MAX_SIDES];  // [to_qk; to_v] in one launch: columns 0-255 -> sd.q, 256-511 -> sd.v, both head-major [4][n][64]
+  for (int i = 0; i < act.n; ++i) {
+    LgSide& sd = s->side[act.side[i]];
+    const size_t e = (size_t)sd.cap * 256;
+    LinArgs& a = p[i];
+    a.a1f = sd.x[sd.cur].as<float>(), a.a1p = planes_of(sd.xs[sd.cur], e), a.lda1 = 256, a.K1 = 256;
+    a.w = w.wqv, a.ldb = 256, a.bias = w.bqv, a.head_major = 1, a.M = sd.n, a.N = 512;
+    a.seg_n = 256, a.seg_f[0] = sd.q.as<float>(), a.seg_f[1] = sd.v.as<float>(), a.seg_p[0] = planes_of(sd.q, e), a.seg_p[1] = planes_of(sd.v, e);
+    a.lo_unscaled = s->use_tc ? 1 : 0;  // attention operands
   }
+  if ((rc = run_linear(ctx, st, tw, p, act.n, "lg_cross_qv"))) return rc;
   // m0 = softmax(s * qk0 qk1^T) v1 ; m1 = softmax(s * qk1 qk0^T) v0 with s = 64^-0.5 (the reference scales each
   // operand by 64^-0.25, lightglue.py:216-221); both directions of every pair in one launch
   FlashJob fj[LG_MAX_SIDES];
@@ -803,7 +807,7 @@ static int lg_cross_block(b2_context* ctx, cudaStream_t st, LightGlueState* s, c
     fj[i] = {&a.q, &b.q, &b.v, &a.ctx, a.n, b.n, a.cap, b.cap};
   }
   if ((rc = run_flash(ctx, st, tw, fj, act.n, 0.125f, fp16_attn))) return rc;
-  return lg_out_and_ffn(ctx, st, s, act, w.wout, w.bout, w.w0, w.b0, w.lng, w.lnb, w.w3, w.b3);
+  return lg_out_and_ffn(ctx, st, s, act, "lg_cross", w.wout, w.bout, w.w0, w.b0, w.lng, w.lnb, w.w3, w.b3);
 }
 
 // One batch of up to LG_MAX_PAIRS pairs walked in lock-step (lightglue.py:474-629 for each of them).
@@ -820,8 +824,8 @@ static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, con
       s->side[2 * p].n = s->side[2 * p + 1].n = 0;
       continue;
     }
-    if ((rc = lg_side_alloc(ctx, s->side[2 * p], pr.n0))) return rc;
-    if ((rc = lg_side_alloc(ctx, s->side[2 * p + 1], pr.n1))) return rc;
+    if ((rc = lg_side_alloc(ctx, s->side[2 * p], pr.n0, s->use_tc))) return rc;
+    if ((rc = lg_side_alloc(ctx, s->side[2 * p + 1], pr.n1, s->use_tc))) return rc;
   }
   LgActive act = lg_active_sides(s, np);
   if (act.n == 0) return B2_OK;
@@ -943,7 +947,7 @@ static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, con
       }
     }
     if (ns == 0) continue;
-    if ((rc = run_linear(ctx, st, tw, g, ns))) return rc;
+    if ((rc = run_linear(ctx, st, tw, g, ns, "lg_assign_proj"))) return rc;
     B2_LAUNCH(ctx, k_lg_rowheads, dim3(cdiv(mx, 8), ns), 256, 0, st, hj, (const float*)nullptr, (const float*)nullptr);
     B2_CHECK_LAUNCH(ctx);
   }
@@ -958,7 +962,7 @@ static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, con
       g.bf = b.md.as<float>(), g.bp = planes_of(b.md, (size_t)b.cap * 256), g.ldb = 256;
       g.cf = s->sim[p].as<float>(), g.ldc = b.n, g.tc_want_f32 = true, g.M = a.n, g.N = b.n;
     }
-    if ((rc = run_linear(ctx, st, tw, gs, nlive))) return rc;
+    if ((rc = run_linear(ctx, st, tw, gs, nlive, "lg_assign_sim"))) return rc;
   }
   for (int li = 0; li < nlive; ++li) {
     const int p = live[li];

@@ -52,30 +52,50 @@ struct LinArgs {
   int gelu = 0;  // exact GELU after bias / scale, before the residual (wgmma path only)
   int lo_unscaled = 0;  // plane output with an unscaled lo plane (attention operands)
   int M = 0, N = 0;
+  // Column segments (seg_n > 0, N = seg_n x segments, head_major): columns s seg_n .. (s + 1) seg_n - 1 go to seg_f[s]
+  // (SIMT path) or seg_p[s] (wgmma path) instead of cf / cp.  rot_mask bit s applies rotary (cos / sin [M][32]) to
+  // segment s; only the wgmma path has it.
+  int seg_n = 0;
+  float* seg_f[GW_SEGS] = {};
+  Pl seg_p[GW_SEGS] = {};
+  int rot_mask = 0;
+  const float *cs = nullptr, *sn = nullptr;
 };
 
 // `a[0 .. np)`: the same linear applied to np problems.  With a weight operand (a[0].w) every problem shares weights, K,
 // N and epilogue, and the wgmma path runs them as ONE persistent launch; with activation B operands (a[i].bf / bp: the
 // assignment similarity of each pair) N, ldc and B are per problem, K and the epilogue flags are a[0]'s.
-static int run_linear(b2_context* ctx, cudaStream_t st, const TcWeights& tw, const LinArgs* a, int np) {
+// `site` labels the launch for the profiler: it matches "k_gemm_ws/<site>" (and so the prefix "k_gemm_ws").
+static int run_linear(b2_context* ctx, cudaStream_t st, const TcWeights& tw, const LinArgs* a, int np, const char* site = nullptr) {
   if (np <= 0) return B2_OK;
   if (np > GW_MAXP) return b2_fail(ctx, B2_ERR_ARG, "run_linear: too many problems in one launch");
+  const LinArgs& a0 = a[0];
+  const int nseg = a0.seg_n > 0 ? a0.N / a0.seg_n : 1;
+  if (a0.seg_n > 0 && (a0.seg_n % GW_N || a0.N != nseg * a0.seg_n || nseg > GW_SEGS || !a0.head_major || a0.resid || a0.tc_want_f32 ||
+                       (a0.rot_mask && (!a0.cs || !a0.sn))))
+    return b2_fail(ctx, B2_ERR_ARG, "run_linear: column segments need N = seg_n x (<= 3), seg_n % 128 == 0, head-major planes, "
+                                    "no residual or fp32 output, and a rotary table when rotary is on");
   if (!tw.use_tc) {
+    if (a0.rot_mask) return b2_fail(ctx, B2_ERR_ARG, "run_linear: the rotary epilogue exists on the wgmma path only");
     for (int i = 0; i < np; ++i) {
       const LinArgs& x = a[i];
       if (x.M <= 0 || x.N <= 0) continue;
       if (x.gelu) return b2_fail(ctx, B2_ERR_ARG, "run_linear: the GELU epilogue exists on the wgmma path only");
-      GemmArgs g{};
-      g.A1 = x.a1f, g.lda1 = x.lda1, g.K1 = x.K1, g.A2 = x.a2f, g.lda2 = x.lda2, g.K2 = x.K2;
-      g.B = x.w ? x.w : x.bf, g.ldb = x.ldb, g.C = x.cf, g.ldc = x.ldc, g.M = x.M, g.N = x.N;
-      g.bias = x.bias, g.resid = x.resid, g.ldr = x.ldr, g.scale = x.scale, g.head_major = x.head_major, g.relu = x.relu;
-      int rc = launch_gemm(ctx, st, g);
-      if (rc) return rc;
+      for (int s = 0; s < nseg; ++s) {  // a segmented linear runs one launch per segment here
+        const int c0 = s * x.seg_n;
+        GemmArgs g{};
+        g.A1 = x.a1f, g.lda1 = x.lda1, g.K1 = x.K1, g.A2 = x.a2f, g.lda2 = x.lda2, g.K2 = x.K2;
+        g.B = (x.w ? x.w : x.bf) + (size_t)c0 * x.ldb, g.ldb = x.ldb, g.C = x.seg_n ? x.seg_f[s] : x.cf, g.ldc = x.ldc, g.M = x.M;
+        g.N = x.seg_n ? x.seg_n : x.N;
+        g.bias = x.bias ? x.bias + c0 : nullptr, g.resid = x.resid, g.ldr = x.ldr, g.scale = x.scale, g.head_major = x.head_major;
+        g.relu = x.relu;
+        int rc = launch_gemm(ctx, st, g);
+        if (rc) return rc;
+      }
     }
     return B2_OK;
   }
   if (!tma_encoder()) return b2_fail(ctx, B2_ERR_CUDA, "cuTensorMapEncodeTiled is not available (driver too old?)");
-  const LinArgs& a0 = a[0];
   const bool per_b = a0.w == nullptr;
   static thread_local GemmWsMaps maps;  // 12 KB: keep it off the stack of deep call chains
   GemmWsArgs q{};
@@ -99,13 +119,23 @@ static int run_linear(b2_context* ctx, cudaStream_t st, const TcWeights& tw, con
       ok = ok && tma_map_2d(&maps.bh[nz], bh, x.N, x.K1 + x.K2, x.ldb, GW_N) && tma_map_2d(&maps.bl[nz], bl, x.N, x.K1 + x.K2, x.ldb, GW_N);
     }
     GemmProblem& pr = q.p[nz];
-    pr.resid = x.resid, pr.C = x.tc_want_f32 ? x.cf : nullptr, pr.Ch = x.cp.hi, pr.Cl = x.cp.lo, pr.M = x.M, pr.N = x.N, pr.ldc = x.ldc;
+    pr.resid = x.resid, pr.C = x.tc_want_f32 ? x.cf : nullptr, pr.M = x.M, pr.N = x.N, pr.ldc = x.ldc;
+    for (int s = 0; s < GW_SEGS; ++s) {
+      const Pl p = x.seg_n ? (s < nseg ? x.seg_p[s] : Pl{nullptr, nullptr}) : (s == 0 ? x.cp : Pl{nullptr, nullptr});
+      pr.Ch[s] = p.hi, pr.Cl[s] = p.lo;
+    }
+    pr.cs = x.cs, pr.sn = x.sn;
     {  // 16-byte accesses in the epilogue need aligned bases and leading dimensions
       auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+      auto al8 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 7) == 0; };
       const bool hm = x.head_major != 0;
       bool v = al16(pr.resid) && (x.ldr % 4 == 0 || !pr.resid) && al16(pr.C) && (hm || x.ldc % 4 == 0 || !pr.C);
-      v = v && (reinterpret_cast<uintptr_t>(pr.Ch) & 7) == 0 && (reinterpret_cast<uintptr_t>(pr.Cl) & 7) == 0 && (hm || x.ldch % 4 == 0 || !pr.Ch);
+      v = v && (hm || x.ldch % 4 == 0 || !pr.Ch[0]);
+      for (int s = 0; s < GW_SEGS; ++s) v = v && al8(pr.Ch[s]) && al8(pr.Cl[s]);
+      v = v && al8(pr.cs) && al8(pr.sn);
       pr.vec4 = v ? 1 : 0;
+      // segments are written 4 columns at a time only (a rotary pair must not be split across the per-element path)
+      if (x.seg_n && !v) return b2_fail(ctx, B2_ERR_ARG, "run_linear: column segments need 8-byte aligned planes and rotary tables");
     }
     pr.tiles_n = cdiv(x.N, GW_N);
     tiles += cdiv(x.M, GW_M) * pr.tiles_n;
@@ -118,8 +148,10 @@ static int run_linear(b2_context* ctx, cudaStream_t st, const TcWeights& tw, con
   q.nprob = nz, q.tiles = tiles, q.K1 = a0.K1, q.K2 = a0.K2, q.b_per_problem = per_b ? 1 : 0;
   q.bias = a0.bias, q.ldr = a0.ldr, q.scale = a0.scale, q.ldch = a0.ldch;
   q.head_major = a0.head_major, q.relu = a0.relu, q.gelu = a0.gelu, q.lo_unscaled = a0.lo_unscaled, q.err_flag = tw.err;
-  b2_prof_work(ctx, "k_gemm_ws", work);
-  B2_LAUNCH(ctx, k_gemm_ws, tiles < tw.sm_count ? tiles : tw.sm_count, GW_THREADS, GW_SMEM, st, maps, q);
+  q.seg_n = a0.seg_n, q.rot_mask = a0.rot_mask;
+  const std::string name = site ? std::string("k_gemm_ws/") + site : std::string("k_gemm_ws");
+  b2_prof_work(ctx, name.c_str(), work);
+  B2_LAUNCH_NAMED(ctx, name.c_str(), k_gemm_ws, tiles < tw.sm_count ? tiles : tw.sm_count, GW_THREADS, GW_SMEM, st, maps, q);
   B2_CHECK_LAUNCH(ctx);
   return B2_OK;
 }

@@ -69,6 +69,13 @@ int64_t b2_debug_fetch(b2_context* ctx, const char* name, float* host_out, int64
  * kernel with fp32 B converted in-kernel, 2 = wgmma split-fp16 kernel with pre-split fp16 B.  K must be a multiple of 64. */
 int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, const float* B, const float* bias, float* C, int M, int N,
                        int K);
+/* Test-only: the wgmma GEMM's column-segment epilogue on HOST fp32 buffers.  A [M][K], B [256 nseg][K], bias [256 nseg]
+ * (1 <= nseg <= 3, K a multiple of 64); output columns 256 s .. 256 s + 255 go to segment s of out_hi / out_lo, each
+ * [nseg][4][M][64] fp16 bits (head-major, unscaled lo).  Segments with a rot_mask bit get rotary from cs / sn [M][32].
+ * separate = 1 runs each segment as a launch of its own instead (rot_mask must then be 0). */
+int b2_debug_gemm_segments_host(b2_context* ctx, const float* A, const float* B, const float* bias, int M, int K, int nseg,
+                                int rot_mask, const float* cs, const float* sn, int separate, uint16_t* out_hi,
+                                uint16_t* out_lo);
 /* Test-only: one batched launch of the wgmma flash attention on HOST fp32 buffers.  Problem z (0 <= z < np <= 16) has
  * nq[z] queries, nk[z] keys and `heads` heads of 64: q as [heads][nq[z]][64], k and v as [heads][nk[z]][64] (head-major),
  * each concatenated over z; o receives softmax(scale * q k^T) v as [nq[z]][64 * heads] per problem, concatenated over z.
@@ -133,6 +140,10 @@ int b2_image_resize_dev(b2_context* ctx, const uint8_t* src, int height, int wid
  * (out,in) row-major as in the checkpoint).  n_floats must equal 11851601 (the 251 parameter tensors; the
  * confidence_thresholds buffer is recomputed). */
 int b2_lightglue_set_weights(b2_context* ctx, const float* host_blob, size_t n_floats);
+/* Host-only, needs no device: out[r] (768 ints) = the checkpoint row of each self block's QKV projection that the device
+ * copy holds at row r.  The device copy is [q | k | v], 256 rows each in head-major order h * 64 + j; the checkpoint
+ * interleaves them as (h * 64 + j) * 3 + {q, k, v}. */
+int b2_lightglue_qkv_rows(int* out);
 
 typedef struct b2_lightglue_params {
   /* doubles on purpose: the reference holds these as Python floats and rounds the DERIVED value to float32 at the
