@@ -54,6 +54,11 @@ class D2NetImage(C.Structure):
                 ("out_desc", C.c_void_p), ("out_n", C.c_int), ("out_total", C.c_int)]
 
 
+class JpegImage(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("size", C.c_size_t), ("out", C.c_void_p), ("out_pitch", C.c_size_t), ("out_status", C.c_int),
+                ("out_rounds", C.c_int)]
+
+
 SIFT_CAPACITY = -5  # b2_sift_detect_host: more keypoints than the capacity; *out_n holds the count needed
 
 
@@ -124,6 +129,9 @@ SIGNATURES = {
     "b2_debug_conv_ps_host": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
     "b2_debug_d2net_avgpool_host": (_i, [_vp, _vp, _i, _i, _vp]),
     "b2_debug_d2net_rank_host": (_i, [_vp, _vp, _vp, _i, _i, _vp]),
+    "b2_jpeg_status_string": (C.c_char_p, [_i]),
+    "b2_jpeg_info_host": (_i, [_vp, _sz, _ip, _ip, _ip]),
+    "b2_jpeg_decode_batched_dev": (_i, [_vp, C.POINTER(JpegImage), _i, _vp]),
 }
 
 

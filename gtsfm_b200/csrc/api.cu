@@ -39,6 +39,7 @@ extern "C" void b2_destroy(b2_context* ctx) {
   sf_destroy(ctx);
   ml_destroy(ctx);
   d2_destroy(ctx);
+  jp_destroy(ctx);
   for (cudaEvent_t e : ctx->prof.ev) cudaEventDestroy(e);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   delete ctx;

@@ -100,6 +100,7 @@ struct MnnState;
 struct SiftState;
 struct MegaLocState;
 struct D2NetState;
+struct JpegState;
 
 // Device copies of host feature arrays handed to the *_host matcher entry points.  GTSfM matches one image's (keypoints,
 // descriptors) against ~20-40 partners, always passing the same host arrays, so re-uploading 5 MB per image per pair is
@@ -138,6 +139,7 @@ struct b2_context {
   SiftState* sf = nullptr;
   MegaLocState* ml = nullptr;
   D2NetState* d2 = nullptr;
+  JpegState* jp = nullptr;
   // staging shared by the *_host entry points
   DevBuf stage_d[8];
   HostBuf stage_h[4];
@@ -209,6 +211,7 @@ void mn_destroy(b2_context* ctx);
 void sf_destroy(b2_context* ctx);
 void ml_destroy(b2_context* ctx);
 void d2_destroy(b2_context* ctx);
+void jp_destroy(b2_context* ctx);
 
 // shared device helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

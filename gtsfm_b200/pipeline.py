@@ -117,6 +117,16 @@ class DeviceFrontEnd:
         self.ctx.check(rc, "image_resize_dev")
         return out
 
+    def ingest_jpeg(self, datas: Sequence[bytes], max_resolution: int = 760) -> List[torch.Tensor]:
+        """JPEG file bytes -> device RGB frames (the pixels PIL would give, image_io.JpegEngine) -> `ingest`'s cubic down-size:
+        a loader's files reach `detect` / `detect_many` without the pixels touching the host.  ValueError for a file the
+        device decoder does not accept."""
+        if getattr(self, "_jpeg", None) is None:
+            from .image_io import JpegEngine
+
+            self._jpeg = JpegEngine(self.device.index, ctx=self.ctx)
+        return [self.ingest(f, max_resolution) for f in self._jpeg.decode_many(datas)]
+
     def detect(self, image: torch.Tensor, mask: Optional[np.ndarray] = None) -> DeviceFeatures:
         """image: uint8 device tensor (H, W) or (H, W, 3|4), contiguous.  One C call (detect -> device top-k -> describe): no
         torch kernels on the path, and the dense map never outlives the call (interleaving images on one handle is safe).

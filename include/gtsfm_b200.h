@@ -377,6 +377,35 @@ int b2_debug_conv_ps_host(b2_context* ctx, int dilation, const float* in, int he
 int b2_debug_d2net_avgpool_host(b2_context* ctx, const float* in, int height, int width, float* out);
 int b2_debug_d2net_rank_host(b2_context* ctx, const float* scores, const int* cij, int n, int max_k, int* order);
 
+/* ---- baseline JPEG decode (gtsfm/utils/io.py:39-72 load_image: np.asarray(PIL.Image.open(f).convert("RGB"))) --------------------
+ * Output equals PIL's (libjpeg-turbo defaults: islow IDCT, fancy upsampling, jdcolor.c's fixed-point YCbCr -> RGB) bit for bit.
+ * Scope: SOF0 / SOF1, 8-bit, Huffman coded, one scan holding every component: 3-component YCbCr with luma sampling h1v1, h2v1,
+ * h1v2 or h2v2 and chroma 1x1, or 1-component gray (replicated to three channels); optional restart intervals; any size.
+ * EXIF orientation is not applied.  Everything else is refused with a status naming it:
+ *   -2 beyond the limits (a side over 16384, over 2^26 pixels, a file over 256 MiB, or an output pitch under 3 W)
+ *   -10 not a JPEG / corrupt header, -11 progressive, -12 arithmetic coding, -13 lossless or hierarchical, -14 not 8-bit,
+ *   -15 not 1 or 3 components (CMYK / YCCK), -16 RGB colour space (Adobe transform 0, or component ids R G B without JFIF),
+ *   -17 other sampling factors, -18 multi-scan, -19 DNL, -20 truncated (no EOI after the scan), -21 corrupt entropy-coded data
+ *   (invalid code, coefficient index past 63, wrong MCU count, restart marker out of sequence), -22 a Huffman table with an
+ *   all-ones code (which encoders never write).
+ * b2_jpeg_status_string(code) gives the text of a status. */
+const char* b2_jpeg_status_string(int code);
+/* Header only (markers up to SOS, plus the presence of an EOI after the scan): no context, no GPU.  0 or a status above. */
+int b2_jpeg_info_host(const uint8_t* data, size_t size, int* height, int* width, int* components);
+typedef struct b2_jpeg_image {
+  const uint8_t* data; /* HOST file bytes */
+  size_t size;
+  uint8_t* out;        /* DEVICE H x W x 3 uint8, row pitch out_pitch bytes (>= 3 W) */
+  size_t out_pitch;
+  int out_status;      /* written on the HOST struct: 0, or a status above (nothing is written to `out`) */
+  int out_rounds;      /* written on the HOST struct: synchronisation rounds the entropy decode took (9 = serial fallback) */
+} b2_jpeg_image;
+/* Up to 256 images of any sizes and sampling factors.  The compressed bytes go up in one copy through pinned staging, every
+ * stage is one launch over the batch, and `stream` is synchronised once.  Returns 0 when the batch ran (per-image results in
+ * out_status), -2 for more than 256 images.  Workspace: 2 bytes per coefficient (64 per block) plus the MCU-padded component planes, about 4.5 bytes per pixel at 4:2:0
+ * and 9 at 4:4:4, plus about 3 x the compressed size. */
+int b2_jpeg_decode_batched_dev(b2_context* ctx, b2_jpeg_image* images, int n_images, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
