@@ -84,6 +84,9 @@ SIGNATURES = {
     "b2_debug_gemm_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i]),
     "b2_debug_gemm_segments_host": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "b2_debug_attention_host": (_i, [_vp, _i, _ip, _ip, _i, _f, _i, _vp, _vp, _vp, _vp]),
+    "b2_debug_superglue_assign_host": (_i, [_vp, _i, _i, _vp, _i, _i, _f, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ip, _ip]),
+    "b2_debug_lightglue_assign_host": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ip,
+                                            _ip]),
     "b2_superpoint_set_weights": (_i, [_vp, _vp, _sz]),
     "b2_superpoint_detect_dev": (_i, [_vp, _vp, _i, _i, _i, _sz, _f, _i, _i, _vp, _vp, _i, _ip, C.POINTER(C.c_uint64), _vp]),
     "b2_superpoint_describe_dev": (_i, [_vp, C.c_uint64, _vp, _i, _vp, _vp]),

@@ -548,6 +548,65 @@ __global__ void __launch_bounds__(1024) k_lg_filter(const float* __restrict__ be
 // host side
 // ------------------------------------------------------------------------------------------------------------------
 
+// The assignment step on the similarity sim [M][N]: the row / column log-softmax statistics and logsigmoid terms of
+// sigmoid_log_double_softmax (lightglue.py:265-277), the mutual arg-max and threshold of filter_matches (:302-318), and
+// the match list mapped through ind0 / ind1 (:598-602).
+struct LgStats {
+  float *max, *log, *lsg;  // per row (or column): max, log of the sum of exp(x - max), logsigmoid of the matchability logit
+};
+struct LgAssign {
+  const float* sim;
+  int M, N;
+  const float *z0, *z1;  // matchability logits [M], [N]
+  const int *ind0, *ind1;
+  float thr;
+  LgStats r, c;
+  float* best0;
+  int *arg0, *arg1;
+  DevBuf *part, *bar;  // scratch of the persistent kernel
+  int* err_flag;
+  long long* out_matches;
+  float* out_scores;
+  int* count;
+};
+
+// path 0 runs the persistent kernel when it fits (what the matcher does), 1 forces it, 2 forces the multi-launch passes; G
+// is the persistent kernel's CTA count.  *ran (when given) receives the path that ran, 1 or 2.
+static int lg_assign(b2_context* ctx, cudaStream_t st, const LgAssign& p, int path, int G, int* ran) {
+  const float* sim = p.sim;
+  const int M = p.M, N = p.N;
+  const bool persistent = path == 0 ? assign_ps_fits(1, N) : path == 1;
+  if (persistent && !assign_ps_fits(1, N)) return b2_fail(ctx, B2_ERR_ARG, "the persistent assignment kernel holds at most 6240 columns");
+  if (ran) *ran = persistent ? 1 : 2;
+  int rc;
+  if (persistent) {
+    // persistent cooperative kernel (assign_ps.cuh, KIND 1): row / column log-softmax statistics in one sweep of the
+    // similarity, mutual arg-max in a second one - 2 reads and 1 launch instead of 4 and 4
+    B2_CUDA(ctx, p.part->ensure((size_t)G * 2 * N * sizeof(float)));
+    B2_CUDA(ctx, p.bar->ensure(16));
+    B2_CUDA(ctx, cudaMemsetAsync(p.bar->p, 0, 16, st));
+    SinkArgs sa{};
+    sa.Z = sim, sa.M = M, sa.N = N, sa.iters = 1, sa.u = p.r.max, sa.v = p.c.max;
+    sa.rlog = p.r.log, sa.clog = p.c.log, sa.z0 = p.z0, sa.z1 = p.z1;
+    sa.lsg0 = p.r.lsg, sa.lsg1 = p.c.lsg, sa.part = p.part->as<float>(), sa.bar = p.bar->as<unsigned>();
+    sa.best0 = p.best0, sa.arg0 = p.arg0, sa.arg1 = p.arg1, sa.err_flag = p.err_flag;
+    if ((rc = launch_assign_ps<1>(ctx, st, sa, G, "k_lg_assign"))) return rc;
+  } else {
+    B2_LAUNCH(ctx, k_lg_row_stats, cdiv(M, 8), 256, 0, st, sim, M, N, p.r.max, p.r.log, p.z0, p.r.lsg);
+    B2_CHECK_LAUNCH(ctx);
+    B2_LAUNCH(ctx, k_lg_col_stats, cdiv(N, 32), 1024, 0, st, sim, M, N, p.c.max, p.c.log, p.z1, p.c.lsg);
+    B2_CHECK_LAUNCH(ctx);
+    B2_LAUNCH(ctx, k_lg_row_argmax, cdiv(M, 8), 256, 0, st, sim, M, N, p.r.max, p.r.log, p.c.max, p.c.log, p.r.lsg, p.c.lsg, p.best0,
+              p.arg0);
+    B2_CHECK_LAUNCH(ctx);
+    B2_LAUNCH(ctx, k_lg_col_argmax, cdiv(N, 32), 1024, 0, st, sim, M, N, p.r.max, p.r.log, p.c.max, p.c.log, p.r.lsg, p.c.lsg, p.arg1);
+    B2_CHECK_LAUNCH(ctx);
+  }
+  B2_LAUNCH(ctx, k_lg_filter, 1, 1024, 0, st, p.best0, p.arg0, p.arg1, M, p.thr, p.ind0, p.ind1, p.out_matches, p.out_scores, p.count);
+  B2_CHECK_LAUNCH(ctx);
+  return B2_OK;
+}
+
 // Row r of the device copy of a self block's QKV projection (weight and bias) is row out[r] of the checkpoint's.  The
 // checkpoint interleaves q, k, v per feature, (h * 64 + j) * 3 + {q, k, v} (lightglue.py:166-167); the device copy is
 // [q | k | v], each 256 rows in head-major order h * 64 + j, so the rotary pair (2p, 2p + 1) of a head is two adjacent
@@ -967,38 +1026,12 @@ static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, con
   for (int li = 0; li < nlive; ++li) {
     const int p = live[li];
     LgSide &a = s->side[2 * p], &b = s->side[2 * p + 1];
-    const float* sim = s->sim[p].as<float>();
-    if (assign_ps_fits(1, b.n)) {
-      // persistent cooperative kernel (assign_ps.cuh, KIND 1): row / column log-softmax statistics in one sweep of the
-      // similarity, mutual arg-max in a second one - 2 reads and 1 launch instead of 4 and 4
-      const int G = s->persist_ctas;
-      B2_CUDA(ctx, s->as_part.ensure((size_t)G * 2 * b.n * sizeof(float)));
-      B2_CUDA(ctx, s->as_bar.ensure(16));
-      B2_CUDA(ctx, cudaMemsetAsync(s->as_bar.p, 0, 16, st));
-      SinkArgs sa{};
-      sa.Z = sim, sa.M = a.n, sa.N = b.n, sa.iters = 1, sa.u = a.rmax.as<float>(), sa.v = b.rmax.as<float>();
-      sa.rlog = a.rlog.as<float>(), sa.clog = b.rlog.as<float>(), sa.z0 = a.ls.as<float>(), sa.z1 = b.ls.as<float>();
-      sa.lsg0 = a.lsg.as<float>(), sa.lsg1 = b.lsg.as<float>(), sa.part = s->as_part.as<float>(), sa.bar = s->as_bar.as<unsigned>();
-      sa.best0 = a.amax.as<float>(), sa.arg0 = a.aidx.as<int>(), sa.arg1 = b.aidx.as<int>(), sa.err_flag = s->errflag.as<int>();
-      if ((rc = launch_assign_ps<1>(ctx, st, sa, G, "k_lg_assign"))) return rc;
-    } else {
-    B2_LAUNCH(ctx, k_lg_row_stats, cdiv(a.n, 8), 256, 0, st, sim, a.n, b.n, a.rmax.as<float>(), a.rlog.as<float>(), a.ls.as<float>(),
-              a.lsg.as<float>());
-    B2_CHECK_LAUNCH(ctx);
-    B2_LAUNCH(ctx, k_lg_col_stats, cdiv(b.n, 32), 1024, 0, st, sim, a.n, b.n, b.rmax.as<float>(), b.rlog.as<float>(), b.ls.as<float>(),
-              b.lsg.as<float>());
-    B2_CHECK_LAUNCH(ctx);
-    B2_LAUNCH(ctx, k_lg_row_argmax, cdiv(a.n, 8), 256, 0, st, sim, a.n, b.n, a.rmax.as<float>(), a.rlog.as<float>(),
-              b.rmax.as<float>(), b.rlog.as<float>(), a.lsg.as<float>(), b.lsg.as<float>(), a.amax.as<float>(), a.aidx.as<int>());
-    B2_CHECK_LAUNCH(ctx);
-    B2_LAUNCH(ctx, k_lg_col_argmax, cdiv(b.n, 32), 1024, 0, st, sim, a.n, b.n, a.rmax.as<float>(), a.rlog.as<float>(),
-              b.rmax.as<float>(), b.rlog.as<float>(), a.lsg.as<float>(), b.lsg.as<float>(), b.aidx.as<int>());
-    B2_CHECK_LAUNCH(ctx);
-    }
-    B2_LAUNCH(ctx, k_lg_filter, 1, 1024, 0, st, a.amax.as<float>(), a.aidx.as<int>(), b.aidx.as<int>(), a.n,
-              (float)prm->filter_threshold, a.ind[a.cur].as<int>(), b.ind[b.cur].as<int>(), s->pair[p].out_matches, s->pair[p].out_scores,
-              counters + 4 * LG_MAX_PAIRS + p);
-    B2_CHECK_LAUNCH(ctx);
+    const LgAssign la{s->sim[p].as<float>(), a.n, b.n, a.ls.as<float>(), b.ls.as<float>(), a.ind[a.cur].as<int>(), b.ind[b.cur].as<int>(),
+                      (float)prm->filter_threshold, {a.rmax.as<float>(), a.rlog.as<float>(), a.lsg.as<float>()},
+                      {b.rmax.as<float>(), b.rlog.as<float>(), b.lsg.as<float>()}, a.amax.as<float>(), a.aidx.as<int>(), b.aidx.as<int>(),
+                      &s->as_part, &s->as_bar, s->errflag.as<int>(), s->pair[p].out_matches, s->pair[p].out_scores,
+                      counters + 4 * LG_MAX_PAIRS + p};
+    if ((rc = lg_assign(ctx, st, la, 0, s->persist_ctas, nullptr))) return rc;
   }
   B2_CUDA(ctx, cudaMemcpyAsync(hread + 4 * LG_MAX_PAIRS, counters + 4 * LG_MAX_PAIRS, LG_MAX_PAIRS * sizeof(int), cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaMemcpyAsync(hread + 5 * LG_MAX_PAIRS, s->errflag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1145,5 +1178,65 @@ extern "C" int b2_lightglue_match_host(b2_context* ctx, const float* kp0, const 
     if (out_scores) B2_CUDA(ctx, cudaMemcpyAsync(out_scores, ctx->stage_d[6].p, (size_t)*out_k * 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA(ctx, cudaStreamSynchronize(st));
   }
+  return B2_OK;
+}
+
+// ---- test-only entry point: the assignment step on its own, on a host similarity matrix --------------------------------------
+
+extern "C" int b2_debug_lightglue_assign_host(b2_context* ctx, int path, int ctas, const float* sim, int M, int N, const float* z0,
+                                              const float* z1, const int* ind0, const int* ind1, float threshold, float* row_stats,
+                                              float* col_stats, float* best0, int* arg0, int* arg1, int64_t* out_matches,
+                                              float* out_scores, int* out_k, int* out_path) {
+  if (!ctx || !sim || !z0 || !z1 || !row_stats || !col_stats || !best0 || !arg0 || !arg1 || !out_matches || !out_scores || !out_k ||
+      !out_path || M <= 0 || N <= 0 || path < 0 || path > 2 || ctas < 0 || ctas > ctx->sm_count)
+    return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  DevBuf dsim, dz0, dz1, di0, di1, rs, cs, dbest, da0, da1, part, bar, err, out, outs, cnt;
+  B2_CUDA(ctx, dsim.ensure((size_t)M * N * 4));
+  B2_CUDA(ctx, dz0.ensure((size_t)M * 4));
+  B2_CUDA(ctx, dz1.ensure((size_t)N * 4));
+  B2_CUDA(ctx, di0.ensure((size_t)M * 4));
+  B2_CUDA(ctx, di1.ensure((size_t)N * 4));
+  B2_CUDA(ctx, rs.ensure((size_t)3 * M * 4));
+  B2_CUDA(ctx, cs.ensure((size_t)3 * N * 4));
+  B2_CUDA(ctx, dbest.ensure((size_t)M * 4));
+  B2_CUDA(ctx, da0.ensure((size_t)M * 4));
+  B2_CUDA(ctx, da1.ensure((size_t)N * 4));
+  B2_CUDA(ctx, err.ensure(16));
+  B2_CUDA(ctx, out.ensure((size_t)M * 16));
+  B2_CUDA(ctx, outs.ensure((size_t)M * 4));
+  B2_CUDA(ctx, cnt.ensure(16));
+  std::vector<int> iota((size_t)(M > N ? M : N));
+  for (size_t i = 0; i < iota.size(); ++i) iota[i] = (int)i;
+  B2_CUDA(ctx, cudaMemcpyAsync(dsim.p, sim, (size_t)M * N * 4, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(dz0.p, z0, (size_t)M * 4, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(dz1.p, z1, (size_t)N * 4, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(di0.p, ind0 ? ind0 : iota.data(), (size_t)M * 4, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(di1.p, ind1 ? ind1 : iota.data(), (size_t)N * 4, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemsetAsync(err.p, 0, 16, st));
+  const int G = ctas > 0 ? ctas : (ctx->sm_count - ctx->reserve_sms > 0 ? ctx->sm_count - ctx->reserve_sms : 1);
+  float *r = rs.as<float>(), *c = cs.as<float>();
+  const LgAssign p{dsim.as<float>(), M, N, dz0.as<float>(), dz1.as<float>(), di0.as<int>(), di1.as<int>(), threshold, {r, r + M, r + 2 * M},
+                   {c, c + N, c + 2 * N}, dbest.as<float>(), da0.as<int>(), da1.as<int>(), &part, &bar, err.as<int>(),
+                   out.as<long long>(), outs.as<float>(), cnt.as<int>()};
+  const int rc = lg_assign(ctx, st, p, path, G, out_path);
+  if (rc) return rc;
+  int k = 0, e = 0;
+  B2_CUDA(ctx, cudaMemcpyAsync(&k, cnt.p, 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(&e, err.p, 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(row_stats, rs.p, (size_t)3 * M * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(col_stats, cs.p, (size_t)3 * N * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(best0, dbest.p, (size_t)M * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(arg0, da0.p, (size_t)M * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(arg1, da1.p, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  if (k > 0) {
+    B2_CUDA(ctx, cudaMemcpy(out_matches, out.p, (size_t)k * 16, cudaMemcpyDeviceToHost));
+    B2_CUDA(ctx, cudaMemcpy(out_scores, outs.p, (size_t)k * 4, cudaMemcpyDeviceToHost));
+  }
+  *out_k = k;
+  if (e) return b2_fail(ctx, B2_ERR_STATE, "the persistent assignment kernel timed out in its grid barrier (kernel bug)");
   return B2_OK;
 }

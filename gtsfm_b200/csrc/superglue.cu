@@ -332,7 +332,70 @@ extern "C" int b2_superglue_set_weights(b2_context* ctx, const float* blob, size
   return B2_OK;
 }
 
-static int sg_match_impl(b2_context* ctx, const float* kp0, const float* sc0, const float* desc0, int n0, int h0, int w0,
+// The assignment step on the score matrix Z [M][N]: log-space Sinkhorn (superglue.py:141-170), mutual arg-max and threshold
+// (:266-276) -> the ordered match list.  u [M + 1] and v [N + 1] receive the duals, best0 / arg0 [M] and arg1 [N] the arg-max.
+struct SgAssign {
+  const float* Z;
+  int M, N;
+  float alpha;
+  int iters;
+  float thr;
+  float *u, *v, *best0;
+  int *arg0, *arg1;
+  DevBuf *part, *bar;  // scratch of the persistent kernel
+  int* err_flag;
+  unsigned* out_matches;
+  float* out_scores;
+  int* count;
+};
+
+// path 0 runs the persistent kernel when it fits (what the matcher does), 1 forces it, 2 forces the multi-launch passes; G
+// is the persistent kernel's CTA count.  *ran (when given) receives the path that ran, 1 or 2.
+static int sg_assign(b2_context* ctx, cudaStream_t st, const SgAssign& p, int path, int G, int* ran) {
+  const float* Z = p.Z;
+  const int M = p.M, N = p.N, iters = p.iters;
+  const float norm = -logf((float)(M + N));
+  float* u = p.u;
+  float* v = p.v;
+  const bool persistent = path == 0 ? assign_ps_fits(0, N) : path == 1;
+  if (persistent && !assign_ps_fits(0, N)) return b2_fail(ctx, B2_ERR_ARG, "the persistent Sinkhorn kernel holds at most 8191 columns");
+  if (ran) *ran = persistent ? 1 : 2;
+  int rc;
+  if (persistent) {
+    // persistent cooperative kernel: all iterations + the mutual arg-max passes in one launch, every score read once per iteration
+    B2_CUDA(ctx, p.part->ensure((size_t)G * 2 * (N + 1) * sizeof(float)));
+    B2_CUDA(ctx, p.bar->ensure(16));
+    B2_CUDA(ctx, cudaMemsetAsync(p.bar->p, 0, 16, st));
+    if (iters == 0) B2_CUDA(ctx, cudaMemsetAsync(u, 0, (size_t)(M + 1) * sizeof(float), st));
+    SinkArgs sa{};
+    sa.Z = Z, sa.M = M, sa.N = N, sa.alpha = p.alpha, sa.norm = norm, sa.iters = iters, sa.u = u, sa.v = v;
+    sa.part = p.part->as<float>(), sa.bar = p.bar->as<unsigned>(), sa.best0 = p.best0, sa.arg0 = p.arg0;
+    sa.arg1 = p.arg1, sa.err_flag = p.err_flag;
+    if ((rc = launch_assign_ps<0>(ctx, st, sa, G, "k_sg_sinkhorn"))) return rc;
+  } else {
+    B2_LAUNCH(ctx, k_sg_fill, cdiv(N + 1, 256), 256, 0, st, v, N + 1, 0.f);
+    B2_CHECK_LAUNCH(ctx);
+    for (int it = 0; it < iters; ++it) {
+      B2_LAUNCH(ctx, k_sg_rows, cdiv(M + 1, 8), 256, 0, st, Z, M, N, v, p.alpha, norm, u);
+      B2_CHECK_LAUNCH(ctx);
+      B2_LAUNCH(ctx, k_sg_cols, cdiv(N + 1, 32), 256, 0, st, Z, M, N, u, p.alpha, norm, v);
+      B2_CHECK_LAUNCH(ctx);
+    }
+    if (iters == 0) {
+      B2_LAUNCH(ctx, k_sg_fill, cdiv(M + 1, 256), 256, 0, st, u, M + 1, 0.f);
+      B2_CHECK_LAUNCH(ctx);
+    }
+    B2_LAUNCH(ctx, k_sg_row_argmax, cdiv(M, 8), 256, 0, st, Z, M, N, u, v, norm, p.best0, p.arg0);
+    B2_CHECK_LAUNCH(ctx);
+    B2_LAUNCH(ctx, k_sg_col_argmax, cdiv(N, 32), 256, 0, st, Z, M, N, u, v, norm, p.arg1);
+    B2_CHECK_LAUNCH(ctx);
+  }
+  B2_LAUNCH(ctx, k_sg_filter, 1, 1024, 0, st, p.best0, p.arg0, p.arg1, M, p.thr, p.out_matches, p.out_scores, p.count);
+  B2_CHECK_LAUNCH(ctx);
+  return B2_OK;
+}
+
+static int sg_match_impl(b2_context* ctx,const float* kp0, const float* sc0, const float* desc0, int n0, int h0, int w0,
                          const float* kp1, const float* sc1, const float* desc1, int n1, int h1, int w1, int iters, float thr,
                          unsigned* out_matches, float* out_scores, int* out_k, cudaStream_t st) {
   SuperGlueState* s = ctx->sg;
@@ -427,44 +490,10 @@ static int sg_match_impl(b2_context* ctx, const float* kp0, const float* sc0, co
   gs.cf = s->sim.as<float>(), gs.ldc = N, gs.tc_want_f32 = true, gs.M = M, gs.N = N;
   if ((rc = run_linear(ctx, st, tw, &gs, 1))) return rc;
   // log-space Sinkhorn (superglue.py:141-170); u lives in a.u [M+1], v in b.vv [N+1]
-  const float* Z = s->sim.as<float>();
-  const float norm = -logf((float)(M + N));
-  float* u = a.u.as<float>();
-  float* v = b.vv.as<float>();
-  if (assign_ps_fits(0, N)) {
-    // persistent cooperative kernel: all iterations + the mutual arg-max passes in one launch, every score read once per iteration
-    const int G = tw.sm_count;
-    B2_CUDA(ctx, s->sk_part.ensure((size_t)G * 2 * (N + 1) * sizeof(float)));
-    B2_CUDA(ctx, s->sk_bar.ensure(16));
-    B2_CUDA(ctx, cudaMemsetAsync(s->sk_bar.p, 0, 16, st));
-    if (iters == 0) B2_CUDA(ctx, cudaMemsetAsync(u, 0, (size_t)(M + 1) * sizeof(float), st));
-    SinkArgs sa{};
-    sa.Z = Z, sa.M = M, sa.N = N, sa.alpha = s->bin_score, sa.norm = norm, sa.iters = iters, sa.u = u, sa.v = v;
-    sa.part = s->sk_part.as<float>(), sa.bar = s->sk_bar.as<unsigned>(), sa.best0 = a.best.as<float>(), sa.arg0 = a.arg.as<int>();
-    sa.arg1 = b.arg.as<int>(), sa.err_flag = s->errflag.as<int>();
-    if ((rc = launch_assign_ps<0>(ctx, st, sa, G, "k_sg_sinkhorn"))) return rc;
-  } else {
-  B2_LAUNCH(ctx, k_sg_fill, cdiv(N + 1, 256), 256, 0, st, v, N + 1, 0.f);
-  B2_CHECK_LAUNCH(ctx);
-  for (int it = 0; it < iters; ++it) {
-    B2_LAUNCH(ctx, k_sg_rows, cdiv(M + 1, 8), 256, 0, st, Z, M, N, v, s->bin_score, norm, u);
-    B2_CHECK_LAUNCH(ctx);
-    B2_LAUNCH(ctx, k_sg_cols, cdiv(N + 1, 32), 256, 0, st, Z, M, N, u, s->bin_score, norm, v);
-    B2_CHECK_LAUNCH(ctx);
-  }
-  if (iters == 0) {
-    B2_LAUNCH(ctx, k_sg_fill, cdiv(M + 1, 256), 256, 0, st, u, M + 1, 0.f);
-    B2_CHECK_LAUNCH(ctx);
-  }
-  B2_LAUNCH(ctx, k_sg_row_argmax, cdiv(M, 8), 256, 0, st, Z, M, N, u, v, norm, a.best.as<float>(), a.arg.as<int>());
-  B2_CHECK_LAUNCH(ctx);
-  B2_LAUNCH(ctx, k_sg_col_argmax, cdiv(N, 32), 256, 0, st, Z, M, N, u, v, norm, b.arg.as<int>());
-  B2_CHECK_LAUNCH(ctx);
-  }
   int* counters = s->counters.as<int>();
-  B2_LAUNCH(ctx, k_sg_filter, 1, 1024, 0, st, a.best.as<float>(), a.arg.as<int>(), b.arg.as<int>(), M, thr, out_matches, out_scores,
-            counters);
-  B2_CHECK_LAUNCH(ctx);
+  const SgAssign sg{s->sim.as<float>(), M, N, s->bin_score, iters, thr, a.u.as<float>(), b.vv.as<float>(), a.best.as<float>(),
+                    a.arg.as<int>(), b.arg.as<int>(), &s->sk_part, &s->sk_bar, s->errflag.as<int>(), out_matches, out_scores, counters};
+  if ((rc = sg_assign(ctx, st, sg, 0, tw.sm_count, nullptr))) return rc;
   int hres[2] = {0, 0};
   B2_CUDA(ctx, cudaMemcpyAsync(&hres[0], counters, sizeof(int), cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaMemcpyAsync(&hres[1], s->errflag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -516,5 +545,54 @@ extern "C" int b2_superglue_match_host(b2_context* ctx, const float* kp0, const 
     if (out_scores) B2_CUDA(ctx, cudaMemcpyAsync(out_scores, ctx->stage_d[7].p, (size_t)*out_k * 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA(ctx, cudaStreamSynchronize(st));
   }
+  return B2_OK;
+}
+
+// ---- test-only entry point: the assignment step on its own, on a host score matrix ------------------------------------------
+
+extern "C" int b2_debug_superglue_assign_host(b2_context* ctx, int path, int ctas, const float* Z, int M, int N, float alpha, int iters,
+                                              float threshold, float* u, float* v, float* best0, int* arg0, int* arg1,
+                                              uint32_t* out_matches, float* out_scores, int* out_k, int* out_path) {
+  if (!ctx || !Z || !u || !v || !best0 || !arg0 || !arg1 || !out_matches || !out_scores || !out_k || !out_path || M <= 0 || N <= 0 ||
+      iters < 0 || path < 0 || path > 2 || ctas < 0 || ctas > ctx->sm_count)
+    return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  DevBuf dZ, du, dv, dbest, da0, da1, part, bar, err, out, outs, cnt;
+  B2_CUDA(ctx, dZ.ensure((size_t)M * N * 4));
+  B2_CUDA(ctx, du.ensure((size_t)(M + 1) * 4));
+  B2_CUDA(ctx, dv.ensure((size_t)(N + 1) * 4));
+  B2_CUDA(ctx, dbest.ensure((size_t)M * 4));
+  B2_CUDA(ctx, da0.ensure((size_t)M * 4));
+  B2_CUDA(ctx, da1.ensure((size_t)N * 4));
+  B2_CUDA(ctx, err.ensure(16));
+  B2_CUDA(ctx, out.ensure((size_t)M * 8));
+  B2_CUDA(ctx, outs.ensure((size_t)M * 4));
+  B2_CUDA(ctx, cnt.ensure(16));
+  B2_CUDA(ctx, cudaMemcpyAsync(dZ.p, Z, (size_t)M * N * 4, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemsetAsync(err.p, 0, 16, st));
+  // without iterations the persistent kernel never writes v; the reference's v is then its initial 0
+  if (iters == 0) B2_CUDA(ctx, cudaMemsetAsync(dv.p, 0, (size_t)(N + 1) * 4, st));
+  const int G = ctas > 0 ? ctas : (ctx->sm_count - ctx->reserve_sms > 0 ? ctx->sm_count - ctx->reserve_sms : 1);
+  const SgAssign p{dZ.as<float>(), M, N, alpha, iters, threshold, du.as<float>(), dv.as<float>(), dbest.as<float>(), da0.as<int>(),
+                   da1.as<int>(), &part, &bar, err.as<int>(), out.as<unsigned>(), outs.as<float>(), cnt.as<int>()};
+  const int rc = sg_assign(ctx, st, p, path, G, out_path);
+  if (rc) return rc;
+  int k = 0, e = 0;
+  B2_CUDA(ctx, cudaMemcpyAsync(&k, cnt.p, 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(&e, err.p, 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(u, du.p, (size_t)(M + 1) * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(v, dv.p, (size_t)(N + 1) * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(best0, dbest.p, (size_t)M * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(arg0, da0.p, (size_t)M * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(arg1, da1.p, (size_t)N * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  if (k > 0) {
+    B2_CUDA(ctx, cudaMemcpy(out_matches, out.p, (size_t)k * 8, cudaMemcpyDeviceToHost));
+    B2_CUDA(ctx, cudaMemcpy(out_scores, outs.p, (size_t)k * 4, cudaMemcpyDeviceToHost));
+  }
+  *out_k = k;
+  if (e) return b2_fail(ctx, B2_ERR_STATE, "the persistent assignment kernel timed out in its grid barrier (kernel bug)");
   return B2_OK;
 }

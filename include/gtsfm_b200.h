@@ -82,6 +82,21 @@ int b2_debug_gemm_segments_host(b2_context* ctx, const float* A, const float* B,
  * The operands are split into fp16 hi / lo planes on the device; single = 1 runs the fp16 variant (hi planes only). */
 int b2_debug_attention_host(b2_context* ctx, int np, const int* nq, const int* nk, int heads, float scale, int single,
                             const float* q, const float* k, const float* v, float* o);
+/* Test-only: the matchers' assignment step on HOST buffers, through the same dispatch the matchers use.  path 0 = what the
+ * matcher picks, 1 = the persistent cooperative kernel (an error when N is above its limit), 2 = the multi-launch kernels;
+ * ctas = the persistent kernel's CTA count (1 .. SM count; 0 = the matcher's).  *out_path receives the path that ran (1 or
+ * 2), out_matches / out_scores the filtered match list (M rows of room), *out_k its length.
+ *  SuperGlue: Z [M][N] scores, bin score alpha, `iters` Sinkhorn iterations -> duals u [M + 1], v [N + 1]; uint32 rows (i, j).
+ *  LightGlue: sim [M][N], matchability logits z0 [M], z1 [N], ind0 [M] / ind1 [N] (NULL = identity) -> row_stats [3][M] =
+ *  (max, log sum exp(x - max), logsigmoid(z0)) and col_stats [3][N] alike; int64 rows (ind0[i], ind1[j]).
+ * Both: best0 [M] row maxima of the final scores, arg0 [M] / arg1 [N] row / column arg-max (first maximum). */
+int b2_debug_superglue_assign_host(b2_context* ctx, int path, int ctas, const float* Z, int M, int N, float alpha, int iters,
+                                   float threshold, float* u, float* v, float* best0, int* arg0, int* arg1, uint32_t* out_matches,
+                                   float* out_scores, int* out_k, int* out_path);
+int b2_debug_lightglue_assign_host(b2_context* ctx, int path, int ctas, const float* sim, int M, int N, const float* z0,
+                                   const float* z1, const int* ind0, const int* ind1, float threshold, float* row_stats,
+                                   float* col_stats, float* best0, int* arg0, int* arg1, int64_t* out_matches, float* out_scores,
+                                   int* out_k, int* out_path);
 
 /* ---- SuperPoint -------------------------------------------------------------------------------------------------- */
 /* `blob`: the 24 state-dict tensors in reference order (conv1a.weight, conv1a.bias, conv1b.weight, ... convDb.bias;

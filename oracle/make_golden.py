@@ -281,6 +281,49 @@ def golden_superglue_large():
         print(f"superglue seed {seed} ({n0},{n1}): K={len(rows)}")
 
 
+def golden_superglue_wide():
+    """(d) SuperGlue with n1 + 1 > 8192 columns: more than the persistent assignment kernel holds, so the engine runs the
+    multi-launch Sinkhorn and arg-max passes."""
+    sd = syn.superglue_state_dict(1, "sharp")
+    model = ref_modules.ref_superglue(sd, weights="outdoor", sinkhorn_iterations=20, descriptor_dim=256)
+    seed, n0, n1 = 14, 600, 8300
+    kp0, sc0, d0, kp1, sc1, d1, gt = syn.synthetic_features(seed, n0, n1)
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))[None]
+    data = {"keypoints0": t(kp0), "keypoints1": t(kp1), "descriptors0": t(d0.T), "descriptors1": t(d1.T),
+            "scores0": t(sc0), "scores1": t(sc1), "image0": torch.empty(1, 1, 480, 640), "image1": torch.empty(1, 1, 480, 640)}
+    with torch.no_grad():
+        pred = model(data)
+    m0 = pred["matches0"][0].numpy()
+    valid = m0 > -1
+    rows = np.hstack([np.arange(n0)[valid].reshape(-1, 1), np.arange(n1)[m0[valid]].reshape(-1, 1)]).astype(np.uint32)
+    rows2 = superglue_ref.superglue_match(kp0, sc0, d0, kp1, sc1, d1, (480, 640, 3), (480, 640, 3), sd)
+    assert np.array_equal(rows, rows2), f"superglue restatement != reference (seed {seed}): {len(rows)} vs {len(rows2)}"
+    assert len(rows) > 500, len(rows)
+    np.savez_compressed(OUT / f"superglue_{seed}.npz", matches=rows, mscores=pred["matching_scores0"][0].numpy()[valid],
+                        seed=seed, n0=n0, n1=n1, profile="sharp")
+    print(f"superglue seed {seed} ({n0},{n1}): K={len(rows)}")
+
+
+def golden_lightglue_wide():
+    """(e) LightGlue whose final layer has more than 6240 columns: the persistent assignment kernel's shared memory does
+    not hold them, so the engine runs the multi-launch log-softmax and arg-max passes.  'full' weights prune nothing."""
+    sd = syn.lightglue_state_dict(2, "full")
+    model = ref_modules.ref_lightglue(sd)
+    profile, seed, n0, n1 = "full", 15, 1000, 6400
+    kp0, sc0, d0, kp1, sc1, d1, gt = syn.synthetic_features(seed, n0, n1)
+    m, stop, pr0, pr1, ms = run_ref_lightglue(model, kp0, d0, kp1, d1, (480, 640), (480, 640))
+    tr = {}
+    m2 = lightglue_ref.lightglue_match(kp0, d0, kp1, d1, sd, trace=tr)
+    assert np.array_equal(m, m2), f"lightglue restatement != reference ({profile},{seed}): {len(m)} vs {len(m2)}"
+    assert tr["stop"] == stop
+    assert tr["sizes"][-1][1] > 6240, tr["sizes"].tolist()
+    assert len(m) >= 0.25 * min(n0, n1), len(m)
+    np.savez_compressed(OUT / f"lightglue_{profile}_{seed}.npz", matches=m, stop=stop, sizes=tr["sizes"],
+                        prune0=pr0.astype(np.int8), prune1=pr1.astype(np.int8), mscores=ms,
+                        seed=seed, n0=n0, n1=n1, profile=profile)
+    print(f"lightglue {profile} seed {seed} ({n0},{n1}): K={len(m)} stop={stop} sizes={tr['sizes'].tolist()[-1]}")
+
+
 def golden_lund_door():
     """(d) BASELINE configs[0]: all 12 lund-door images (loader resize to short side 760) and the 66 exhaustive pairs through
     SuperPoint (max 5000 keypoints, wrapper argpartition) -> LightGlue ('sharp' weights).  Stores the resized gray frames
@@ -430,6 +473,8 @@ def main():
     golden_lightglue_bench()
     golden_superpoint_mp1()
     golden_superglue_large()
+    golden_superglue_wide()
+    golden_lightglue_wide()
     golden_lund_door()
     golden_retriever()
     golden_netvlad()

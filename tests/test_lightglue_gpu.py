@@ -21,8 +21,9 @@ def engine(ctx, profile):
 
 
 # bench_11 IS the configuration bench.py times: 5000 x 5000 keypoints, 'bench' weights, 9 full layers (79 key tiles x 160
-# attention items through the stream-K split / fix-up); bench_12 the same weights at 1024 keypoints
-@pytest.mark.parametrize("tag", ["full_5", "full_6", "prune_7", "stop_8", "prune_9", "stop_10", "bench_12", "bench_11"])
+# attention items through the stream-K split / fix-up); bench_12 the same weights at 1024 keypoints; full_15 has 6400
+# columns in its final layer, more than the persistent assignment kernel holds (the multi-launch path)
+@pytest.mark.parametrize("tag", ["full_5", "full_6", "prune_7", "stop_8", "prune_9", "stop_10", "bench_12", "bench_11", "full_15"])
 def test_matches_equal_reference_fixture(b200_ctx, golden_dir, tag):
     fx = np.load(golden_dir / f"lightglue_{tag}.npz")
     kp0, _, d0, kp1, _, d1, _ = syn.synthetic_features(int(fx["seed"]), int(fx["n0"]), int(fx["n1"]))

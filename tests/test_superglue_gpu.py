@@ -12,7 +12,9 @@ from gtsfm_b200.matcher import B200SuperGlueMatcher, SuperGlueEngine
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("seed", [5, 6, 9, 12, 13])  # 12: 2048 x 1900, 13: 5000 x 5000 keypoints (100 MB coupling matrix)
+# 12: 2048 x 1900, 13: 5000 x 5000 keypoints (100 MB coupling matrix), 14: 600 x 8300 (more columns than the persistent
+# Sinkhorn kernel holds: the multi-launch path)
+@pytest.mark.parametrize("seed", [5, 6, 9, 12, 13, 14])
 def test_matches_equal_reference_fixture(b200_ctx, golden_dir, seed):
     fx = np.load(golden_dir / f"superglue_{seed}.npz")
     kp0, sc0, d0, kp1, sc1, d1, _ = syn.synthetic_features(seed, int(fx["n0"]), int(fx["n1"]))
