@@ -66,6 +66,17 @@ class RansacParams(C.Structure):
     _fields_ = [("threshold", C.c_double), ("confidence", C.c_double), ("max_iters", C.c_int), ("seed", C.c_uint64)]
 
 
+class RansacCandidate(C.Structure):
+    _fields_ = [("model", C.c_double * 9), ("cost", C.c_double), ("ninl", C.c_int), ("valid", C.c_int)]
+
+
+class RansacTrace(C.Structure):  # b2_ransac_trace (tests only)
+    _fields_ = [("batch", C.c_int), ("max_records", C.c_int), ("nsol", C.c_void_p), ("models", C.c_void_p), ("cost", C.c_void_p),
+                ("ninl", C.c_void_p), ("selected", C.c_void_p), ("more", C.c_void_p), ("batches", C.c_int), ("ext_go", C.c_int),
+                ("records", C.c_int), ("prerefine", RansacCandidate * 8), ("refined", RansacCandidate * 8), ("pick", RansacCandidate),
+                ("mask_count", C.c_int), ("votes", C.c_int * 4), ("winner", C.c_int), ("pose_cands", C.c_double * 21)]
+
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 
@@ -120,6 +131,8 @@ SIGNATURES = {
     "b2_ransac_fundamental_host": (_i, [_vp, _vp, _vp, _i, C.POINTER(RansacParams), _vp, _vp, _ip]),
     "b2_ransac_essential_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, C.POINTER(RansacParams), _vp, _vp, _ip, _vp, _vp, _vp]),
     "b2_recover_pose_host": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _ip]),
+    "b2_debug_ransac_trace_host": (_i, [_vp, _i, _vp, _vp, _i, C.POINTER(RansacParams), C.POINTER(RansacTrace), _vp, _vp, _ip, _vp, _vp]),
+    "b2_debug_recover_pose_host": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _ip, _vp, _vp, _ip]),
     "b2_mnn_match_batched_dev": (_i, [_vp, C.POINTER(MnnPair), _i, _i, _i, C.c_double, _vp]),
     "b2_mnn_match_host": (_i, [_vp, _vp, _i, _vp, _i, _i, _i, C.c_double, _vp, _vp, _ip]),
     "b2_sift_detect_batched_dev": (_i, [_vp, C.POINTER(SiftImage), _i, _i, _i, _i, _sz, _vp]),

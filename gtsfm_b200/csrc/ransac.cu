@@ -22,6 +22,7 @@ constexpr int RS_SCORE_THREADS = 128;
 constexpr int RS_LO_THREADS = 512;
 constexpr int RS_LO_ITERS = 6;
 constexpr int RS_TOP = 8;  // hypotheses handed to the local optimisation (the refined candidate with the lowest MSAC cost wins)
+constexpr int RS_BATCH = 16384;  // hypotheses per launch (buffers are sized for it; a trace may ask for fewer)
 }  // namespace
 
 struct RansacState {
@@ -34,13 +35,8 @@ void rs_destroy(b2_context* ctx) {
   ctx->rs = nullptr;
 }
 
-// best-model record kept on the device between batches
-struct RsBest {
-  double model[9];
-  double cost;
-  int ninl;
-  int valid;
-};
+// best-model record kept on the device between batches (the header's b2_ransac_candidate, so traces copy it as is)
+using RsBest = b2_ransac_candidate;
 
 __device__ __forceinline__ double rs_err(int mode, const double* M, double a, double b, double c, double d) {
   return mode == 0 ? sampson_sq(M, a, b, c, d) : epiline_sq(M, a, b, c, d);
@@ -75,45 +71,13 @@ __global__ void __launch_bounds__(64) k_rs_hyp_F(const double* __restrict__ x1, 
   if (s >= n_samples) return;
   int idx[8];
   sample_distinct(seed, (unsigned long long)(sample0 + s), k, 8, idx);
-  double c1x = 0, c1y = 0, c2x = 0, c2y = 0;
-  for (int i = 0; i < 8; ++i) c1x += x1[2 * idx[i]], c1y += x1[2 * idx[i] + 1], c2x += x2[2 * idx[i]], c2y += x2[2 * idx[i] + 1];
-  c1x /= 8, c1y /= 8, c2x /= 8, c2y /= 8;
-  double d1 = 0, d2 = 0;
+  double a[8][2], b[8][2];
   for (int i = 0; i < 8; ++i) {
-    d1 += sqrt((x1[2 * idx[i]] - c1x) * (x1[2 * idx[i]] - c1x) + (x1[2 * idx[i] + 1] - c1y) * (x1[2 * idx[i] + 1] - c1y));
-    d2 += sqrt((x2[2 * idx[i]] - c2x) * (x2[2 * idx[i]] - c2x) + (x2[2 * idx[i] + 1] - c2y) * (x2[2 * idx[i] + 1] - c2y));
+    a[i][0] = x1[2 * idx[i]], a[i][1] = x1[2 * idx[i] + 1];
+    b[i][0] = x2[2 * idx[i]], b[i][1] = x2[2 * idx[i] + 1];
   }
-  if (d1 < 1e-12 || d2 < 1e-12) {
-    nsol[s] = 0;
-    return;
-  }
-  double s1 = 1.4142135623730951 * 8 / d1, s2 = 1.4142135623730951 * 8 / d2;
-  double A[81];
-  for (int i = 0; i < 81; ++i) A[i] = 0;
-  for (int p = 0; p < 8; ++p) {
-    double ax = (x1[2 * idx[p]] - c1x) * s1, ay = (x1[2 * idx[p] + 1] - c1y) * s1;
-    double bx = (x2[2 * idx[p]] - c2x) * s2, by = (x2[2 * idx[p] + 1] - c2y) * s2;
-    double q[9] = {bx * ax, bx * ay, bx, by * ax, by * ay, by, ax, ay, 1.0};
-    for (int i = 0; i < 9; ++i)
-      for (int j = 0; j < 9; ++j) A[i * 9 + j] += q[i] * q[j];
-  }
-  double Fn[9];
-  smallest_eigvec9(A, Fn);
-  enforce_rank2(Fn);
-  // F = T2^T Fn T1, T = [s 0 -s c; 0 s -s c; 0 0 1]
-  double T1[9] = {s1, 0, -s1 * c1x, 0, s1, -s1 * c1y, 0, 0, 1}, T2t[9] = {s2, 0, 0, 0, s2, 0, -s2 * c2x, -s2 * c2y, 1};
-  double tmp[9], F[9];
-  mat3_mul(T2t, Fn, tmp);
-  mat3_mul(tmp, T1, F);
-  double n = 0;
-  for (int i = 0; i < 9; ++i) n += F[i] * F[i];
-  n = sqrt(n);
-  if (!(n > 1e-300)) {
-    nsol[s] = 0;
-    return;
-  }
-  nsol[s] = 1;
-  for (int i = 0; i < 9; ++i) models[(size_t)s * RS_MAX_SOL * 9 + i] = F[i] / n;
+  const int n = eightpt_solve(a, b, models + (size_t)s * RS_MAX_SOL * 9);
+  nsol[s] = n;
 }
 
 // ---- scoring: one CTA per model slot ---------------------------------------------------------------------------------
@@ -463,7 +427,8 @@ constexpr int RS_POSE_THREADS = 128;
 __global__ void __launch_bounds__(RS_POSE_THREADS) k_rs_pose(const double* __restrict__ E, const double* __restrict__ x1,
                                                               const double* __restrict__ x2, const uint8_t* __restrict__ mask, int k,
                                                               int* __restrict__ gvotes /*[4] votes + [1] CTA counter, zero on entry*/,
-                                                              double* __restrict__ out /*R[9], t[3], good*/) {
+                                                              double* __restrict__ out /*R[9], t[3], good*/,
+                                                              double* __restrict__ cands /*R1[9], R2[9], t[3], winner; tests only*/) {
   __shared__ double R1[9], R2[9], t[3];
   __shared__ int votes[4];
   __shared__ int is_last;
@@ -507,6 +472,11 @@ __global__ void __launch_bounds__(RS_POSE_THREADS) k_rs_pose(const double* __res
     for (int j = 0; j < 9; ++j) out[j] = R[j];
     for (int j = 0; j < 3; ++j) out[9 + j] = sg * t[j];
     out[12] = (double)tot[b];
+    if (cands) {
+      for (int j = 0; j < 9; ++j) cands[j] = R1[j], cands[9 + j] = R2[j];
+      for (int j = 0; j < 3; ++j) cands[18 + j] = t[j];
+      cands[21] = (double)b;
+    }
   }
 }
 
@@ -530,31 +500,34 @@ __global__ void __launch_bounds__(256) k_rs_gather(const float* __restrict__ kp1
 }
 
 // x1 / x2 come either from host arrays (hx != null: uploaded here) or are already in s->x1 / s->x2 (device path).
-// out_mask: host pointer when mask_is_device == 0, device pointer otherwise.
+// out_mask: host pointer when mask_is_device == 0, device pointer otherwise.  tr (tests only, nullptr in production) sets
+// the batch size and receives the intermediate state; it adds copies and synchronisations but no launches.
 static int rs_run(b2_context* ctx, const double* hx1, const double* hx2, int k, const b2_ransac_params* prm, int mode,
                   double* out_model, uint8_t* out_mask, int* out_ninl, double* out_R, double* out_t,
-                  cudaStream_t st = nullptr, int mask_is_device = 0) {
+                  cudaStream_t st = nullptr, int mask_is_device = 0, b2_ransac_trace* tr = nullptr) {
   if (!ctx->rs) ctx->rs = new RansacState();
   RansacState* s = ctx->rs;
   if (!st) st = ctx->stream;
   const int m = mode == 0 ? 5 : 8;
+  if (tr) tr->batches = 0, tr->ext_go = -1, tr->records = 0;
   *out_ninl = 0;
   if (out_mask && !mask_is_device) memset(out_mask, 0, (size_t)k);
   if (out_mask && mask_is_device && k > 0) B2_CUDA(ctx, cudaMemsetAsync(out_mask, 0, (size_t)k, st));
   if (k < m) return 1;
   const int hard_cap = mode == 0 ? 65536 : 262144;
   const int max_iters = prm->max_iters < 1 ? 1 : (prm->max_iters > hard_cap ? hard_cap : prm->max_iters);
-  const int batch = 16384;  // hypotheses per launch (buffers are sized for it)
+  const int batch = tr ? tr->batch : RS_BATCH;
   const double thr2 = prm->threshold * prm->threshold;
   B2_CUDA(ctx, s->x1.ensure((size_t)k * 16));
   B2_CUDA(ctx, s->x2.ensure((size_t)k * 16));
-  B2_CUDA(ctx, s->models.ensure((size_t)batch * RS_MAX_SOL * 9 * 8));
-  B2_CUDA(ctx, s->nsol.ensure((size_t)batch * 4));
-  B2_CUDA(ctx, s->cost.ensure((size_t)batch * RS_MAX_SOL * 8));
-  B2_CUDA(ctx, s->ninl.ensure((size_t)batch * RS_MAX_SOL * 4));
+  B2_CUDA(ctx, s->models.ensure((size_t)RS_BATCH * RS_MAX_SOL * 9 * 8));
+  B2_CUDA(ctx, s->nsol.ensure((size_t)RS_BATCH * 4));
+  B2_CUDA(ctx, s->cost.ensure((size_t)RS_BATCH * RS_MAX_SOL * 8));
+  B2_CUDA(ctx, s->ninl.ensure((size_t)RS_BATCH * RS_MAX_SOL * 4));
   B2_CUDA(ctx, s->best.ensure(sizeof(RsBest) * (1 + RS_TOP) + 16));  // [0] result, then the counter, then the RS_TOP candidates
   B2_CUDA(ctx, s->mask.ensure((size_t)k + 16));
-  B2_CUDA(ctx, s->pose.ensure(48 * 8));  // [0,13) R, t, votes of the winner | [16,25) E (recover_pose) | [32,..) int votes[4] + counter
+  // [0,13) R, t, votes of the winner | [16,25) E (recover_pose) | [32,36) int votes[4] + counter | [36,58) R1, R2, t, winner
+  B2_CUDA(ctx, s->pose.ensure(64 * 8));
   B2_CUDA(ctx, s->hbuf.ensure(sizeof(RsBest) + 16 * 8 + 64));
   if (hx1) {
     B2_CUDA(ctx, cudaMemcpyAsync(s->x1.p, hx1, (size_t)k * 16, cudaMemcpyHostToDevice, st));
@@ -566,6 +539,25 @@ static int rs_run(b2_context* ctx, const double* hx1, const double* hx2, int k, 
   RsBest* dcand = reinterpret_cast<RsBest*>(s->best.as<char>() + sizeof(RsBest) + 16);
   RsBest* hbest = s->hbuf.as<RsBest>();
   const double *x1 = s->x1.as<double>(), *x2 = s->x2.as<double>();
+  // trace record of one k_rs_select launch over n samples (more_written: it wrote the confidence flag)
+  auto record = [&](int n, bool more_written) -> int {
+    if (tr->records >= tr->max_records) return B2_OK;
+    const int r = tr->records++;
+    const size_t ns = (size_t)tr->batch;
+    const auto d2h = cudaMemcpyDeviceToHost;
+    if (tr->nsol) B2_CUDA(ctx, cudaMemcpyAsync(tr->nsol + r * ns, s->nsol.p, (size_t)n * 4, d2h, st));
+    if (tr->models)
+      B2_CUDA(ctx, cudaMemcpyAsync(tr->models + r * ns * RS_MAX_SOL * 9, s->models.p, (size_t)n * RS_MAX_SOL * 72, d2h, st));
+    if (tr->cost) B2_CUDA(ctx, cudaMemcpyAsync(tr->cost + r * ns * RS_MAX_SOL, s->cost.p, (size_t)n * RS_MAX_SOL * 8, d2h, st));
+    if (tr->ninl) B2_CUDA(ctx, cudaMemcpyAsync(tr->ninl + r * ns * RS_MAX_SOL, s->ninl.p, (size_t)n * RS_MAX_SOL * 4, d2h, st));
+    if (tr->selected) B2_CUDA(ctx, cudaMemcpyAsync(tr->selected + (size_t)r * RS_TOP, dcand, sizeof(RsBest) * RS_TOP, d2h, st));
+    if (tr->more) {
+      if (more_written) B2_CUDA(ctx, cudaMemcpyAsync(tr->more + r, dcount + 1, 4, d2h, st));
+      else tr->more[r] = -1;
+    }
+    B2_CUDA(ctx, cudaStreamSynchronize(st));
+    return B2_OK;
+  };
   int done = 0;
   while (done < max_iters) {
     const int n = (max_iters - done) < batch ? (max_iters - done) : batch;
@@ -582,6 +574,10 @@ static int rs_run(b2_context* ctx, const double* hx1, const double* hx2, int k, 
     B2_LAUNCH(ctx, k_rs_select, 1, 1024, 0, st, s->models.as<double>(), s->cost.as<double>(), s->ninl.as<int>(),
               n * RS_MAX_SOL, dcand, (const int*)nullptr, dcount + 1, k, m, log(1.0 - prm->confidence), (double)(done + n));
     B2_CHECK_LAUNCH(ctx);
+    if (tr) {
+      ++tr->batches;
+      if (int rc = record(n, true)) return rc;
+    }
     done += n;
     if (done >= max_iters) break;
     // adaptive termination (standard RANSAC bound) between batches
@@ -609,20 +605,41 @@ static int rs_run(b2_context* ctx, const double* hx1, const double* hx2, int k, 
     B2_LAUNCH(ctx, k_rs_select, 1, 1024, 0, st, s->models.as<double>(), s->cost.as<double>(), s->ninl.as<int>(), n2 * RS_MAX_SOL, dcand, go,
               (int*)nullptr, k, m, 0.0, 0.0);
     B2_CHECK_LAUNCH(ctx);
+    if (tr) {  // the extension's buffers are only worth recording when its kernels ran
+      B2_CUDA(ctx, cudaMemcpyAsync(&tr->ext_go, go, 4, cudaMemcpyDeviceToHost, st));
+      B2_CUDA(ctx, cudaStreamSynchronize(st));
+      if (tr->ext_go)
+        if (int rc = record(n2, false)) return rc;
+    }
   }
+  if (tr) B2_CUDA(ctx, cudaMemcpyAsync(tr->prerefine, dcand, sizeof(RsBest) * RS_TOP, cudaMemcpyDeviceToHost, st));
   B2_LAUNCH(ctx, k_rs_refine, RS_TOP, RS_LO_THREADS, 0, st, x1, x2, k, thr2, mode, dcand);
   B2_CHECK_LAUNCH(ctx);
+  if (tr) B2_CUDA(ctx, cudaMemcpyAsync(tr->refined, dcand, sizeof(RsBest) * RS_TOP, cudaMemcpyDeviceToHost, st));
   B2_LAUNCH(ctx, k_rs_pick, 1, 32, 0, st, dcand, dbest);
   B2_CHECK_LAUNCH(ctx);
   B2_LAUNCH(ctx, k_rs_mask, cdiv(k, 256), 256, 0, st, x1, x2, k, thr2, mode, dbest, s->mask.as<uint8_t>(), dcount);
   B2_CHECK_LAUNCH(ctx);
   const bool want_pose = mode == 0 && out_R && out_t;
+  int* gvotes = reinterpret_cast<int*>(s->pose.as<double>() + 32);
+  double* pose_cands = tr ? s->pose.as<double>() + 36 : nullptr;
   if (want_pose) {
-    int* gvotes = reinterpret_cast<int*>(s->pose.as<double>() + 32);
     B2_CUDA(ctx, cudaMemsetAsync(gvotes, 0, 8 * sizeof(int), st));
     B2_LAUNCH(ctx, k_rs_pose, cdiv(k, RS_POSE_THREADS), RS_POSE_THREADS, 0, st, dbest->model, x1, x2, s->mask.as<uint8_t>(), k, gvotes,
-              s->pose.as<double>());
+              s->pose.as<double>(), pose_cands);
     B2_CHECK_LAUNCH(ctx);
+  }
+  if (tr) {
+    B2_CUDA(ctx, cudaMemcpyAsync(&tr->pick, dbest, sizeof(RsBest), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(ctx, cudaMemcpyAsync(&tr->mask_count, dcount, 4, cudaMemcpyDeviceToHost, st));
+    if (want_pose) {
+      double c[22];
+      B2_CUDA(ctx, cudaMemcpyAsync(tr->votes, gvotes, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
+      B2_CUDA(ctx, cudaMemcpyAsync(c, pose_cands, sizeof(c), cudaMemcpyDeviceToHost, st));
+      B2_CUDA(ctx, cudaStreamSynchronize(st));
+      memcpy(tr->pose_cands, c, 21 * 8);
+      tr->winner = (int)c[21];
+    }
   }
   char* hb = s->hbuf.as<char>();
   B2_CUDA(ctx, cudaMemcpyAsync(hb, dbest, sizeof(RsBest) + 16, cudaMemcpyDeviceToHost, st));
@@ -685,8 +702,9 @@ extern "C" int b2_ransac_essential_dev(b2_context* ctx, const float* kp1, const 
                 st ? st : cudaStreamLegacy, 1);
 }
 
-extern "C" int b2_recover_pose_host(b2_context* ctx, const double* E, const double* x1, const double* x2, int k,
-                                    double* out_R, double* out_t, int* out_num_good) {
+// out_cands / out_votes / out_winner: tests only (nullptr from b2_recover_pose_host)
+static int recover_pose(b2_context* ctx, const double* E, const double* x1, const double* x2, int k, double* out_R, double* out_t,
+                        int* out_num_good, double* out_cands, int* out_votes, int* out_winner) {
   if (!ctx || !E || !out_R || !out_t || k < 0 || (k > 0 && (!x1 || !x2))) return B2_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
   cudaSetDevice(ctx->device);
@@ -695,7 +713,7 @@ extern "C" int b2_recover_pose_host(b2_context* ctx, const double* E, const doub
   cudaStream_t st = ctx->stream;
   B2_CUDA(ctx, s->x1.ensure((size_t)(k + 1) * 16));
   B2_CUDA(ctx, s->x2.ensure((size_t)(k + 1) * 16));
-  B2_CUDA(ctx, s->pose.ensure(48 * 8));
+  B2_CUDA(ctx, s->pose.ensure(64 * 8));
   B2_CUDA(ctx, s->hbuf.ensure(sizeof(RsBest) + 16 * 8 + 64));
   if (k > 0) {
     B2_CUDA(ctx, cudaMemcpyAsync(s->x1.p, x1, (size_t)k * 16, cudaMemcpyHostToDevice, st));
@@ -707,14 +725,48 @@ extern "C" int b2_recover_pose_host(b2_context* ctx, const double* E, const doub
     int* gvotes = reinterpret_cast<int*>(s->pose.as<double>() + 32);
     B2_CUDA(ctx, cudaMemsetAsync(gvotes, 0, 8 * sizeof(int), st));
     B2_LAUNCH(ctx, k_rs_pose, k > 0 ? cdiv(k, RS_POSE_THREADS) : 1, RS_POSE_THREADS, 0, st, dE, s->x1.as<double>(), s->x2.as<double>(),
-              (const uint8_t*)nullptr, k, gvotes, s->pose.as<double>());
+              (const uint8_t*)nullptr, k, gvotes, s->pose.as<double>(), out_cands ? s->pose.as<double>() + 36 : nullptr);
   }
   B2_CHECK_LAUNCH(ctx);
   double* h = s->hbuf.as<double>();
   B2_CUDA(ctx, cudaMemcpyAsync(h, s->pose.p, 13 * 8, cudaMemcpyDeviceToHost, st));
+  if (out_cands) {
+    double c[22];
+    B2_CUDA(ctx, cudaMemcpyAsync(c, s->pose.as<double>() + 36, sizeof(c), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(ctx, cudaMemcpyAsync(out_votes, s->pose.as<double>() + 32, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(ctx, cudaStreamSynchronize(st));
+    memcpy(out_cands, c, 21 * 8);
+    *out_winner = (int)c[21];
+  }
   B2_CUDA(ctx, cudaStreamSynchronize(st));
   memcpy(out_R, h, 9 * 8);
   memcpy(out_t, h + 9, 3 * 8);
   if (out_num_good) *out_num_good = (int)h[12];
   return B2_OK;
+}
+
+extern "C" int b2_recover_pose_host(b2_context* ctx, const double* E, const double* x1, const double* x2, int k,
+                                    double* out_R, double* out_t, int* out_num_good) {
+  return recover_pose(ctx, E, x1, x2, k, out_R, out_t, out_num_good, nullptr, nullptr, nullptr);
+}
+
+// ---- test-only entry points: the same kernels and host logic, with their intermediate state --------------------------
+
+extern "C" int b2_debug_recover_pose_host(b2_context* ctx, const double* E, const double* x1, const double* x2, int k,
+                                          double* out_cands, int* out_votes, int* out_winner, double* out_R, double* out_t,
+                                          int* out_num_good) {
+  if (!out_cands || !out_votes || !out_winner) return B2_ERR_ARG;
+  return recover_pose(ctx, E, x1, x2, k, out_R, out_t, out_num_good, out_cands, out_votes, out_winner);
+}
+
+extern "C" int b2_debug_ransac_trace_host(b2_context* ctx, int mode, const double* x1, const double* x2, int k,
+                                          const b2_ransac_params* params, b2_ransac_trace* trace, double* out_model,
+                                          uint8_t* out_mask, int* out_num_inliers, double* out_R, double* out_t) {
+  if (!ctx || !x1 || !x2 || !params || !trace || !out_model || !out_num_inliers || k < 0 || (mode != 0 && mode != 1) ||
+      trace->batch < 1 || trace->batch > RS_BATCH || trace->max_records < 0)
+    return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  return rs_run(ctx, x1, x2, k, params, mode, out_model, out_mask, out_num_inliers, mode == 0 ? out_R : nullptr,
+                mode == 0 ? out_t : nullptr, nullptr, 0, trace);
 }

@@ -519,6 +519,44 @@ RM_HDN void enforce_rank2(double* F) {
     for (int j = 0; j < 3; ++j) F[i * 3 + j] = U[i * 3] * s[0] * V[j * 3] + U[i * 3 + 1] * s[1] * V[j * 3 + 1];
 }
 
+// normalised 8-point algorithm (Hartley 1997) on 8 correspondences: F (unit Frobenius norm, rank 2) with x2^T F x1 = 0.
+// Returns 1, or 0 for a degenerate sample (coincident points, zero F).
+RM_HDN int eightpt_solve(const double (*x1)[2], const double (*x2)[2], double* F_out) {
+  double c1x = 0, c1y = 0, c2x = 0, c2y = 0;
+  for (int i = 0; i < 8; ++i) c1x += x1[i][0], c1y += x1[i][1], c2x += x2[i][0], c2y += x2[i][1];
+  c1x /= 8, c1y /= 8, c2x /= 8, c2y /= 8;
+  double d1 = 0, d2 = 0;
+  for (int i = 0; i < 8; ++i) {
+    d1 += sqrt((x1[i][0] - c1x) * (x1[i][0] - c1x) + (x1[i][1] - c1y) * (x1[i][1] - c1y));
+    d2 += sqrt((x2[i][0] - c2x) * (x2[i][0] - c2x) + (x2[i][1] - c2y) * (x2[i][1] - c2y));
+  }
+  if (d1 < 1e-12 || d2 < 1e-12) return 0;
+  double s1 = 1.4142135623730951 * 8 / d1, s2 = 1.4142135623730951 * 8 / d2;
+  double A[81];
+  for (int i = 0; i < 81; ++i) A[i] = 0;
+  for (int p = 0; p < 8; ++p) {
+    double ax = (x1[p][0] - c1x) * s1, ay = (x1[p][1] - c1y) * s1;
+    double bx = (x2[p][0] - c2x) * s2, by = (x2[p][1] - c2y) * s2;
+    double q[9] = {bx * ax, bx * ay, bx, by * ax, by * ay, by, ax, ay, 1.0};
+    for (int i = 0; i < 9; ++i)
+      for (int j = 0; j < 9; ++j) A[i * 9 + j] += q[i] * q[j];
+  }
+  double Fn[9];
+  smallest_eigvec9(A, Fn);
+  enforce_rank2(Fn);
+  // F = T2^T Fn T1, T = [s 0 -s c; 0 s -s c; 0 0 1]
+  double T1[9] = {s1, 0, -s1 * c1x, 0, s1, -s1 * c1y, 0, 0, 1}, T2t[9] = {s2, 0, 0, 0, s2, 0, -s2 * c2x, -s2 * c2y, 1};
+  double tmp[9], F[9];
+  mat3_mul(T2t, Fn, tmp);
+  mat3_mul(tmp, T1, F);
+  double n = 0;
+  for (int i = 0; i < 9; ++i) n += F[i] * F[i];
+  n = sqrt(n);
+  if (!(n > 1e-300)) return 0;
+  for (int i = 0; i < 9; ++i) F_out[i] = F[i] / n;
+  return 1;
+}
+
 // ---- pose from E -----------------------------------------------------------------------------------------------
 // The four (R, t) decompositions of E (Hartley & Zisserman 9.6.2): R = U W V^T or U W^T V^T, t = +-u3.
 RM_HDN void decompose_E(const double* E, double* R1, double* R2, double* t) {

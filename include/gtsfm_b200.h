@@ -251,6 +251,45 @@ int b2_ransac_essential_dev(b2_context* ctx, const float* kp1, const float* kp2,
 int b2_recover_pose_host(b2_context* ctx, const double* E, const double* x1, const double* x2, int k, double* out_R,
                          double* out_t, int* out_num_good);
 
+/* Test-only: the verifier's intermediate state.  One RANSAC candidate (the layout the kernels keep on the device). */
+typedef struct b2_ransac_candidate {
+  double model[9];
+  double cost;  /* MSAC cost; 1e300 when not valid */
+  int ninl;
+  int valid;
+} b2_ransac_candidate;
+/* A record is one k_rs_select launch: a sampling batch, or the E extension stage (always the record after the last
+ * batch when it is enqueued).  Array pointers may be NULL (not recorded); the arrays have room for `max_records`. */
+typedef struct b2_ransac_trace {
+  int batch;                       /* in: hypotheses per launch, 1 .. 16384 (production: 16384) */
+  int max_records;                 /* in: records the arrays below hold */
+  int* nsol;                       /* [max_records][batch] solutions per sample */
+  double* models;                  /* [max_records][batch][10][9] */
+  double* cost;                    /* [max_records][batch * 10] MSAC cost per slot (1e300 for an empty slot) */
+  int* ninl;                       /* [max_records][batch * 10] */
+  b2_ransac_candidate* selected;   /* [max_records][8] the candidate list after the record's k_rs_select */
+  int* more;                       /* [max_records] the confidence flag that select wrote (-1: the extension writes none) */
+  int batches;                     /* out: sampling batches run (the extension not counted) */
+  int ext_go;                      /* out: -1 extension not enqueued, else the flag it ran under (0: its kernels returned) */
+  int records;                     /* out: records written (<= max_records) */
+  b2_ransac_candidate prerefine[8];/* out: the list handed to k_rs_refine */
+  b2_ransac_candidate refined[8];  /* out: the list after k_rs_refine */
+  b2_ransac_candidate pick;        /* out: k_rs_pick's result */
+  int mask_count;                  /* out: k_rs_mask's inlier count */
+  int votes[4];                    /* out (E): cheirality votes of (R1,t), (R2,t), (R1,-t), (R2,-t) */
+  int winner;                      /* out (E): index of the winning decomposition */
+  double pose_cands[21];           /* out (E): the device's R1 [9], R2 [9], t [3] */
+} b2_ransac_trace;
+/* Test-only: rs_run with a trace.  mode 0 = essential (5-point, Sampson), 1 = fundamental (8-point, epiline).  Same
+ * arguments and return value as b2_ransac_essential_host / _fundamental_host; out_R / out_t are used for mode 0. */
+int b2_debug_ransac_trace_host(b2_context* ctx, int mode, const double* x1, const double* x2, int k,
+                               const b2_ransac_params* params, b2_ransac_trace* trace, double* out_model, uint8_t* out_mask,
+                               int* out_num_inliers, double* out_R, double* out_t);
+/* Test-only: b2_recover_pose_host that also returns the device's four decompositions (R1 [9], R2 [9], t [3]), the four
+ * vote totals and the winner's index. */
+int b2_debug_recover_pose_host(b2_context* ctx, const double* E, const double* x1, const double* x2, int k, double* out_cands,
+                               int* out_votes, int* out_winner, double* out_R, double* out_t, int* out_num_good);
+
 /* ---- NetVLAD global descriptor (SURVEY.md section 8f rank 4; gtsfm/frontend/global_descriptor/netvlad_global_descriptor.py:53-71,
  * thirdparty/hloc/netvlad.py:52-75,163-193) ------------------------------------------------------------------------------------- */
 /* blob = 13 x (conv weight OIHW, bias) of VGG16 features[:-2], score_proj [64][512], centers [512][64], whitening weight
