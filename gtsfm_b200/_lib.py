@@ -23,7 +23,12 @@ class LightGlueParams(C.Structure):
 
 class LightGluePair(C.Structure):
     _fields_ = [("kp0", C.c_void_p), ("desc0", C.c_void_p), ("n0", C.c_int), ("kp1", C.c_void_p), ("desc1", C.c_void_p), ("n1", C.c_int),
-                ("out_matches", C.c_void_p), ("out_scores", C.c_void_p), ("out_k", C.c_int), ("out_stop_layer", C.c_int)]
+                ("out_matches", C.c_void_p), ("out_scores", C.c_void_p), ("out_k", C.c_int), ("out_stop_layer", C.c_int),
+                ("enc0", C.c_void_p), ("enc1", C.c_void_p)]
+
+
+class LightGlueImage(C.Structure):
+    _fields_ = [("kp", C.c_void_p), ("desc", C.c_void_p), ("n", C.c_int), ("out", C.c_void_p)]
 
 
 class MnnPair(C.Structure):
@@ -113,6 +118,8 @@ SIGNATURES = {
     "b2_lightglue_match_dev": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, C.POINTER(LightGlueParams), _vp, _vp, _ip, _ip, _vp]),
     "b2_lightglue_match_host": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, C.POINTER(LightGlueParams), _vp, _vp, _ip, _ip]),
     "b2_lightglue_match_batched_dev": (_i, [_vp, C.POINTER(LightGluePair), _i, C.POINTER(LightGlueParams), _vp]),
+    "b2_lightglue_encoded_bytes": (_sz, [_i]),
+    "b2_lightglue_encode_batched_dev": (_i, [_vp, C.POINTER(LightGlueImage), _i, C.POINTER(LightGlueParams), _vp]),
     "b2_superglue_set_weights": (_i, [_vp, _vp, _sz]),
     "b2_superglue_match_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _vp, _ip, _vp]),
     "b2_superglue_match_host": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _vp, _ip]),
@@ -192,6 +199,7 @@ class Context:
                 f"b2_create(device={device}) failed with {rc}: an sm_90 (H100) GPU is required; there is no CPU fallback")
         self.handle = h
         self.device = device
+        self.options = {}  # what set_option was given, by name (the last value)
 
     def check(self, rc: int, what: str) -> None:
         if rc < 0:
@@ -206,6 +214,7 @@ class Context:
 
     def set_option(self, name: str, value: int) -> None:
         self.check(self._lib.b2_set_option(self.handle, name.encode(), int(value)), f"set_option({name})")
+        self.options[name] = int(value)
 
     def h2d_bytes(self) -> int:
         return int(self._lib.b2_h2d_bytes(self.handle))

@@ -152,6 +152,35 @@ __global__ void __launch_bounds__(256) k_lg_load_desc(const __grid_constant__ Jo
   }
 }
 
+// An image's encoding (b2_lightglue_encode_batched_dev): its state after the layer-0 self block, packed row-count-major as
+// x fp32 [n][256] | x hi [n][256] | x lo [n][256] (split planes, wgmma path only) | cos [n][32] | sin [n][32].
+constexpr size_t LG_ENC_ROW_BYTES = 256 * 4 + 2 * 256 * 2 + 2 * 32 * 4;
+struct EncJob {
+  float4* blob;
+  int n;
+  float* x;
+  __half *hi, *lo;  // null on the SIMT path: the blob's plane segments are neither written nor read
+  float *cs, *sn;
+  int* ind;
+};
+// to_blob = 1: side workspace -> blob.  0: blob -> side workspace, and ind[n] = n.
+__global__ void __launch_bounds__(256) k_lg_enc_copy(const __grid_constant__ JobList<EncJob> jobs, int to_blob) {
+  const EncJob& jb = jobs.j[blockIdx.y];
+  const size_t n = (size_t)jb.n, g = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // float4 index into the blob
+  if (!to_blob && g < n) jb.ind[g] = (int)g;
+  size_t i = g;
+  float4* side;
+  if (i < n * 64) side = reinterpret_cast<float4*>(jb.x);
+  else if ((i -= n * 64) < n * 32) side = reinterpret_cast<float4*>(jb.hi);
+  else if ((i -= n * 32) < n * 32) side = reinterpret_cast<float4*>(jb.lo);
+  else if ((i -= n * 32) < n * 8) side = reinterpret_cast<float4*>(jb.cs);
+  else if ((i -= n * 8) < n * 8) side = reinterpret_cast<float4*>(jb.sn);
+  else return;
+  if (!side) return;
+  if (to_blob) jb.blob[g] = side[i];
+  else side[i] = jb.blob[g];
+}
+
 // SIMT path: qkv [N][768] as [q | k | v] (b2_lightglue_qkv_rows) -> rotary on q,k (lightglue.py:58-65) -> fp32 [4][N][64].
 // The wgmma path does the same in the projection's epilogue (gemm_ws.cuh, column segments).
 struct RotJob {  // one image's share of a two-image launch (blockIdx.y)
@@ -869,6 +898,45 @@ static int lg_cross_block(b2_context* ctx, cudaStream_t st, LightGlueState* s, c
   return lg_out_and_ffn(ctx, st, s, act, "lg_cross", w.wout, w.bout, w.w0, w.b0, w.lng, w.lnb, w.w3, w.b3);
 }
 
+// Network input of the sides in `act` (kp[i], desc[i] belong to act.side[i]): x = desc and its split planes, the rotary
+// table of the keypoints, ind = identity.
+static int lg_load_sides(b2_context* ctx, cudaStream_t st, LightGlueState* s, const LgActive& act, const float* const* kp,
+                         const float* const* desc) {
+  if (act.n == 0) return B2_OK;
+  JobList<LoadJob> lj{};
+  JobList<PosJob> pj{};
+  for (int i = 0; i < act.n; ++i) {
+    LgSide& sd = s->side[act.side[i]];
+    const Pl xp = planes_of(sd.xs[0], (size_t)sd.cap * 256);
+    lj.j[i] = {desc[i], sd.n, sd.x[0].as<float>(), s->use_tc ? xp.hi : (__half*)nullptr, s->use_tc ? xp.lo : (__half*)nullptr};
+    pj.j[i] = {kp[i], sd.n, sd.cs[0].as<float>(), sd.sn[0].as<float>(), sd.ind[0].as<int>()};
+  }
+  const int mx = lg_max_n(s, act);
+  B2_LAUNCH(ctx, k_lg_load_desc, dim3(cdiv(mx * 64, 256), act.n), 256, 0, st, lj);
+  B2_CHECK_LAUNCH(ctx);
+  const int pb = cdiv(mx * 32, 1024);
+  B2_LAUNCH(ctx, k_lg_posenc, dim3(pb < 16 ? pb : 16, act.n), 1024, 0, st, pj, s->wr);
+  B2_CHECK_LAUNCH(ctx);
+  return B2_OK;
+}
+
+// Copies the live layer-0 state (x / xs / cs / sn [0]) of the sides in `act` to the encoding blob[i] of act.side[i]
+// (to_blob), or back from it, setting ind[0] to the identity.
+static int lg_enc_copy(b2_context* ctx, cudaStream_t st, LightGlueState* s, const LgActive& act, void* const* blob, bool to_blob) {
+  if (act.n == 0) return B2_OK;
+  JobList<EncJob> ej{};
+  for (int i = 0; i < act.n; ++i) {
+    LgSide& sd = s->side[act.side[i]];
+    const Pl xp = planes_of(sd.xs[0], (size_t)sd.cap * 256);
+    ej.j[i] = {static_cast<float4*>(blob[i]), sd.n, sd.x[0].as<float>(), s->use_tc ? xp.hi : (__half*)nullptr,
+               s->use_tc ? xp.lo : (__half*)nullptr, sd.cs[0].as<float>(), sd.sn[0].as<float>(), sd.ind[0].as<int>()};
+  }
+  const int mx = lg_max_n(s, act);
+  B2_LAUNCH(ctx, k_lg_enc_copy, dim3(cdiv(mx * (int)(LG_ENC_ROW_BYTES / 16), 256), act.n), 256, 0, st, ej, to_blob ? 1 : 0);
+  B2_CHECK_LAUNCH(ctx);
+  return B2_OK;
+}
+
 // One batch of up to LG_MAX_PAIRS pairs walked in lock-step (lightglue.py:474-629 for each of them).
 static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, const b2_lightglue_params* prm, cudaStream_t st) {
   LightGlueState* s = ctx->lg;
@@ -888,33 +956,30 @@ static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, con
   }
   LgActive act = lg_active_sides(s, np);
   if (act.n == 0) return B2_OK;
-  {
-    JobList<LoadJob> lj{};
-    JobList<PosJob> pj{};
-    for (int i = 0; i < act.n; ++i) {
-      const int sdi = act.side[i];
-      LgSide& sd = s->side[sdi];
-      const b2_lightglue_pair& pr = pairs[sdi >> 1];
-      const float* desc = (sdi & 1) ? pr.desc1 : pr.desc0;
-      const float* kp = (sdi & 1) ? pr.kp1 : pr.kp0;
-      const Pl xp = planes_of(sd.xs[0], (size_t)sd.cap * 256);
-      lj.j[i] = {desc, sd.n, sd.x[0].as<float>(), s->use_tc ? xp.hi : (__half*)nullptr, s->use_tc ? xp.lo : (__half*)nullptr};
-      pj.j[i] = {kp, sd.n, sd.cs[0].as<float>(), sd.sn[0].as<float>(), sd.ind[0].as<int>()};
+  LgActive fresh, encoded;  // sides handed in as features / as encodings (which have been through layer 0's self block)
+  const float *kp[LG_MAX_SIDES], *desc[LG_MAX_SIDES];
+  void* blob[LG_MAX_SIDES];
+  for (int i = 0; i < act.n; ++i) {
+    const int sdi = act.side[i];
+    const b2_lightglue_pair& pr = pairs[sdi >> 1];
+    const void* enc = (sdi & 1) ? pr.enc1 : pr.enc0;
+    if (enc) {
+      blob[encoded.n] = const_cast<void*>(enc);
+      encoded.side[encoded.n++] = sdi;
+    } else {
+      kp[fresh.n] = (sdi & 1) ? pr.kp1 : pr.kp0, desc[fresh.n] = (sdi & 1) ? pr.desc1 : pr.desc0;
+      fresh.side[fresh.n++] = sdi;
     }
-    const int mx = lg_max_n(s, act);
-    B2_LAUNCH(ctx, k_lg_load_desc, dim3(cdiv(mx * 64, 256), act.n), 256, 0, st, lj);
-    B2_CHECK_LAUNCH(ctx);
-    const int pb = cdiv(mx * 32, 1024);
-    B2_LAUNCH(ctx, k_lg_posenc, dim3(pb < 16 ? pb : 16, act.n), 1024, 0, st, pj, s->wr);
-    B2_CHECK_LAUNCH(ctx);
   }
+  if ((rc = lg_load_sides(ctx, st, s, fresh, kp, desc))) return rc;
+  if ((rc = lg_enc_copy(ctx, st, s, encoded, blob, false))) return rc;
   const bool do_stop = prm->depth_confidence > 0.0, do_prune = prm->width_confidence > 0.0;
   const float keep_thr = (float)(1.0 - prm->width_confidence);  // scores > float32(1 - width_confidence)
   int* counters = s->counters.as<int>();
   int* hread = s->hread.as<int>();
   for (int layer = 0; layer < LG_LAYERS && act.n > 0; ++layer) {
     const bool fp16_attn = prm->fp16_attention != 0 && s->use_tc;
-    if ((rc = lg_self_layer(ctx, st, s, act, layer, fp16_attn))) return rc;
+    if ((rc = lg_self_layer(ctx, st, s, layer == 0 ? fresh : act, layer, fp16_attn))) return rc;
     if ((rc = lg_cross_block(ctx, st, s, act, layer, fp16_attn))) return rc;
     for (int p = 0; p < np; ++p)
       if (s->pair[p].active) s->pair[p].stop = layer;
@@ -1063,10 +1128,48 @@ extern "C" int b2_lightglue_match_batched_dev(b2_context* ctx, b2_lightglue_pair
     const b2_lightglue_pair& pr = pairs[p];
     if (pr.n0 < 0 || pr.n1 < 0) return B2_ERR_ARG;
     if (pr.n0 > 0 && pr.n1 > 0 && (!pr.kp0 || !pr.desc0 || !pr.kp1 || !pr.desc1 || !pr.out_matches)) return B2_ERR_ARG;
+    if (((uintptr_t)pr.enc0 | (uintptr_t)pr.enc1) & 15) return B2_ERR_ARG;  // the blob is copied 16 bytes at a time
   }
   std::lock_guard<std::mutex> lk(ctx->mu);
   cudaSetDevice(ctx->device);
   return lg_match_pairs(ctx, pairs, n_pairs, params, (cudaStream_t)stream);
+}
+
+extern "C" size_t b2_lightglue_encoded_bytes(int n) { return n > 0 ? (size_t)n * LG_ENC_ROW_BYTES : 0; }
+
+extern "C" int b2_lightglue_encode_batched_dev(b2_context* ctx, const b2_lightglue_image* imgs, int n_imgs, const b2_lightglue_params* params,
+                                               void* stream) {
+  if (!ctx || !params || n_imgs < 0 || (n_imgs > 0 && !imgs)) return B2_ERR_ARG;
+  for (int i = 0; i < n_imgs; ++i) {
+    const b2_lightglue_image& im = imgs[i];
+    if (im.n < 0 || (im.n > 0 && (!im.kp || !im.desc || !im.out || ((uintptr_t)im.out & 15)))) return B2_ERR_ARG;
+  }
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  LightGlueState* s = ctx->lg;
+  if (!s || !s->loaded) return b2_fail(ctx, B2_ERR_STATE, "lightglue weights not set");
+  s->persist_ctas = ctx->sm_count - ctx->reserve_sms > 0 ? ctx->sm_count - ctx->reserve_sms : 1;
+  const cudaStream_t st = (cudaStream_t)stream;
+  const bool fp16_attn = params->fp16_attention != 0 && s->use_tc;
+  int rc;
+  // the images go through layer 0's self block LG_MAX_SIDES at a time on the side workspaces, as the sides of a batch do
+  for (int i = 0; i < n_imgs;) {
+    LgActive act;
+    const float *kp[LG_MAX_SIDES], *desc[LG_MAX_SIDES];
+    void* out[LG_MAX_SIDES];
+    for (; i < n_imgs && act.n < LG_MAX_SIDES; ++i) {
+      const b2_lightglue_image& im = imgs[i];
+      if (im.n == 0) continue;
+      if ((rc = lg_side_alloc(ctx, s->side[act.n], im.n, s->use_tc))) return rc;
+      kp[act.n] = im.kp, desc[act.n] = im.desc, out[act.n] = im.out;
+      act.side[act.n] = act.n;
+      ++act.n;
+    }
+    if ((rc = lg_load_sides(ctx, st, s, act, kp, desc))) return rc;
+    if ((rc = lg_self_layer(ctx, st, s, act, 0, fp16_attn))) return rc;
+    if ((rc = lg_enc_copy(ctx, st, s, act, out, true))) return rc;
+  }
+  return B2_OK;
 }
 
 extern "C" int b2_lightglue_match_dev(b2_context* ctx, const float* kp0, const float* desc0, int n0, const float* kp1,

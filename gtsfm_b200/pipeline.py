@@ -8,10 +8,11 @@ PyTorch is used for device buffers and the stream only; all arithmetic is libgts
 from __future__ import annotations
 
 import contextlib
+import itertools
 import os
 import threading
-from dataclasses import dataclass
-from typing import List, Optional, Sequence, Tuple
+from dataclasses import dataclass, field
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -27,6 +28,9 @@ class DeviceFeatures:
     score: torch.Tensor  # (k,)
     desc: torch.Tensor  # (k, 256)
     shape: Tuple[int, int]
+    # LightGlue's pair-independent layer-0 state of this image (b2_lightglue_encode_batched_dev), made on first use by
+    # DeviceFrontEnd.match_batch / match_many and keyed by DeviceFrontEnd._enc_key(); freed with the features
+    enc: Dict[tuple, torch.Tensor] = field(default_factory=dict, repr=False, compare=False)
 
     def __len__(self) -> int:
         return int(self.kp.shape[0])
@@ -40,6 +44,7 @@ DETECT_LANES = int(os.environ.get("B2_DETECT_LANES", "4"))  # concurrent SuperPo
 # SMs the matcher's persistent kernels leave to the concurrent RANSAC kernels.  H100 (132 SMs), 40-pair LightGlue steps:
 # 99 pairs/s reserving 8, 103-107 reserving 0-4; 4 keeps k_rs_hyp_E's CTAs off the matcher's SMs at no measured cost
 RESERVE_SMS_FOR_VERIFY = int(os.environ.get("B2_RESERVE_SMS", "4"))
+_FRONT_END_SERIAL = itertools.count()  # one per DeviceFrontEnd: an image's LightGlue encoding is only valid for the one that made it
 
 
 class DeviceFrontEnd:
@@ -62,6 +67,9 @@ class DeviceFrontEnd:
         self._mlanes = []  # extra (context, stream, executor) LightGlue lanes of match_many
         self._mpool0 = None
         self._reserve_sms = 0
+        self._serial = next(_FRONT_END_SERIAL)
+        # the kernel path (force_simt) LightGlue's weights are loaded under; the extra match_many lanes load them the same way
+        self._lg_simt = self.ctx.options.get("force_simt")
         if lightglue_sd is not None:
             blob = weights.pack_lightglue(weights.load_state_dict(lightglue_sd))
             self._lg_blob = blob
@@ -299,6 +307,7 @@ class DeviceFrontEnd:
         as a batch is complete - the hook bench.py uses to start verification early.  Results in input order."""
         from concurrent.futures import ThreadPoolExecutor
 
+        self.encode([f for p in pairs for f in p])  # on the caller's stream, before the lanes wait for it
         chunks = [(c0, pairs[c0:c0 + 8]) for c0 in range(0, len(pairs), 8)]
         lanes = min(MATCH_LANES, len(chunks))
         if lanes <= 1:
@@ -311,6 +320,8 @@ class DeviceFrontEnd:
             return out
         while len(self._mlanes) < lanes - 1:  # extra lanes: context + LightGlue weights + stream + a one-thread executor
             ctx = _lib.Context(self.device.index or 0)
+            if self._lg_simt is not None:
+                ctx.set_option("force_simt", self._lg_simt)
             ctx.check(self.lib.b2_lightglue_set_weights(ctx.handle, _lib.ptr(self._lg_blob), self._lg_blob.size), "lightglue_set_weights")
             ctx.set_option("reserve_sms", self._reserve_sms)
             self._mlanes.append((ctx, torch.cuda.Stream(self.device), ThreadPoolExecutor(max_workers=1)))
@@ -347,23 +358,50 @@ class DeviceFrontEnd:
     def match_batch(self, pairs: Sequence[Tuple[DeviceFeatures, DeviceFeatures]], depth_confidence=0.95, width_confidence=0.99,
                     filter_threshold=0.1, ctx: Optional[_lib.Context] = None) -> List[Tuple[torch.Tensor, int]]:
         """LightGlue over a list of pairs through `b2_lightglue_match_batched_dev`: the library walks up to 8 pairs in
-        lock-step (one launch per layer step for all their images).  -> [(matches (k, 2) int64 device tensor, stop layer)]."""
+        lock-step (one launch per layer step for all their images), starting every image from its encoding (`encode`).
+        -> [(matches (k, 2) int64 device tensor, stop layer)]."""
         n = len(pairs)
         if n == 0:
             return []
+        ctx = ctx or self.ctx
+        key = self.encode([f for p in pairs for f in p], ctx=ctx)
         arr = (_lib.LightGluePair * n)()
         outs = []
         for i, (a, b) in enumerate(pairs):
             out = torch.empty((max(1, min(len(a), len(b))), 2), dtype=torch.int64, device=self.device)
             outs.append(out)
-            arr[i].kp0, arr[i].desc0, arr[i].n0 = a.kp.data_ptr(), a.desc.data_ptr(), len(a)
-            arr[i].kp1, arr[i].desc1, arr[i].n1 = b.kp.data_ptr(), b.desc.data_ptr(), len(b)
+            arr[i].kp0, arr[i].desc0, arr[i].n0, arr[i].enc0 = a.kp.data_ptr(), a.desc.data_ptr(), len(a), a.enc[key].data_ptr()
+            arr[i].kp1, arr[i].desc1, arr[i].n1, arr[i].enc1 = b.kp.data_ptr(), b.desc.data_ptr(), len(b), b.enc[key].data_ptr()
             arr[i].out_matches, arr[i].out_scores = out.data_ptr(), None
         prm = _lib.LightGlueParams(depth_confidence, width_confidence, filter_threshold, self.prune_min, self.fp16_attention)
-        ctx = ctx or self.ctx
         rc = self.lib.b2_lightglue_match_batched_dev(ctx.handle, arr, n, _lib.C.byref(prm), self._stream())
         ctx.check(rc, "lightglue_match_batched_dev")
         return [(outs[i][: arr[i].out_k], int(arr[i].out_stop_layer)) for i in range(n)]
+
+    def _enc_key(self) -> tuple:
+        # an encoding holds layer-0 activations: valid only under the weights and kernel path (force_simt) of the front end
+        # that made it, and under the attention numerics it was made with
+        return self._serial, self.fp16_attention
+
+    def encode(self, feats: Sequence[DeviceFeatures], ctx: Optional[_lib.Context] = None) -> tuple:
+        """Give every image in `feats` that has none its LightGlue encoding under this front end (the state after layer 0's
+        self block, which does not depend on the partner image): one b2_lightglue_encode_batched_dev call on the current
+        stream for all of them, so that an image matched against many partners runs that block once.  -> the encoding key."""
+        key = self._enc_key()
+        todo = list({id(f): f for f in feats if key not in f.enc}.values())
+        if not todo:
+            return key
+        bufs = [torch.empty(int(self.lib.b2_lightglue_encoded_bytes(len(f))), dtype=torch.uint8, device=self.device) for f in todo]
+        imgs = (_lib.LightGlueImage * len(todo))()
+        for i, (f, buf) in enumerate(zip(todo, bufs)):
+            imgs[i].kp, imgs[i].desc, imgs[i].n, imgs[i].out = f.kp.data_ptr(), f.desc.data_ptr(), len(f), buf.data_ptr()
+        prm = _lib.LightGlueParams(0.0, 0.0, 0.0, self.prune_min, self.fp16_attention)
+        ctx = ctx or self.ctx
+        ctx.check(self.lib.b2_lightglue_encode_batched_dev(ctx.handle, imgs, len(todo), _lib.C.byref(prm), self._stream()),
+                  "lightglue_encode_batched_dev")
+        for f, buf in zip(todo, bufs):
+            f.enc[key] = buf
+        return key
 
     def verify_async(self, a: DeviceFeatures, b: DeviceFeatures, matches: torch.Tensor, cal1, cal2, threshold_px: float = 4.0,
                      seed: int = DEFAULT_SEED):

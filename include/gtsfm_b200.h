@@ -187,8 +187,13 @@ int b2_lightglue_match_host(b2_context* ctx, const float* kp0, const float* desc
  * gtsfm/frontend/correspondence_generator/det_desc_correspondence_generator.py:65-85, one matcher task per pair).  Up to 8
  * pairs at a time are walked in lock-step: every linear layer, attention call and pruning step is ONE launch over all
  * images of the batch, the per-layer early-exit / pruning counters of all pairs come back in one 128-byte read, pairs
- * that stop early drop out of the later launches.  Results are identical to n_pairs calls of b2_lightglue_match_dev.
- * All pointers inside `pairs` are DEVICE pointers; out_k / out_stop_layer are written on the HOST struct. */
+ * that stop early drop out of the later launches.  Each image goes through the same kernels as in n_pairs calls of
+ * b2_lightglue_match_dev, but the wgmma attention splits its key range by the launch's total work, so internal state and
+ * match scores may differ from the per-pair calls in the last bits, and a match or early-exit decision that sits on its
+ * threshold to that precision could differ.  The SIMT kernels (force_simt) do not split: there results are bit-identical.
+ * All pointers inside `pairs` are DEVICE pointers; out_k / out_stop_layer are written on the HOST struct.
+ * enc0 / enc1: NULL, or a blob b2_lightglue_encode_batched_dev made from (kp0, desc0) / (kp1, desc1) on a context with the
+ * same weights and kernel path (force_simt) under the same fp16_attention; that side then skips its layer-0 self block. */
 typedef struct b2_lightglue_pair {
   const float* kp0;   /* [n0][2] (x, y) pixels */
   const float* desc0; /* [n0][256] */
@@ -200,9 +205,27 @@ typedef struct b2_lightglue_pair {
   float* out_scores;    /* [min(n0, n1)] or NULL */
   int out_k;            /* written: number of matches */
   int out_stop_layer;   /* written: 1-based stopping layer */
+  const void* enc0;     /* [b2_lightglue_encoded_bytes(n0)] or NULL */
+  const void* enc1;     /* [b2_lightglue_encoded_bytes(n1)] or NULL */
 } b2_lightglue_pair;
 int b2_lightglue_match_batched_dev(b2_context* ctx, b2_lightglue_pair* pairs, int n_pairs, const b2_lightglue_params* params,
                                    void* stream);
+
+/* Pair-independent encoding of one image: LightGlue's state after the layer-0 self block (input_proj is the identity
+ * for SuperPoint, the positional encoding normalises by the image's own bounding box, and pruning / early exit are
+ * decided after layer 0's cross block, so none of it depends on the partner).  An image matched against many partners
+ * is encoded once and handed to b2_lightglue_match_batched_dev as enc0 / enc1.  `out` is a caller-allocated DEVICE
+ * blob of b2_lightglue_encoded_bytes(n) bytes (n = 0 allowed) whose layout is private to the library; kp / desc are
+ * DEVICE pointers.  Of `params` only fp16_attention is used.  Enqueued on `stream`, does not synchronise it. */
+typedef struct b2_lightglue_image {
+  const float* kp;   /* [n][2] (x, y) pixels */
+  const float* desc; /* [n][256] */
+  int n;
+  void* out;
+} b2_lightglue_image;
+size_t b2_lightglue_encoded_bytes(int n);
+int b2_lightglue_encode_batched_dev(b2_context* ctx, const b2_lightglue_image* imgs, int n_imgs, const b2_lightglue_params* params,
+                                    void* stream);
 
 /* ---- SuperGlue --------------------------------------------------------------------------------------------------- */
 /* `blob`: packed fp32 tensors in gtsfm_b200/weights.py::SUPERGLUE_ORDER with eval-mode BatchNorm already folded

@@ -33,7 +33,7 @@ LOOKAHEAD, NEW_FRAMES, THR_PX = 20, 2, 4.0
 
 GEMM_SITES = ["lg_self_qkv", "lg_self_out", "lg_self_ffn0", "lg_self_ffn3", "lg_cross_qk", "lg_cross_v", "lg_cross_qv",
               "lg_cross_out", "lg_cross_ffn0", "lg_cross_ffn3", "lg_assign_proj", "lg_assign_sim"]
-LG_KERNELS = ["k_lg_load_desc", "k_lg_posenc", "k_lg_split_rotary", "k_lg_ln_gelu", "k_lg_rowheads", "k_lg_prune_plan", "k_lg_gather",
+LG_KERNELS = ["k_lg_load_desc", "k_lg_posenc", "k_lg_enc_copy", "k_lg_split_rotary", "k_lg_ln_gelu", "k_lg_rowheads", "k_lg_prune_plan", "k_lg_gather",
               "k_lg_assign", "k_lg_row_stats", "k_lg_col_stats", "k_lg_row_argmax", "k_lg_col_argmax", "k_lg_filter"]
 # (N, K) of each GEMM site and its HBM bytes per output row: split-fp16 A planes are 4 B per element, plane outputs 4 B,
 # fp32 outputs / residuals 4 B, the rotary table 2 x 32 x 4 B per row of each of q and k
