@@ -71,6 +71,16 @@ class RansacParams(C.Structure):
     _fields_ = [("threshold", C.c_double), ("confidence", C.c_double), ("max_iters", C.c_int), ("seed", C.c_uint64)]
 
 
+class RansacProblem(C.Structure):  # b2_ransac_problem
+    _fields_ = [("kp1", C.c_void_p), ("kp2", C.c_void_p), ("matches", C.c_void_p), ("x1", C.c_void_p), ("x2", C.c_void_p),
+                ("k", C.c_int), ("mode", C.c_int), ("max_iters", C.c_int), ("cal1", C.c_double * 3), ("cal2", C.c_double * 3),
+                ("threshold", C.c_double), ("mask", C.c_void_p)]
+
+
+class RansacResult(C.Structure):  # b2_ransac_result
+    _fields_ = [("status", C.c_int), ("num_inliers", C.c_int), ("model", C.c_double * 9), ("R", C.c_double * 9), ("t", C.c_double * 3)]
+
+
 class RansacCandidate(C.Structure):
     _fields_ = [("model", C.c_double * 9), ("cost", C.c_double), ("ninl", C.c_int), ("valid", C.c_int)]
 
@@ -137,6 +147,10 @@ SIGNATURES = {
     "b2_ransac_essential_host": (_i, [_vp, _vp, _vp, _i, C.POINTER(RansacParams), _vp, _vp, _ip, _vp, _vp]),
     "b2_ransac_fundamental_host": (_i, [_vp, _vp, _vp, _i, C.POINTER(RansacParams), _vp, _vp, _ip]),
     "b2_ransac_essential_dev": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, C.POINTER(RansacParams), _vp, _vp, _ip, _vp, _vp, _vp]),
+    "b2_ransac_verify_batched_dev": (_i, [_vp, C.POINTER(RansacProblem), _i, C.POINTER(RansacParams), C.POINTER(RansacResult), _vp]),
+    "b2_ransac_workspace_bytes": (_sz, [C.POINTER(RansacProblem)]),
+    "b2_ransac_plan": (_i, [C.POINTER(RansacProblem), _i, _sz, _ip]),
+    "b2_ransac_sync_count": (C.c_uint64, [_vp]),
     "b2_recover_pose_host": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _ip]),
     "b2_debug_ransac_trace_host": (_i, [_vp, _i, _vp, _vp, _i, C.POINTER(RansacParams), C.POINTER(RansacTrace), _vp, _vp, _ip, _vp, _vp]),
     "b2_debug_recover_pose_host": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _ip, _vp, _vp, _ip]),
@@ -211,6 +225,10 @@ class Context:
 
     def launch_count(self) -> int:
         return int(self._lib.b2_launch_count(self.handle))
+
+    def ransac_sync_count(self) -> int:
+        """Stream synchronisations the RANSAC entry points have performed through this context."""
+        return int(self._lib.b2_ransac_sync_count(self.handle))
 
     def set_option(self, name: str, value: int) -> None:
         self.check(self._lib.b2_set_option(self.handle, name.encode(), int(value)), f"set_option({name})")

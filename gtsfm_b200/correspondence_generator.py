@@ -122,12 +122,12 @@ class B200CorrespondenceGenerator(_Base):
         pending = []
 
         def on_chunk(c0, res):  # lock-step batches of 8 pairs (b2_lightglue_match_batched_dev), in completion order
-            for (i1, i2), (m, _) in zip(mine[c0:c0 + len(res)], res):
-                if verify_with is not None and int(m.shape[0]) >= 6:
-                    intr, thr = verify_with
-                    pending.append(((i1, i2), m, fe.verify_async(feats[i1], feats[i2], m, intr[i1], intr[i2], thr)))
-                elif verify_with is not None:
-                    pending.append(((i1, i2), m, None))
+            if verify_with is None:
+                return
+            intr, thr = verify_with  # the chunk is verified by one batched call (pairs under 6 matches fail inside it)
+            prs = mine[c0:c0 + len(res)]
+            items = [(feats[i1], feats[i2], m, intr[i1], intr[i2]) for (i1, i2), (m, _) in zip(prs, res)]
+            pending.append((prs, [m for m, _ in res], fe.verify_many_async(items, thr)))
 
         matched = fe.match_many([(feats[i1], feats[i2]) for i1, i2 in mine], on_chunk=on_chunk)
         for f in feats.values():  # the matcher's per-image encodings (11.5 MB at 5000 keypoints) are not needed past matching
@@ -136,14 +136,11 @@ class B200CorrespondenceGenerator(_Base):
         for (i1, i2), (m, _) in zip(mine, matched):
             local[(i1, i2)] = m.cpu().numpy()
         if verify_with is not None:
-            from .two_view import B200TwoViewBatch, _failure
+            from .two_view import B200TwoViewBatch
 
             self.last_two_view = {}
-            for item in pending:
-                if item[2] is None:
-                    self.last_two_view[item[0]] = _failure(int(item[1].shape[0]))
-                else:
-                    B200TwoViewBatch._collect(item, self.last_two_view)
+            for chunk in pending:
+                B200TwoViewBatch._collect_chunk(chunk, self.last_two_view)
         t_verify = time.perf_counter()
         self.last_device_features = feats
         matches = D.gather_pair_results(local)

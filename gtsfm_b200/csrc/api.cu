@@ -61,6 +61,11 @@ extern "C" int b2_set_option(b2_context* ctx, const char* name, int64_t value) {
     ctx->lg_batch = (int)value;
     return B2_OK;
   }
+  if (!strcmp(name, "ransac_workspace_mb")) {  // budget of one sub-batch of b2_ransac_verify_batched_dev
+    if (value < 1 || value > (1 << 20)) return b2_fail(ctx, B2_ERR_ARG, "ransac_workspace_mb takes 1..1048576");
+    ctx->rs_workspace_mb = (int)value;
+    return B2_OK;
+  }
   if (!strcmp(name, "superpoint_graph")) {  // 1 (default): replay the SuperPoint network as one CUDA graph; 0: direct launches
     ctx->sp_graph = value ? 1 : 0;
     return B2_OK;

@@ -122,10 +122,12 @@ struct b2_context {
   int reserve_sms = 0;  // SMs the persistent kernels of this context leave free (b2_set_option "reserve_sms")
   int lg_batch = 0;     // pairs per LightGlue batch (0 = the library maximum, 8); b2_set_option "lightglue_batch"
   int sp_graph = -1;    // SuperPoint network as a CUDA graph: 1 / 0, -1 = B2_SP_GRAPH env (default off)
+  int rs_workspace_mb = 1024;  // RANSAC workspace budget per sub-batch of a batched call; b2_set_option "ransac_workspace_mb"
   int force_simt = -1;  // 1: models loaded afterwards run the exact-fp32 SIMT kernels (no tensor cores); -1 = B2_FORCE_SIMT env
   std::string err;
   std::mutex mu;
   uint64_t launches = 0;
+  uint64_t rs_syncs = 0;  // stream synchronisations performed by the RANSAC entry points (b2_ransac_sync_count)
   ProfState prof;
   cudaStream_t stream = nullptr;  // owned; used by *_host entry points
   std::map<std::string, DebugView> debug;

@@ -9,6 +9,19 @@
 // Work decomposition: hypotheses are generated one per thread (fp64 minimal solvers from ransac_math.cuh), scored one
 // CTA per model over all matches, reduced to the best model by a single CTA, then refined / masked / decomposed by
 // single-CTA kernels.  Everything is deterministic for a given seed (fixed-order reductions, counter-based RNG).
+//
+// Every kernel takes a TABLE of problems (RsProb, device memory) and works on problem blockIdx.y, so one launch of a stage
+// covers every live pair of a call; problems never interact, and each runs the arithmetic, reduction order and tie rules
+// it would run alone, so a pair's result does not depend on what it is batched with.  The per-pair entry points are the
+// same code with a table of one.  Sampling rounds are enqueued for all live problems at once: the host rewrites the round
+// fields (first sample, count, flags) of the records that still run and uploads that compacted table; k_rs_select writes one
+// "confidence not reached" flag per problem, the E extension stage is gated by it on the device, and where a problem still
+// has budget left the host reads the whole flag array once per round and drops the problems that are done.
+//
+// Workspace: a problem's slices of models / nsol / cost / ninl hold its largest round (844 B per sample: 3.4 MB for an E
+// problem at 1000 + 4000 samples, 13.8 MB for an F round of 16 384), plus 32 B per match when the calibrated points are
+// made here.  A call is cut into consecutive sub-batches whose slices fit the workspace budget (1 GiB unless
+// b2_set_option "ransac_workspace_mb" says otherwise; a problem that alone exceeds it runs alone).
 #include <string.h>
 
 #include "common.cuh"
@@ -25,8 +38,57 @@ constexpr int RS_TOP = 8;  // hypotheses handed to the local optimisation (the r
 constexpr int RS_BATCH = 16384;  // hypotheses per launch (buffers are sized for it; a trace may ask for fewer)
 }  // namespace
 
+// best-model record kept on the device between rounds (the header's b2_ransac_candidate, so traces copy it as is)
+using RsBest = b2_ransac_candidate;
+
+// One problem as the kernels see it.  The host keeps the table of a sub-batch in pinned memory and uploads it once for the
+// stages that run on every problem (gather, refine, pick, mask, pose) and once per sampling round, compacted to the problems
+// that run the round, with the round fields set.
+struct RsProb {
+  const float *kp1, *kp2;     // k_rs_gather's input (null: x1 / x2 are ready)
+  const long long* matches;
+  double g1[3], g2[3];        // f, u0, v0 applied by k_rs_gather
+  double *x1, *x2;            // [k][2] points every later stage reads
+  int k, mode;                // mode 0 = essential (5-point, Sampson), 1 = fundamental (8-point, epiline)
+  double thr2;
+  // ---- this sampling round
+  int sample0, n;             // counter of the first sample, samples drawn
+  const int* go;              // extension stage: the round's kernels return at once unless *go
+  int* more;                  // where k_rs_select writes "the confidence bound needs more than done_after samples" (null: nowhere)
+  double done_after;
+  // ---- the problem's slices of the workspace
+  double* models;
+  int* nsol;
+  double* cost;
+  int* ninl;
+  RsBest *cand, *best;        // RS_TOP candidates, the result
+  int* count;                 // inliers counted by k_rs_mask
+  uint8_t* mask;
+  // ---- pose recovery
+  const double* E;            // the essential matrix, or (pose_cal) the fundamental matrix it is formed from
+  const uint8_t* pose_mask;   // null: every point votes
+  int* gvotes;                // [4] votes + [1] CTA counter, zero on entry
+  double* pose;               // R[9], t[3], votes of the winner
+  double* pose_cands;         // R1[9], R2[9], t[3], winner (tests only, else null)
+  int pose_on, pose_cal;      // pose_cal: x1 / x2 are pixels, E = K2^T F K1 and the points are calibrated with c1 / c2
+  double c1[3], c2[3];
+};
+
+// what a call returns per problem, one D2H copy for the whole sub-batch
+struct RsOut {
+  RsBest best;
+  int count, pad;
+  double pose[13];
+};
+struct RsScratch {
+  RsBest cand[RS_TOP];
+  double E[9];  // b2_recover_pose_host's input
+  double pose_cands[22];
+  int gvotes[8];
+};
+
 struct RansacState {
-  DevBuf x1, x2, models, nsol, cost, ninl, best, mask, pose;
+  DevBuf x1, x2, models, nsol, cost, ninl, small, mask, tab;
   HostBuf hbuf;
 };
 
@@ -35,22 +97,28 @@ void rs_destroy(b2_context* ctx) {
   ctx->rs = nullptr;
 }
 
-// best-model record kept on the device between batches (the header's b2_ransac_candidate, so traces copy it as is)
-using RsBest = b2_ransac_candidate;
+// Copies a problem's record to shared memory, where the register-bound kernels read its fields at the point of use (as they
+// would read kernel parameters) instead of holding them in registers from the first line on.
+__device__ __forceinline__ void rs_load_prob(RsProb* sp, const RsProb* __restrict__ gp) {
+  for (int i = threadIdx.x; i < (int)(sizeof(RsProb) / 8); i += blockDim.x)
+    reinterpret_cast<unsigned long long*>(sp)[i] = reinterpret_cast<const unsigned long long*>(gp)[i];
+  __syncthreads();
+}
 
 __device__ __forceinline__ double rs_err(int mode, const double* M, double a, double b, double c, double d) {
   return mode == 0 ? sampson_sq(M, a, b, c, d) : epiline_sq(M, a, b, c, d);
 }
 
 // ---- hypothesis generation -------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(64) k_rs_hyp_E(const double* __restrict__ x1, const double* __restrict__ x2, int k,
-                                                  unsigned long long seed, int sample0, int n_samples,
-                                                  double* __restrict__ models, int* __restrict__ nsol, const int* __restrict__ go) {
-  if (go && !*go) return;  // extension stage not needed (decided on the device by k_rs_select)
+__global__ void __launch_bounds__(64) k_rs_hyp_E(const RsProb* __restrict__ tab, unsigned long long seed) {
+  const RsProb& p = tab[blockIdx.y];
+  if (p.go && !*p.go) return;  // extension stage not needed (decided on the device by k_rs_select)
   int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= n_samples) return;
+  if (s >= p.n) return;
+  const double *__restrict__ x1 = p.x1, *__restrict__ x2 = p.x2;
+  double* __restrict__ models = p.models;
   int idx[5];
-  sample_distinct(seed, (unsigned long long)(sample0 + s), k, 5, idx);
+  sample_distinct(seed, (unsigned long long)(p.sample0 + s), p.k, 5, idx);
   double a[5][2], b[5][2];
   for (int i = 0; i < 5; ++i) {
     a[i][0] = x1[2 * idx[i]], a[i][1] = x1[2 * idx[i] + 1];
@@ -58,43 +126,47 @@ __global__ void __launch_bounds__(64) k_rs_hyp_E(const double* __restrict__ x1, 
   }
   double sol[RS_MAX_SOL][9];
   int n = fivept_solve(a, b, sol);
-  nsol[s] = n;
+  p.nsol[s] = n;
   for (int j = 0; j < n; ++j)
     for (int i = 0; i < 9; ++i) models[((size_t)s * RS_MAX_SOL + j) * 9 + i] = sol[j][i];
 }
 
 // normalised 8-point algorithm on one 8-sample (Hartley 1997): one F per sample
-__global__ void __launch_bounds__(64) k_rs_hyp_F(const double* __restrict__ x1, const double* __restrict__ x2, int k,
-                                                  unsigned long long seed, int sample0, int n_samples,
-                                                  double* __restrict__ models, int* __restrict__ nsol) {
+__global__ void __launch_bounds__(64) k_rs_hyp_F(const RsProb* __restrict__ tab, unsigned long long seed) {
+  const RsProb& p = tab[blockIdx.y];
   int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s >= n_samples) return;
+  if (s >= p.n) return;
+  const double *__restrict__ x1 = p.x1, *__restrict__ x2 = p.x2;
   int idx[8];
-  sample_distinct(seed, (unsigned long long)(sample0 + s), k, 8, idx);
+  sample_distinct(seed, (unsigned long long)(p.sample0 + s), p.k, 8, idx);
   double a[8][2], b[8][2];
   for (int i = 0; i < 8; ++i) {
     a[i][0] = x1[2 * idx[i]], a[i][1] = x1[2 * idx[i] + 1];
     b[i][0] = x2[2 * idx[i]], b[i][1] = x2[2 * idx[i] + 1];
   }
-  const int n = eightpt_solve(a, b, models + (size_t)s * RS_MAX_SOL * 9);
-  nsol[s] = n;
+  const int n = eightpt_solve(a, b, p.models + (size_t)s * RS_MAX_SOL * 9);
+  p.nsol[s] = n;
 }
 
-// ---- scoring: one CTA per model slot ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(RS_SCORE_THREADS) k_rs_score(const double* __restrict__ models, const int* __restrict__ nsol,
-                                                                const double* __restrict__ x1, const double* __restrict__ x2,
-                                                                int k, double thr2, int mode, double* __restrict__ cost,
-                                                                int* __restrict__ ninl, const int* __restrict__ go) {
-  if (go && !*go) return;
+// ---- scoring: one CTA per model slot (the grid spans the largest round of the table) ---------------------------------
+__global__ void __launch_bounds__(RS_SCORE_THREADS) k_rs_score(const RsProb* __restrict__ tab) {
+  const RsProb& p = tab[blockIdx.y];
+  if (p.go && !*p.go) return;
   const int slot = blockIdx.x, s = slot / RS_MAX_SOL, j = slot % RS_MAX_SOL;
-  if (j >= nsol[s]) {
+  if (s >= p.n) return;
+  const double *__restrict__ x1 = p.x1, *__restrict__ x2 = p.x2;
+  double* __restrict__ cost = p.cost;
+  int* __restrict__ ninl = p.ninl;
+  const int k = p.k, mode = p.mode;
+  const double thr2 = p.thr2;
+  if (j >= p.nsol[s]) {
     if (threadIdx.x == 0) cost[slot] = 1e300, ninl[slot] = 0;
     return;
   }
   __shared__ double M[9];
   __shared__ double wc[RS_SCORE_THREADS / 32];
   __shared__ int wn[RS_SCORE_THREADS / 32];
-  if (threadIdx.x < 9) M[threadIdx.x] = models[(size_t)slot * 9 + threadIdx.x];
+  if (threadIdx.x < 9) M[threadIdx.x] = p.models[(size_t)slot * 9 + threadIdx.x];
   __syncthreads();
   double c = 0;
   int n = 0;
@@ -124,11 +196,13 @@ __global__ void __launch_bounds__(RS_SCORE_THREADS) k_rs_score(const double* __r
 // cand[0 .. RS_TOP) is kept sorted by (cost, arrival); each round is one block arg-min over the slots that come after the
 // previous winner in (cost, index) order.  A contaminated sample (4 of 5 inliers) usually scores close to the best one and
 // converges to the right model under the local optimisation, which is what makes few hypotheses enough at 30 % inliers.
-__global__ void __launch_bounds__(1024) k_rs_select(const double* __restrict__ models, const double* __restrict__ cost,
-                                                     const int* __restrict__ ninl, int n_slots, RsBest* __restrict__ cand,
-                                                     const int* __restrict__ go, int* __restrict__ more, int k, int msize,
-                                                     double log_1mc, double done_after) {
-  if (go && !*go) return;
+__global__ void __launch_bounds__(1024) k_rs_select(const RsProb* __restrict__ tab, double log_1mc) {
+  const RsProb& p = tab[blockIdx.y];
+  if (p.go && !*p.go) return;
+  const double *__restrict__ models = p.models, *__restrict__ cost = p.cost;
+  const int* __restrict__ ninl = p.ninl;
+  RsBest* __restrict__ cand = p.cand;
+  const int n_slots = p.n * RS_MAX_SOL;
   __shared__ double sc[1024];
   __shared__ int si[1024];
   __shared__ RsBest merged[RS_TOP];
@@ -181,23 +255,26 @@ __global__ void __launch_bounds__(1024) k_rs_select(const double* __restrict__ m
     __syncthreads();
   }
   if (threadIdx.x < RS_TOP) cand[threadIdx.x] = merged[threadIdx.x];
-  if (threadIdx.x == 0 && more) {
+  if (threadIdx.x == 0 && p.more) {
     // standard RANSAC bound with the support of the best hypothesis so far: are `done_after` samples enough for the requested
-    // confidence?  If not, the (already enqueued) extension stage runs; otherwise its kernels return at once.
+    // confidence?  If not, the (already enqueued) extension stage runs, or the host enqueues the problem's next round;
+    // otherwise the extension's kernels return at once and the problem is left out of later rounds.
     int need_more = 1;
     if (merged[0].valid) {
-      const double w = (double)merged[0].ninl / (double)k;
-      const double pw = pow(w, (double)msize);
+      const double w = (double)merged[0].ninl / (double)p.k;
+      const double pw = pow(w, p.mode == 0 ? 5.0 : 8.0);
       const double need = pw >= 1.0 ? 1.0 : (pw <= 0.0 ? 1e300 : log_1mc / log(1.0 - pw));
-      need_more = need > done_after ? 1 : 0;
+      need_more = need > p.done_after ? 1 : 0;
     }
-    *more = need_more;
+    *p.more = need_more;
   }
 }
 
 // after the local optimisation: the refined candidate with the lowest cost (ties -> lower rank) becomes the result
-__global__ void k_rs_pick(const RsBest* __restrict__ cand, RsBest* __restrict__ best) {
+__global__ void k_rs_pick(const RsProb* __restrict__ tab) {
   if (threadIdx.x != 0) return;
+  const RsBest* __restrict__ cand = tab[blockIdx.y].cand;
+  RsBest* __restrict__ best = tab[blockIdx.y].best;
   int b = -1;
   for (int j = 0; j < RS_TOP; ++j)
     if (cand[j].valid && (b < 0 || cand[j].cost < cand[b].cost)) b = j;
@@ -276,9 +353,13 @@ __device__ void jacobi9_warp(double* A, double* V, int lane) {
   }
 }
 
-__global__ void __launch_bounds__(RS_LO_THREADS) k_rs_refine(const double* __restrict__ x1, const double* __restrict__ x2, int k,
-                                                              double thr2, int mode, RsBest* __restrict__ cands) {
-  RsBest* best = cands + blockIdx.x;  // one CTA per candidate
+__global__ void __launch_bounds__(RS_LO_THREADS) k_rs_refine(const RsProb* __restrict__ tab) {
+  __shared__ RsProb p;
+  rs_load_prob(&p, tab + blockIdx.y);
+  const double *__restrict__ x1 = p.x1, *__restrict__ x2 = p.x2;
+  const int k = p.k, mode = p.mode;
+  const double thr2 = p.thr2;
+  RsBest* best = p.cand + blockIdx.x;  // one CTA per candidate
   __shared__ double sh[RS_LO_THREADS / 32];
   __shared__ double M[9], cand[9];
   __shared__ double mom[45];
@@ -411,29 +492,48 @@ __global__ void __launch_bounds__(RS_LO_THREADS) k_rs_refine(const double* __res
   if (threadIdx.x < 9) best->model[threadIdx.x] = M[threadIdx.x];
 }
 
-__global__ void __launch_bounds__(256) k_rs_mask(const double* __restrict__ x1, const double* __restrict__ x2, int k, double thr2,
-                                                  int mode, const RsBest* __restrict__ best, uint8_t* __restrict__ mask,
-                                                  int* __restrict__ count) {
+__global__ void __launch_bounds__(256) k_rs_mask(const RsProb* __restrict__ tab) {
+  const RsProb& p = tab[blockIdx.y];
+  const double *__restrict__ x1 = p.x1, *__restrict__ x2 = p.x2;
+  const RsBest* __restrict__ best = p.best;
+  const int k = p.k;
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   bool in = false;
-  if (i < k && best->valid) in = rs_err(mode, best->model, x1[2 * i], x1[2 * i + 1], x2[2 * i], x2[2 * i + 1]) < thr2;
-  if (i < k) mask[i] = in ? 1 : 0;
+  if (i < k && best->valid) in = rs_err(p.mode, best->model, x1[2 * i], x1[2 * i + 1], x2[2 * i], x2[2 * i + 1]) < p.thr2;
+  if (i < k) p.mask[i] = in ? 1 : 0;
   unsigned m = __ballot_sync(0xffffffffu, in);
-  if ((threadIdx.x & 31) == 0 && m) atomicAdd(count, __popc(m));
+  if ((threadIdx.x & 31) == 0 && m) atomicAdd(p.count, __popc(m));
 }
 
 // ---- pose recovery (cv2.recoverPose semantics): one correspondence per thread, integer votes, last CTA decides ------
 constexpr int RS_POSE_THREADS = 128;
-__global__ void __launch_bounds__(RS_POSE_THREADS) k_rs_pose(const double* __restrict__ E, const double* __restrict__ x1,
-                                                              const double* __restrict__ x2, const uint8_t* __restrict__ mask, int k,
-                                                              int* __restrict__ gvotes /*[4] votes + [1] CTA counter, zero on entry*/,
-                                                              double* __restrict__ out /*R[9], t[3], good*/,
-                                                              double* __restrict__ cands /*R1[9], R2[9], t[3], winner; tests only*/) {
+// The grid spans the largest problem of the table; a CTA past its problem's points casts no vote but is still counted, so
+// "last" means the same for every problem.  A fundamental-matrix problem (pose_cal) first forms E = K2^T F K1 and calibrates
+// its pixel coordinates with each side's (f, u0, v0), which is gtsfm/utils/verification.py:54-112.
+__global__ void __launch_bounds__(RS_POSE_THREADS) k_rs_pose(const RsProb* __restrict__ tab) {
+  __shared__ RsProb p;
+  rs_load_prob(&p, tab + blockIdx.y);
+  if (!p.pose_on) return;
+  const double *__restrict__ x1 = p.x1, *__restrict__ x2 = p.x2;
+  const uint8_t* __restrict__ mask = p.pose_mask;
+  int* __restrict__ gvotes = p.gvotes;
+  double *__restrict__ out = p.pose, *__restrict__ cands = p.pose_cands;
+  const int k = p.k;
   __shared__ double R1[9], R2[9], t[3];
   __shared__ int votes[4];
   __shared__ int is_last;
   if (threadIdx.x == 0) {
-    decompose_E(E, R1, R2, t);
+    if (p.pose_cal) {
+      const double K2t[9] = {p.c2[0], 0, 0, 0, p.c2[0], 0, p.c2[1], p.c2[2], 1};
+      const double K1[9] = {p.c1[0], 0, p.c1[1], 0, p.c1[0], p.c1[2], 0, 0, 1};
+      double F[9], tmp[9], Em[9];
+      for (int j = 0; j < 9; ++j) F[j] = p.E[j];
+      mat3_mul(K2t, F, tmp);
+      mat3_mul(tmp, K1, Em);
+      decompose_E(Em, R1, R2, t);
+    } else {
+      decompose_E(p.E, R1, R2, t);
+    }
     votes[0] = votes[1] = votes[2] = votes[3] = 0;
   }
   __syncthreads();
@@ -441,10 +541,15 @@ __global__ void __launch_bounds__(RS_POSE_THREADS) k_rs_pose(const double* __res
   const int i = blockIdx.x * RS_POSE_THREADS + threadIdx.x;
   if (i < k && (!mask || mask[i])) {
     const double tn[3] = {-t[0], -t[1], -t[2]};
-    v[0] = cheirality_ok(R1, t, x1[2 * i], x1[2 * i + 1], x2[2 * i], x2[2 * i + 1], 50.0);
-    v[1] = cheirality_ok(R2, t, x1[2 * i], x1[2 * i + 1], x2[2 * i], x2[2 * i + 1], 50.0);
-    v[2] = cheirality_ok(R1, tn, x1[2 * i], x1[2 * i + 1], x2[2 * i], x2[2 * i + 1], 50.0);
-    v[3] = cheirality_ok(R2, tn, x1[2 * i], x1[2 * i + 1], x2[2 * i], x2[2 * i + 1], 50.0);
+    double ax = x1[2 * i], ay = x1[2 * i + 1], bx = x2[2 * i], by = x2[2 * i + 1];
+    if (p.pose_cal) {
+      ax = (ax - p.c1[1]) / p.c1[0], ay = (ay - p.c1[2]) / p.c1[0];
+      bx = (bx - p.c2[1]) / p.c2[0], by = (by - p.c2[2]) / p.c2[0];
+    }
+    v[0] = cheirality_ok(R1, t, ax, ay, bx, by, 50.0);
+    v[1] = cheirality_ok(R2, t, ax, ay, bx, by, 50.0);
+    v[2] = cheirality_ok(R1, tn, ax, ay, bx, by, 50.0);
+    v[3] = cheirality_ok(R2, tn, ax, ay, bx, by, 50.0);
   }
   for (int c = 0; c < 4; ++c) {
     int s = v[c];
@@ -486,179 +591,336 @@ __global__ void __launch_bounds__(RS_POSE_THREADS) k_rs_pose(const double* __res
 
 // gather matched keypoints and calibrate them with a distortion-free pinhole model (utils/features.py:41-51 for
 // Cal3Bundler with k1 = k2 = 0): x = (u - u0) / f, in double.  f = 1, u0 = v0 = 0 leaves pixels (F path).
-__global__ void __launch_bounds__(256) k_rs_gather(const float* __restrict__ kp1, const float* __restrict__ kp2,
-                                                    const long long* __restrict__ matches, int k, double f1, double u1,
-                                                    double v1, double f2, double u2, double v2, double* __restrict__ x1,
-                                                    double* __restrict__ x2) {
+__global__ void __launch_bounds__(256) k_rs_gather(const RsProb* __restrict__ tab) {
+  const RsProb& p = tab[blockIdx.y];
   int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= k) return;
-  long long a = matches[2 * i], b = matches[2 * i + 1];
+  if (!p.kp1 || i >= p.k) return;
+  const float *__restrict__ kp1 = p.kp1, *__restrict__ kp2 = p.kp2;
+  double *__restrict__ x1 = p.x1, *__restrict__ x2 = p.x2;
+  const double f1 = p.g1[0], u1 = p.g1[1], v1 = p.g1[2], f2 = p.g2[0], u2 = p.g2[1], v2 = p.g2[2];
+  long long a = p.matches[2 * i], b = p.matches[2 * i + 1];
   x1[2 * i] = ((double)kp1[2 * a] - u1) / f1;
   x1[2 * i + 1] = ((double)kp1[2 * a + 1] - v1) / f1;
   x2[2 * i] = ((double)kp2[2 * b] - u2) / f2;
   x2[2 * i + 1] = ((double)kp2[2 * b + 1] - v2) / f2;
 }
 
-// x1 / x2 come either from host arrays (hx != null: uploaded here) or are already in s->x1 / s->x2 (device path).
-// out_mask: host pointer when mask_is_device == 0, device pointer otherwise.  tr (tests only, nullptr in production) sets
-// the batch size and receives the intermediate state; it adds copies and synchronisations but no launches.
-static int rs_run(b2_context* ctx, const double* hx1, const double* hx2, int k, const b2_ransac_params* prm, int mode,
-                  double* out_model, uint8_t* out_mask, int* out_ninl, double* out_R, double* out_t,
-                  cudaStream_t st = nullptr, int mask_is_device = 0, b2_ransac_trace* tr = nullptr) {
-  if (!ctx->rs) ctx->rs = new RansacState();
-  RansacState* s = ctx->rs;
-  if (!st) st = ctx->stream;
-  const int m = mode == 0 ? 5 : 8;
-  if (tr) tr->batches = 0, tr->ext_go = -1, tr->records = 0;
-  *out_ninl = 0;
-  if (out_mask && !mask_is_device) memset(out_mask, 0, (size_t)k);
-  if (out_mask && mask_is_device && k > 0) B2_CUDA(ctx, cudaMemsetAsync(out_mask, 0, (size_t)k, st));
-  if (k < m) return 1;
+// One problem as the host entry points describe it.  Points come from host arrays (hx: uploaded here), from device arrays
+// (dx: used where they are) or from keypoints + match rows (k_rs_gather); the mask goes to a device buffer (dmask), to a
+// host one (hmask) or nowhere.
+struct RsJob {
+  const float *kp1 = nullptr, *kp2 = nullptr;
+  const int64_t* matches = nullptr;
+  const double *dx1 = nullptr, *dx2 = nullptr, *hx1 = nullptr, *hx2 = nullptr;
+  int k = 0, mode = 0, max_iters = 0;
+  double threshold = 0;
+  double cal1[3] = {1, 0, 0}, cal2[3] = {1, 0, 0};
+  uint8_t *dmask = nullptr, *hmask = nullptr;
+  bool pose = false;
+};
+
+static int rs_clamp_iters(int mode, int max_iters) {
   const int hard_cap = mode == 0 ? 65536 : 262144;
-  const int max_iters = prm->max_iters < 1 ? 1 : (prm->max_iters > hard_cap ? hard_cap : prm->max_iters);
-  const int batch = tr ? tr->batch : RS_BATCH;
-  const double thr2 = prm->threshold * prm->threshold;
-  B2_CUDA(ctx, s->x1.ensure((size_t)k * 16));
-  B2_CUDA(ctx, s->x2.ensure((size_t)k * 16));
-  B2_CUDA(ctx, s->models.ensure((size_t)RS_BATCH * RS_MAX_SOL * 9 * 8));
-  B2_CUDA(ctx, s->nsol.ensure((size_t)RS_BATCH * 4));
-  B2_CUDA(ctx, s->cost.ensure((size_t)RS_BATCH * RS_MAX_SOL * 8));
-  B2_CUDA(ctx, s->ninl.ensure((size_t)RS_BATCH * RS_MAX_SOL * 4));
-  B2_CUDA(ctx, s->best.ensure(sizeof(RsBest) * (1 + RS_TOP) + 16));  // [0] result, then the counter, then the RS_TOP candidates
-  B2_CUDA(ctx, s->mask.ensure((size_t)k + 16));
-  // [0,13) R, t, votes of the winner | [16,25) E (recover_pose) | [32,36) int votes[4] + counter | [36,58) R1, R2, t, winner
-  B2_CUDA(ctx, s->pose.ensure(64 * 8));
-  B2_CUDA(ctx, s->hbuf.ensure(sizeof(RsBest) + 16 * 8 + 64));
-  if (hx1) {
-    B2_CUDA(ctx, cudaMemcpyAsync(s->x1.p, hx1, (size_t)k * 16, cudaMemcpyHostToDevice, st));
-    B2_CUDA(ctx, cudaMemcpyAsync(s->x2.p, hx2, (size_t)k * 16, cudaMemcpyHostToDevice, st));
+  return max_iters < 1 ? 1 : (max_iters > hard_cap ? hard_cap : max_iters);
+}
+// samples the largest round of a problem draws: a sampling batch, or the E extension stage
+static int rs_round_cap(int mode, int max_iters, int batch) {
+  const int mi = rs_clamp_iters(mode, max_iters);
+  const int main_n = mi < batch ? mi : batch;
+  const int ext_n = (mode == 0 && mi <= 4096) ? (4 * mi < batch ? 4 * mi : batch) : 0;
+  return main_n > ext_n ? main_n : ext_n;
+}
+constexpr size_t RS_SAMPLE_BYTES = RS_MAX_SOL * (72 + 8 + 4) + 4;  // models, cost, ninl of ten slots and nsol
+constexpr size_t RS_FIXED_BYTES = sizeof(RsOut) + sizeof(RsScratch) + 4 + 3 * sizeof(RsProb);
+// workspace bytes of one problem: its sample slices, its points and mask unless the caller's device arrays are used
+static size_t rs_job_bytes(int k, int mode, int max_iters, bool own_x, bool own_mask, int batch = RS_BATCH) {
+  if (k < (mode == 0 ? 5 : 8)) return RS_FIXED_BYTES;
+  return RS_FIXED_BYTES + (size_t)rs_round_cap(mode, max_iters, batch) * RS_SAMPLE_BYTES + (own_x ? (size_t)k * 32 : 0) +
+         (own_mask ? (size_t)k : 0);
+}
+// Consecutive sub-batches under `budget` bytes: first[i] is the first problem of sub-batch i, first[count] = n.  A
+// problem larger than the budget gets a sub-batch of its own.
+static int rs_plan(const size_t* bytes, int n, size_t budget, int* first) {
+  int count = 0;
+  size_t used = 0;
+  for (int i = 0; i < n; ++i) {
+    if (i == 0 || used + bytes[i] > budget) first[count++] = i, used = 0;
+    used += bytes[i];
   }
-  B2_CUDA(ctx, cudaMemsetAsync(s->best.p, 0, sizeof(RsBest) * (1 + RS_TOP) + 16, st));
-  RsBest* dbest = s->best.as<RsBest>();
-  int* dcount = reinterpret_cast<int*>(s->best.as<char>() + sizeof(RsBest));
-  RsBest* dcand = reinterpret_cast<RsBest*>(s->best.as<char>() + sizeof(RsBest) + 16);
-  RsBest* hbest = s->hbuf.as<RsBest>();
-  const double *x1 = s->x1.as<double>(), *x2 = s->x2.as<double>();
+  first[count] = n;
+  return count;
+}
+
+#define RS_SYNC(ctx, st)                            \
+  do {                                              \
+    B2_CUDA(ctx, cudaStreamSynchronize(st));        \
+    (ctx)->rs_syncs++;                              \
+  } while (0)
+
+// One sub-batch: every stage launched once for all its problems.  tr (tests only, nullptr in production, one problem) sets
+// the round size and receives the intermediate state; it adds copies and synchronisations but no launches.
+static int rs_run_sub(b2_context* ctx, const RsJob* jobs, int n, double confidence, uint64_t seed, b2_ransac_result* res,
+                      cudaStream_t st, b2_ransac_trace* tr) {
+  RansacState* s = ctx->rs;
+  const int batch = tr ? tr->batch : RS_BATCH;
+  if (tr) tr->batches = 0, tr->ext_go = -1, tr->records = 0;
+  // live problems, essential ones first (the two hypothesis kernels each take a contiguous part of the table)
+  std::vector<int> live;
+  for (int mode = 0; mode < 2; ++mode)
+    for (int i = 0; i < n; ++i)
+      if (jobs[i].mode == mode && jobs[i].k >= (mode == 0 ? 5 : 8)) live.push_back(i);
+  for (int i = 0; i < n; ++i) {
+    memset(&res[i], 0, sizeof(res[i]));
+    res[i].status = 1;
+    const RsJob& j = jobs[i];
+    if (j.k >= (j.mode == 0 ? 5 : 8) || j.k == 0) continue;
+    if (j.hmask) memset(j.hmask, 0, (size_t)j.k);
+    if (j.dmask) B2_CUDA(ctx, cudaMemsetAsync(j.dmask, 0, (size_t)j.k, st));
+  }
+  const int L = (int)live.size();
+  if (L == 0) return B2_OK;
+
+  size_t n_smp = 0, n_x = 0, n_mask = 0;
+  for (int i : live) {
+    const RsJob& j = jobs[i];
+    n_smp += (size_t)rs_round_cap(j.mode, j.max_iters, batch);
+    if (!j.dx1) n_x += (size_t)j.k;
+    if (!j.dmask) n_mask += (size_t)j.k;
+  }
+  const size_t small_bytes = (size_t)L * (sizeof(RsOut) + sizeof(RsScratch) + 4);
+  B2_CUDA(ctx, s->x1.ensure(n_x * 16 + 16));
+  B2_CUDA(ctx, s->x2.ensure(n_x * 16 + 16));
+  B2_CUDA(ctx, s->models.ensure(n_smp * RS_MAX_SOL * 72));
+  B2_CUDA(ctx, s->nsol.ensure(n_smp * 4));
+  B2_CUDA(ctx, s->cost.ensure(n_smp * RS_MAX_SOL * 8));
+  B2_CUDA(ctx, s->ninl.ensure(n_smp * RS_MAX_SOL * 4));
+  B2_CUDA(ctx, s->mask.ensure(n_mask + 16));
+  B2_CUDA(ctx, s->small.ensure(small_bytes));
+  B2_CUDA(ctx, s->tab.ensure(3 * (size_t)L * sizeof(RsProb)));
+  // pinned: three tables (all problems | this round | the extension round), the results, the flags
+  B2_CUDA(ctx, s->hbuf.ensure((size_t)L * (3 * sizeof(RsProb) + sizeof(RsOut) + 4)));
+  RsProb* htab = s->hbuf.as<RsProb>();
+  RsOut* hout = reinterpret_cast<RsOut*>(htab + 3 * (size_t)L);
+  int* hflags = reinterpret_cast<int*>(hout + L);
+  RsProb* dtab = s->tab.as<RsProb>();
+  RsOut* dout = s->small.as<RsOut>();
+  RsScratch* dscr = reinterpret_cast<RsScratch*>(dout + L);
+  int* dflags = reinterpret_cast<int*>(dscr + L);
+  B2_CUDA(ctx, cudaMemsetAsync(s->small.p, 0, small_bytes, st));
+
+  int max_k = 0;
+  bool any_gather = false, any_pose = false;
+  {
+    size_t o_smp = 0, o_x = 0, o_mask = 0;
+    for (int t = 0; t < L; ++t) {
+      const RsJob& j = jobs[live[t]];
+      RsProb& p = htab[t];
+      memset(&p, 0, sizeof(p));
+      p.k = j.k, p.mode = j.mode, p.thr2 = j.threshold * j.threshold;
+      if (j.dx1) {
+        p.x1 = const_cast<double*>(j.dx1), p.x2 = const_cast<double*>(j.dx2);
+      } else {
+        p.x1 = s->x1.as<double>() + 2 * o_x, p.x2 = s->x2.as<double>() + 2 * o_x;
+        o_x += (size_t)j.k;
+        if (j.hx1) {
+          B2_CUDA(ctx, cudaMemcpyAsync(p.x1, j.hx1, (size_t)j.k * 16, cudaMemcpyHostToDevice, st));
+          B2_CUDA(ctx, cudaMemcpyAsync(p.x2, j.hx2, (size_t)j.k * 16, cudaMemcpyHostToDevice, st));
+        } else {
+          p.kp1 = j.kp1, p.kp2 = j.kp2, p.matches = reinterpret_cast<const long long*>(j.matches);
+          // a fundamental-matrix problem keeps pixels: f = 1, u0 = v0 = 0
+          for (int c = 0; c < 3; ++c) p.g1[c] = j.mode == 0 ? j.cal1[c] : (c == 0), p.g2[c] = j.mode == 0 ? j.cal2[c] : (c == 0);
+          any_gather = true;
+        }
+      }
+      p.models = s->models.as<double>() + o_smp * RS_MAX_SOL * 9, p.nsol = s->nsol.as<int>() + o_smp;
+      p.cost = s->cost.as<double>() + o_smp * RS_MAX_SOL, p.ninl = s->ninl.as<int>() + o_smp * RS_MAX_SOL;
+      o_smp += (size_t)rs_round_cap(j.mode, j.max_iters, batch);
+      p.cand = dscr[t].cand, p.best = &dout[t].best, p.count = &dout[t].count;
+      if (j.dmask) p.mask = j.dmask;
+      else p.mask = s->mask.as<uint8_t>() + o_mask, o_mask += (size_t)j.k;
+      p.E = dout[t].best.model, p.pose_mask = p.mask, p.gvotes = dscr[t].gvotes, p.pose = dout[t].pose;
+      p.pose_cands = tr ? dscr[t].pose_cands : nullptr;
+      p.pose_on = j.pose, p.pose_cal = j.pose && j.mode == 1;
+      for (int c = 0; c < 3; ++c) p.c1[c] = j.cal1[c], p.c2[c] = j.cal2[c];
+      max_k = j.k > max_k ? j.k : max_k;
+      any_pose |= j.pose;
+    }
+  }
+  B2_CUDA(ctx, cudaMemcpyAsync(dtab, htab, (size_t)L * sizeof(RsProb), cudaMemcpyHostToDevice, st));
+  if (any_gather) {
+    B2_LAUNCH(ctx, k_rs_gather, dim3(cdiv(max_k, 256), L), 256, 0, st, dtab);
+    B2_CHECK_LAUNCH(ctx);
+  }
+
+  const double log_1mc = log(1.0 - confidence);
+  // one sampling round over rows [0, R) of table `slot` (rows are sorted essential first): hypotheses, scores, selection
+  auto round = [&](int slot, int R) -> int {
+    RsProb* h = htab + (size_t)slot * L;
+    RsProb* d = dtab + (size_t)slot * L;
+    int nE = 0, maxnE = 0, maxnF = 0;
+    for (int r = 0; r < R; ++r) {
+      if (h[r].mode == 0) ++nE, maxnE = h[r].n > maxnE ? h[r].n : maxnE;
+      else maxnF = h[r].n > maxnF ? h[r].n : maxnF;
+    }
+    B2_CUDA(ctx, cudaMemcpyAsync(d, h, (size_t)R * sizeof(RsProb), cudaMemcpyHostToDevice, st));
+    if (nE) B2_LAUNCH(ctx, k_rs_hyp_E, dim3(cdiv(maxnE, 64), nE), 64, 0, st, d, (unsigned long long)seed);
+    if (R - nE) B2_LAUNCH(ctx, k_rs_hyp_F, dim3(cdiv(maxnF, 64), R - nE), 64, 0, st, d + nE, (unsigned long long)seed);
+    B2_CHECK_LAUNCH(ctx);
+    B2_LAUNCH(ctx, k_rs_score, dim3((maxnE > maxnF ? maxnE : maxnF) * RS_MAX_SOL, R), RS_SCORE_THREADS, 0, st, d);
+    B2_CHECK_LAUNCH(ctx);
+    B2_LAUNCH(ctx, k_rs_select, dim3(1, R), 1024, 0, st, d, log_1mc);
+    B2_CHECK_LAUNCH(ctx);
+    return B2_OK;
+  };
   // trace record of one k_rs_select launch over n samples (more_written: it wrote the confidence flag)
-  auto record = [&](int n, bool more_written) -> int {
+  auto record = [&](int ns_run, bool more_written) -> int {
     if (tr->records >= tr->max_records) return B2_OK;
     const int r = tr->records++;
     const size_t ns = (size_t)tr->batch;
     const auto d2h = cudaMemcpyDeviceToHost;
-    if (tr->nsol) B2_CUDA(ctx, cudaMemcpyAsync(tr->nsol + r * ns, s->nsol.p, (size_t)n * 4, d2h, st));
+    if (tr->nsol) B2_CUDA(ctx, cudaMemcpyAsync(tr->nsol + r * ns, s->nsol.p, (size_t)ns_run * 4, d2h, st));
     if (tr->models)
-      B2_CUDA(ctx, cudaMemcpyAsync(tr->models + r * ns * RS_MAX_SOL * 9, s->models.p, (size_t)n * RS_MAX_SOL * 72, d2h, st));
-    if (tr->cost) B2_CUDA(ctx, cudaMemcpyAsync(tr->cost + r * ns * RS_MAX_SOL, s->cost.p, (size_t)n * RS_MAX_SOL * 8, d2h, st));
-    if (tr->ninl) B2_CUDA(ctx, cudaMemcpyAsync(tr->ninl + r * ns * RS_MAX_SOL, s->ninl.p, (size_t)n * RS_MAX_SOL * 4, d2h, st));
-    if (tr->selected) B2_CUDA(ctx, cudaMemcpyAsync(tr->selected + (size_t)r * RS_TOP, dcand, sizeof(RsBest) * RS_TOP, d2h, st));
+      B2_CUDA(ctx, cudaMemcpyAsync(tr->models + r * ns * RS_MAX_SOL * 9, s->models.p, (size_t)ns_run * RS_MAX_SOL * 72, d2h, st));
+    if (tr->cost) B2_CUDA(ctx, cudaMemcpyAsync(tr->cost + r * ns * RS_MAX_SOL, s->cost.p, (size_t)ns_run * RS_MAX_SOL * 8, d2h, st));
+    if (tr->ninl) B2_CUDA(ctx, cudaMemcpyAsync(tr->ninl + r * ns * RS_MAX_SOL, s->ninl.p, (size_t)ns_run * RS_MAX_SOL * 4, d2h, st));
+    if (tr->selected) B2_CUDA(ctx, cudaMemcpyAsync(tr->selected + (size_t)r * RS_TOP, dscr[0].cand, sizeof(RsBest) * RS_TOP, d2h, st));
     if (tr->more) {
-      if (more_written) B2_CUDA(ctx, cudaMemcpyAsync(tr->more + r, dcount + 1, 4, d2h, st));
+      if (more_written) B2_CUDA(ctx, cudaMemcpyAsync(tr->more + r, dflags, 4, d2h, st));
       else tr->more[r] = -1;
     }
-    B2_CUDA(ctx, cudaStreamSynchronize(st));
+    RS_SYNC(ctx, st);
     return B2_OK;
   };
-  int done = 0;
-  while (done < max_iters) {
-    const int n = (max_iters - done) < batch ? (max_iters - done) : batch;
-    if (mode == 0)
-      B2_LAUNCH(ctx, k_rs_hyp_E, cdiv(n, 64), 64, 0, st, x1, x2, k, (unsigned long long)prm->seed, done, n,
-                s->models.as<double>(), s->nsol.as<int>(), (const int*)nullptr);
-    else
-      B2_LAUNCH(ctx, k_rs_hyp_F, cdiv(n, 64), 64, 0, st, x1, x2, k, (unsigned long long)prm->seed, done, n,
-                s->models.as<double>(), s->nsol.as<int>());
-    B2_CHECK_LAUNCH(ctx);
-    B2_LAUNCH(ctx, k_rs_score, n * RS_MAX_SOL, RS_SCORE_THREADS, 0, st, s->models.as<double>(), s->nsol.as<int>(), x1, x2, k,
-              thr2, mode, s->cost.as<double>(), s->ninl.as<int>(), (const int*)nullptr);
-    B2_CHECK_LAUNCH(ctx);
-    B2_LAUNCH(ctx, k_rs_select, 1, 1024, 0, st, s->models.as<double>(), s->cost.as<double>(), s->ninl.as<int>(),
-              n * RS_MAX_SOL, dcand, (const int*)nullptr, dcount + 1, k, m, log(1.0 - prm->confidence), (double)(done + n));
-    B2_CHECK_LAUNCH(ctx);
+
+  // Sampling.  `run` holds the table rows that still draw samples; a row leaves it when its budget is spent or its flag says
+  // the confidence bound is met.  A problem whose budget ends in a round gets its extension stage (E only: cv2's budget of
+  // `max_iters` samples leaves a 30 %-inlier pair without a single uncontaminated 5-sample one time in eleven; USAC survives
+  // that through its graph-cut local optimisation, a plain RANSAC does not.  The hypothesis kernel is latency-bound, so 4x more
+  // samples cost about as much as the first batch) enqueued right behind that round, gated on the device by the flag the
+  // round's k_rs_select wrote, so an E batch at the default budget never waits for the host.
+  std::vector<int> run(L), done(L, 0), iters(L);
+  for (int t = 0; t < L; ++t) run[t] = t, iters[t] = rs_clamp_iters(jobs[live[t]].mode, jobs[live[t]].max_iters);
+  while (!run.empty()) {
+    RsProb* h = htab + L;
+    for (size_t r = 0; r < run.size(); ++r) {
+      const int t = run[r];
+      h[r] = htab[t];
+      h[r].sample0 = done[t];
+      h[r].n = iters[t] - done[t] < batch ? iters[t] - done[t] : batch;
+      h[r].go = nullptr, h[r].more = dflags + t, h[r].done_after = (double)(done[t] + h[r].n);
+    }
+    if (int rc = round(1, (int)run.size())) return rc;
     if (tr) {
       ++tr->batches;
-      if (int rc = record(n, true)) return rc;
+      if (int rc = record(h[0].n, true)) return rc;
     }
-    done += n;
-    if (done >= max_iters) break;
-    // adaptive termination (standard RANSAC bound) between batches
-    B2_CUDA(ctx, cudaMemcpyAsync(hbest, dcand, sizeof(RsBest), cudaMemcpyDeviceToHost, st));  // the best unrefined candidate
-    B2_CUDA(ctx, cudaStreamSynchronize(st));
-    if (hbest->valid) {
-      double w = (double)hbest->ninl / k, pw = pow(w, m);
-      double need = pw >= 1.0 ? 1.0 : (pw <= 0 ? 1e300 : log(1.0 - prm->confidence) / log(1.0 - pw));
-      if ((double)done >= need) break;
+    std::vector<int> next;
+    RsProb* hx = htab + 2 * (size_t)L;
+    int n_ext = 0;
+    for (size_t r = 0; r < run.size(); ++r) {
+      const int t = run[r];
+      done[t] += h[r].n;
+      if (done[t] < iters[t]) {
+        next.push_back(t);
+      } else if (h[r].mode == 0 && iters[t] <= 4096) {
+        RsProb& e = hx[n_ext++] = htab[t];
+        e.sample0 = done[t];
+        e.n = 4 * iters[t] < batch ? 4 * iters[t] : batch;
+        e.go = dflags + t, e.more = nullptr, e.done_after = 0.0;
+      }
     }
-  }
-  if (mode == 0 && done >= max_iters && max_iters <= 4096) {
-    // Extension stage (E only): cv2's budget of `max_iters` samples leaves a 30 %-inlier pair without a single uncontaminated
-    // 5-sample one time in eleven; USAC survives that through its graph-cut local optimisation, a plain RANSAC does not.  The
-    // hypothesis kernel is latency-bound, so 4x more samples cost about as much as the first batch; they only run when the
-    // confidence bound of the best model so far says `max_iters` were not enough (flag written by k_rs_select on the device).
-    const int n2 = 4 * max_iters < batch ? 4 * max_iters : batch;
-    const int* go = dcount + 1;
-    B2_LAUNCH(ctx, k_rs_hyp_E, cdiv(n2, 64), 64, 0, st, x1, x2, k, (unsigned long long)prm->seed, done, n2, s->models.as<double>(),
-              s->nsol.as<int>(), go);
-    B2_CHECK_LAUNCH(ctx);
-    B2_LAUNCH(ctx, k_rs_score, n2 * RS_MAX_SOL, RS_SCORE_THREADS, 0, st, s->models.as<double>(), s->nsol.as<int>(), x1, x2, k, thr2, mode,
-              s->cost.as<double>(), s->ninl.as<int>(), go);
-    B2_CHECK_LAUNCH(ctx);
-    B2_LAUNCH(ctx, k_rs_select, 1, 1024, 0, st, s->models.as<double>(), s->cost.as<double>(), s->ninl.as<int>(), n2 * RS_MAX_SOL, dcand, go,
-              (int*)nullptr, k, m, 0.0, 0.0);
-    B2_CHECK_LAUNCH(ctx);
-    if (tr) {  // the extension's buffers are only worth recording when its kernels ran
-      B2_CUDA(ctx, cudaMemcpyAsync(&tr->ext_go, go, 4, cudaMemcpyDeviceToHost, st));
-      B2_CUDA(ctx, cudaStreamSynchronize(st));
-      if (tr->ext_go)
-        if (int rc = record(n2, false)) return rc;
+    if (n_ext) {
+      if (int rc = round(2, n_ext)) return rc;
+      if (tr) {  // the extension's buffers are only worth recording when its kernels ran
+        B2_CUDA(ctx, cudaMemcpyAsync(&tr->ext_go, dflags, 4, cudaMemcpyDeviceToHost, st));
+        RS_SYNC(ctx, st);
+        if (tr->ext_go)
+          if (int rc = record(hx[0].n, false)) return rc;
+      }
+    }
+    run.clear();
+    if (!next.empty()) {  // adaptive termination (standard RANSAC bound) between rounds: one read for the whole sub-batch
+      B2_CUDA(ctx, cudaMemcpyAsync(hflags, dflags, (size_t)L * 4, cudaMemcpyDeviceToHost, st));
+      RS_SYNC(ctx, st);
+      for (int t : next)
+        if (hflags[t]) run.push_back(t);
     }
   }
-  if (tr) B2_CUDA(ctx, cudaMemcpyAsync(tr->prerefine, dcand, sizeof(RsBest) * RS_TOP, cudaMemcpyDeviceToHost, st));
-  B2_LAUNCH(ctx, k_rs_refine, RS_TOP, RS_LO_THREADS, 0, st, x1, x2, k, thr2, mode, dcand);
+
+  if (tr) B2_CUDA(ctx, cudaMemcpyAsync(tr->prerefine, dscr[0].cand, sizeof(RsBest) * RS_TOP, cudaMemcpyDeviceToHost, st));
+  B2_LAUNCH(ctx, k_rs_refine, dim3(RS_TOP, L), RS_LO_THREADS, 0, st, dtab);
   B2_CHECK_LAUNCH(ctx);
-  if (tr) B2_CUDA(ctx, cudaMemcpyAsync(tr->refined, dcand, sizeof(RsBest) * RS_TOP, cudaMemcpyDeviceToHost, st));
-  B2_LAUNCH(ctx, k_rs_pick, 1, 32, 0, st, dcand, dbest);
+  if (tr) B2_CUDA(ctx, cudaMemcpyAsync(tr->refined, dscr[0].cand, sizeof(RsBest) * RS_TOP, cudaMemcpyDeviceToHost, st));
+  B2_LAUNCH(ctx, k_rs_pick, dim3(1, L), 32, 0, st, dtab);
   B2_CHECK_LAUNCH(ctx);
-  B2_LAUNCH(ctx, k_rs_mask, cdiv(k, 256), 256, 0, st, x1, x2, k, thr2, mode, dbest, s->mask.as<uint8_t>(), dcount);
+  B2_LAUNCH(ctx, k_rs_mask, dim3(cdiv(max_k, 256), L), 256, 0, st, dtab);
   B2_CHECK_LAUNCH(ctx);
-  const bool want_pose = mode == 0 && out_R && out_t;
-  int* gvotes = reinterpret_cast<int*>(s->pose.as<double>() + 32);
-  double* pose_cands = tr ? s->pose.as<double>() + 36 : nullptr;
-  if (want_pose) {
-    B2_CUDA(ctx, cudaMemsetAsync(gvotes, 0, 8 * sizeof(int), st));
-    B2_LAUNCH(ctx, k_rs_pose, cdiv(k, RS_POSE_THREADS), RS_POSE_THREADS, 0, st, dbest->model, x1, x2, s->mask.as<uint8_t>(), k, gvotes,
-              s->pose.as<double>(), pose_cands);
+  if (any_pose) {
+    B2_LAUNCH(ctx, k_rs_pose, dim3(cdiv(max_k, RS_POSE_THREADS), L), RS_POSE_THREADS, 0, st, dtab);
     B2_CHECK_LAUNCH(ctx);
   }
   if (tr) {
-    B2_CUDA(ctx, cudaMemcpyAsync(&tr->pick, dbest, sizeof(RsBest), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(ctx, cudaMemcpyAsync(&tr->mask_count, dcount, 4, cudaMemcpyDeviceToHost, st));
-    if (want_pose) {
+    B2_CUDA(ctx, cudaMemcpyAsync(&tr->pick, &dout[0].best, sizeof(RsBest), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(ctx, cudaMemcpyAsync(&tr->mask_count, &dout[0].count, 4, cudaMemcpyDeviceToHost, st));
+    if (any_pose) {
       double c[22];
-      B2_CUDA(ctx, cudaMemcpyAsync(tr->votes, gvotes, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
-      B2_CUDA(ctx, cudaMemcpyAsync(c, pose_cands, sizeof(c), cudaMemcpyDeviceToHost, st));
-      B2_CUDA(ctx, cudaStreamSynchronize(st));
+      B2_CUDA(ctx, cudaMemcpyAsync(tr->votes, dscr[0].gvotes, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
+      B2_CUDA(ctx, cudaMemcpyAsync(c, dscr[0].pose_cands, sizeof(c), cudaMemcpyDeviceToHost, st));
+      RS_SYNC(ctx, st);
       memcpy(tr->pose_cands, c, 21 * 8);
       tr->winner = (int)c[21];
     }
   }
-  char* hb = s->hbuf.as<char>();
-  B2_CUDA(ctx, cudaMemcpyAsync(hb, dbest, sizeof(RsBest) + 16, cudaMemcpyDeviceToHost, st));
-  if (want_pose) B2_CUDA(ctx, cudaMemcpyAsync(hb + sizeof(RsBest) + 16, s->pose.p, 13 * 8, cudaMemcpyDeviceToHost, st));
-  if (out_mask)
-    B2_CUDA(ctx, cudaMemcpyAsync(out_mask, s->mask.p, (size_t)k, mask_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-  B2_CUDA(ctx, cudaStreamSynchronize(st));
-  if (!hbest->valid) {
-    if (out_mask && !mask_is_device) memset(out_mask, 0, (size_t)k);
-    return 1;
-  }
-  memcpy(out_model, hbest->model, 9 * 8);
-  *out_ninl = *reinterpret_cast<int*>(hb + sizeof(RsBest));
-  if (want_pose) {
-    const double* p = reinterpret_cast<const double*>(hb + sizeof(RsBest) + 16);
-    memcpy(out_R, p, 9 * 8);
-    memcpy(out_t, p + 9, 3 * 8);
+  B2_CUDA(ctx, cudaMemcpyAsync(hout, dout, (size_t)L * sizeof(RsOut), cudaMemcpyDeviceToHost, st));
+  for (int t = 0; t < L; ++t)
+    if (jobs[live[t]].hmask)
+      B2_CUDA(ctx, cudaMemcpyAsync(jobs[live[t]].hmask, htab[t].mask, (size_t)jobs[live[t]].k, cudaMemcpyDeviceToHost, st));
+  RS_SYNC(ctx, st);
+  for (int t = 0; t < L; ++t) {
+    const RsJob& j = jobs[live[t]];
+    b2_ransac_result& r = res[live[t]];
+    if (!hout[t].best.valid) continue;  // status 1; k_rs_mask wrote zeros
+    r.status = 0;
+    r.num_inliers = hout[t].count;
+    memcpy(r.model, hout[t].best.model, 9 * 8);
+    if (j.pose) memcpy(r.R, hout[t].pose, 9 * 8), memcpy(r.t, hout[t].pose + 9, 3 * 8);
   }
   return B2_OK;
+}
+
+// the caller holds ctx->mu and has selected the device
+static int rs_run(b2_context* ctx, const RsJob* jobs, int n, double confidence, uint64_t seed, b2_ransac_result* res,
+                  cudaStream_t st, b2_ransac_trace* tr = nullptr) {
+  if (!ctx->rs) ctx->rs = new RansacState();
+  std::vector<size_t> bytes(n);
+  for (int i = 0; i < n; ++i)
+    bytes[i] = rs_job_bytes(jobs[i].k, jobs[i].mode, jobs[i].max_iters, !jobs[i].dx1, !jobs[i].dmask, tr ? tr->batch : RS_BATCH);
+  std::vector<int> first(n + 1);
+  const int subs = rs_plan(bytes.data(), n, (size_t)ctx->rs_workspace_mb << 20, first.data());
+  for (int b = 0; b < subs; ++b)
+    if (int rc = rs_run_sub(ctx, jobs + first[b], first[b + 1] - first[b], confidence, seed, res + first[b], st, tr)) return rc;
+  return B2_OK;
+}
+
+// the per-pair entry points: a table of one problem
+static int rs_run_one(b2_context* ctx, const RsJob& job, const b2_ransac_params* prm, double* out_model, int* out_ninl,
+                      double* out_R, double* out_t, cudaStream_t st, b2_ransac_trace* tr = nullptr) {
+  b2_ransac_result r;
+  *out_ninl = 0;
+  if (int rc = rs_run(ctx, &job, 1, prm->confidence, prm->seed, &r, st, tr)) return rc;
+  if (r.status) return 1;
+  memcpy(out_model, r.model, 9 * 8);
+  *out_ninl = r.num_inliers;
+  if (job.pose) memcpy(out_R, r.R, 9 * 8), memcpy(out_t, r.t, 3 * 8);
+  return B2_OK;
+}
+
+static RsJob rs_host_job(int mode, const double* x1, const double* x2, int k, const b2_ransac_params* prm, uint8_t* out_mask,
+                         bool pose) {
+  RsJob j;
+  j.hx1 = x1, j.hx2 = x2, j.k = k, j.mode = mode, j.max_iters = prm->max_iters, j.threshold = prm->threshold;
+  j.hmask = out_mask, j.pose = pose;
+  return j;
 }
 
 extern "C" int b2_ransac_essential_host(b2_context* ctx, const double* x1, const double* x2, int k,
@@ -667,7 +929,8 @@ extern "C" int b2_ransac_essential_host(b2_context* ctx, const double* x1, const
   if (!ctx || !x1 || !x2 || !params || !out_model || !out_num_inliers || k < 0) return B2_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
   cudaSetDevice(ctx->device);
-  return rs_run(ctx, x1, x2, k, params, 0, out_model, out_mask, out_num_inliers, out_R, out_t);
+  return rs_run_one(ctx, rs_host_job(0, x1, x2, k, params, out_mask, out_R && out_t), params, out_model, out_num_inliers, out_R,
+                    out_t, ctx->stream);
 }
 
 extern "C" int b2_ransac_fundamental_host(b2_context* ctx, const double* x1, const double* x2, int k,
@@ -676,7 +939,8 @@ extern "C" int b2_ransac_fundamental_host(b2_context* ctx, const double* x1, con
   if (!ctx || !x1 || !x2 || !params || !out_model || !out_num_inliers || k < 0) return B2_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
   cudaSetDevice(ctx->device);
-  return rs_run(ctx, x1, x2, k, params, 1, out_model, out_mask, out_num_inliers, nullptr, nullptr);
+  return rs_run_one(ctx, rs_host_job(1, x1, x2, k, params, out_mask, false), params, out_model, out_num_inliers, nullptr,
+                    nullptr, ctx->stream);
 }
 
 extern "C" int b2_ransac_essential_dev(b2_context* ctx, const float* kp1, const float* kp2, const int64_t* matches, int k,
@@ -687,20 +951,57 @@ extern "C" int b2_ransac_essential_dev(b2_context* ctx, const float* kp1, const 
   if (k > 0 && (!kp1 || !kp2 || !matches)) return B2_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
   cudaSetDevice(ctx->device);
-  if (!ctx->rs) ctx->rs = new RansacState();
-  RansacState* s = ctx->rs;
-  cudaStream_t st = (cudaStream_t)stream;
-  if (k > 0) {
-    B2_CUDA(ctx, s->x1.ensure((size_t)k * 16));
-    B2_CUDA(ctx, s->x2.ensure((size_t)k * 16));
-    B2_LAUNCH(ctx, k_rs_gather, cdiv(k, 256), 256, 0, st, kp1, kp2, (const long long*)matches, k, cal1[0], cal1[1], cal1[2],
-              cal2[0], cal2[1], cal2[2], s->x1.as<double>(), s->x2.as<double>());
-    B2_CHECK_LAUNCH(ctx);
-  }
-  // rs_run uses the legacy stream when `stream` is NULL; the context stream otherwise stays unused here
-  return rs_run(ctx, nullptr, nullptr, k, params, 0, out_model, out_mask_dev, out_num_inliers, out_R, out_t,
-                st ? st : cudaStreamLegacy, 1);
+  RsJob j;
+  j.kp1 = kp1, j.kp2 = kp2, j.matches = matches, j.k = k, j.mode = 0, j.max_iters = params->max_iters;
+  j.threshold = params->threshold, j.dmask = out_mask_dev, j.pose = out_R && out_t;
+  memcpy(j.cal1, cal1, sizeof(j.cal1)), memcpy(j.cal2, cal2, sizeof(j.cal2));
+  // the legacy stream when `stream` is NULL; the context stream stays unused here
+  return rs_run_one(ctx, j, params, out_model, out_num_inliers, out_R, out_t, stream ? (cudaStream_t)stream : cudaStreamLegacy);
 }
+
+static size_t rs_problem_bytes(const b2_ransac_problem& p) { return rs_job_bytes(p.k, p.mode, p.max_iters, !p.x1, !p.mask); }
+
+extern "C" size_t b2_ransac_workspace_bytes(const b2_ransac_problem* problem) {
+  return problem && (problem->mode == 0 || problem->mode == 1) && problem->k >= 0 ? rs_problem_bytes(*problem) : 0;
+}
+
+extern "C" int b2_ransac_plan(const b2_ransac_problem* problems, int n, size_t budget_bytes, int* out_first) {
+  if (n < 0 || !out_first || (n > 0 && !problems)) return B2_ERR_ARG;
+  std::vector<size_t> bytes(n);
+  for (int i = 0; i < n; ++i) {
+    if ((problems[i].mode != 0 && problems[i].mode != 1) || problems[i].k < 0) return B2_ERR_ARG;
+    bytes[i] = rs_problem_bytes(problems[i]);
+  }
+  return rs_plan(bytes.data(), n, budget_bytes, out_first);
+}
+
+extern "C" int b2_ransac_verify_batched_dev(b2_context* ctx, const b2_ransac_problem* problems, int n,
+                                            const b2_ransac_params* params, b2_ransac_result* results, void* stream) {
+  if (!ctx || !params || n < 0 || (n > 0 && (!problems || !results))) return B2_ERR_ARG;
+  if (!(params->confidence > 0.0 && params->confidence < 1.0)) return b2_fail(ctx, B2_ERR_ARG, "ransac: confidence must be in (0, 1)");
+  std::vector<RsJob> jobs(n);
+  for (int i = 0; i < n; ++i) {
+    const b2_ransac_problem& p = problems[i];
+    const std::string at = "ransac problem " + std::to_string(i) + ": ";
+    if (p.k < 0 || (p.mode != 0 && p.mode != 1)) return b2_fail(ctx, B2_ERR_ARG, at + "k < 0 or mode not 0 / 1");
+    if (!(p.threshold >= 0.0)) return b2_fail(ctx, B2_ERR_ARG, at + "threshold must be >= 0");
+    const bool ready = p.x1 || p.x2;
+    if (ready && (!p.x1 || !p.x2)) return b2_fail(ctx, B2_ERR_ARG, at + "x1 and x2 go together");
+    if (p.k > 0 && !ready && (!p.kp1 || !p.kp2 || !p.matches)) return b2_fail(ctx, B2_ERR_ARG, at + "no points");
+    // the focal lengths divide: E problems calibrate the keypoints with them, F problems their inliers for the pose
+    if ((p.mode == 1 || !ready) && !(p.cal1[0] > 0.0 && p.cal2[0] > 0.0)) return b2_fail(ctx, B2_ERR_ARG, at + "focal length must be > 0");
+    RsJob& j = jobs[i];
+    j.kp1 = p.kp1, j.kp2 = p.kp2, j.matches = p.matches, j.dx1 = p.x1, j.dx2 = p.x2;
+    j.k = p.k, j.mode = p.mode, j.max_iters = p.max_iters, j.threshold = p.threshold, j.dmask = p.mask, j.pose = true;
+    memcpy(j.cal1, p.cal1, sizeof(j.cal1)), memcpy(j.cal2, p.cal2, sizeof(j.cal2));
+  }
+  if (n == 0) return B2_OK;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  return rs_run(ctx, jobs.data(), n, params->confidence, params->seed, results, stream ? (cudaStream_t)stream : cudaStreamLegacy);
+}
+
+extern "C" uint64_t b2_ransac_sync_count(const b2_context* ctx) { return ctx ? ctx->rs_syncs : 0; }
 
 // out_cands / out_votes / out_winner: tests only (nullptr from b2_recover_pose_host)
 static int recover_pose(b2_context* ctx, const double* E, const double* x1, const double* x2, int k, double* out_R, double* out_t,
@@ -713,32 +1014,35 @@ static int recover_pose(b2_context* ctx, const double* E, const double* x1, cons
   cudaStream_t st = ctx->stream;
   B2_CUDA(ctx, s->x1.ensure((size_t)(k + 1) * 16));
   B2_CUDA(ctx, s->x2.ensure((size_t)(k + 1) * 16));
-  B2_CUDA(ctx, s->pose.ensure(64 * 8));
-  B2_CUDA(ctx, s->hbuf.ensure(sizeof(RsBest) + 16 * 8 + 64));
+  B2_CUDA(ctx, s->small.ensure(sizeof(RsOut) + sizeof(RsScratch)));
+  B2_CUDA(ctx, s->tab.ensure(sizeof(RsProb)));
+  B2_CUDA(ctx, s->hbuf.ensure(sizeof(RsProb) + sizeof(RsOut)));
   if (k > 0) {
     B2_CUDA(ctx, cudaMemcpyAsync(s->x1.p, x1, (size_t)k * 16, cudaMemcpyHostToDevice, st));
     B2_CUDA(ctx, cudaMemcpyAsync(s->x2.p, x2, (size_t)k * 16, cudaMemcpyHostToDevice, st));
   }
-  double* dE = s->pose.as<double>() + 16;
-  B2_CUDA(ctx, cudaMemcpyAsync(dE, E, 9 * 8, cudaMemcpyHostToDevice, st));
-  {
-    int* gvotes = reinterpret_cast<int*>(s->pose.as<double>() + 32);
-    B2_CUDA(ctx, cudaMemsetAsync(gvotes, 0, 8 * sizeof(int), st));
-    B2_LAUNCH(ctx, k_rs_pose, k > 0 ? cdiv(k, RS_POSE_THREADS) : 1, RS_POSE_THREADS, 0, st, dE, s->x1.as<double>(), s->x2.as<double>(),
-              (const uint8_t*)nullptr, k, gvotes, s->pose.as<double>(), out_cands ? s->pose.as<double>() + 36 : nullptr);
-  }
+  RsOut* dout = s->small.as<RsOut>();
+  RsScratch* dscr = reinterpret_cast<RsScratch*>(dout + 1);
+  B2_CUDA(ctx, cudaMemsetAsync(dscr->gvotes, 0, sizeof(dscr->gvotes), st));
+  B2_CUDA(ctx, cudaMemcpyAsync(dscr->E, E, 9 * 8, cudaMemcpyHostToDevice, st));
+  RsProb* hp = s->hbuf.as<RsProb>();
+  memset(hp, 0, sizeof(*hp));
+  hp->x1 = s->x1.as<double>(), hp->x2 = s->x2.as<double>(), hp->k = k, hp->E = dscr->E, hp->gvotes = dscr->gvotes;
+  hp->pose = dout->pose, hp->pose_cands = out_cands ? dscr->pose_cands : nullptr, hp->pose_on = 1;
+  B2_CUDA(ctx, cudaMemcpyAsync(s->tab.p, hp, sizeof(RsProb), cudaMemcpyHostToDevice, st));
+  B2_LAUNCH(ctx, k_rs_pose, k > 0 ? cdiv(k, RS_POSE_THREADS) : 1, RS_POSE_THREADS, 0, st, s->tab.as<RsProb>());
   B2_CHECK_LAUNCH(ctx);
-  double* h = s->hbuf.as<double>();
-  B2_CUDA(ctx, cudaMemcpyAsync(h, s->pose.p, 13 * 8, cudaMemcpyDeviceToHost, st));
+  double* h = reinterpret_cast<double*>(hp + 1);
+  B2_CUDA(ctx, cudaMemcpyAsync(h, dout->pose, 13 * 8, cudaMemcpyDeviceToHost, st));
   if (out_cands) {
     double c[22];
-    B2_CUDA(ctx, cudaMemcpyAsync(c, s->pose.as<double>() + 36, sizeof(c), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(ctx, cudaMemcpyAsync(out_votes, s->pose.as<double>() + 32, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    B2_CUDA(ctx, cudaStreamSynchronize(st));
+    B2_CUDA(ctx, cudaMemcpyAsync(c, dscr->pose_cands, sizeof(c), cudaMemcpyDeviceToHost, st));
+    B2_CUDA(ctx, cudaMemcpyAsync(out_votes, dscr->gvotes, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    RS_SYNC(ctx, st);
     memcpy(out_cands, c, 21 * 8);
     *out_winner = (int)c[21];
   }
-  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  RS_SYNC(ctx, st);
   memcpy(out_R, h, 9 * 8);
   memcpy(out_t, h + 9, 3 * 8);
   if (out_num_good) *out_num_good = (int)h[12];
@@ -767,6 +1071,6 @@ extern "C" int b2_debug_ransac_trace_host(b2_context* ctx, int mode, const doubl
     return B2_ERR_ARG;
   std::lock_guard<std::mutex> lk(ctx->mu);
   cudaSetDevice(ctx->device);
-  return rs_run(ctx, x1, x2, k, params, mode, out_model, out_mask, out_num_inliers, mode == 0 ? out_R : nullptr,
-                mode == 0 ? out_t : nullptr, nullptr, 0, trace);
+  return rs_run_one(ctx, rs_host_job(mode, x1, x2, k, params, out_mask, mode == 0 && out_R && out_t), params, out_model,
+                    out_num_inliers, out_R, out_t, ctx->stream, trace);
 }

@@ -5,8 +5,9 @@ The reference runs, per pair and per Dask task (gtsfm/two_view_estimator.py:350-
 `cv2.recoverPose` (gtsfm/frontend/verifier/ransac.py:74-81, gtsfm/utils/verification.py:83) and then hands the inliers
 to triangulation / bundle adjustment on the CPU.  Here a whole shard of pairs is walked on one GPU with every keypoint
 and match tensor resident in HBM: calibration, hypothesis generation, scoring, local optimisation, the inlier mask
-and the cheirality vote are the kernels of csrc/ransac.cu (`b2_ransac_essential_dev`), pair p's verification runs on
-its own stream under pair p+1's matching, and only what the CPU back half consumes leaves the device: the verified rows
+and the cheirality vote are the kernels of csrc/ransac.cu (`b2_ransac_verify_batched_dev`: one call per matched chunk of
+up to 8 pairs, every stage launched once for the chunk), chunk c's verification runs on its own stream under chunk c+1's
+matching, and only what the CPU back half consumes leaves the device: the verified rows
 of the match array, R, t and the inlier ratio - exactly the `VerifierBase.verify` tuple (verifier_base.py:67-90).
 """
 from __future__ import annotations
@@ -53,31 +54,38 @@ class B200TwoViewBatch:
             putative: Optional[Mapping[Tuple[int, int], torch.Tensor]] = None) -> Dict[Tuple[int, int], TwoViewResult]:
         """`putative[(i1, i2)]`: (k, 2) int64 device tensor of match indices; matched here with LightGlue when absent."""
         out: Dict[Tuple[int, int], TwoViewResult] = {}
-        pending = []  # (pair, matches, future) in flight on the verification stream
+        pending = []  # (pairs, matches, future) of a chunk in flight on the verification stream
         pairs = list(pairs)
         for c0 in range(0, len(pairs), MATCH_BATCH):
             chunk = pairs[c0:c0 + MATCH_BATCH]
             todo = [pr for pr in chunk if putative is None or pr not in putative]
             matched = dict(zip(todo, self.fe.match_batch([(features[i1], features[i2]) for i1, i2 in todo])))
+            prs, items = [], []
             for i1, i2 in chunk:
-                a, b = features[i1], features[i2]
                 m = putative[(i1, i2)] if (i1, i2) not in matched else matched[(i1, i2)][0]
                 k = int(m.shape[0])
                 if k < MIN_MATCHES_E:
                     out[(i1, i2)] = _failure(k)
                     continue
-                # this chunk's verifications run on their own stream / thread under the next chunk's matching
-                pending.append(((i1, i2), m, self.fe.verify_async(a, b, m, intrinsics[i1], intrinsics[i2], self.threshold_px, self.seed)))
-            while len(pending) > MATCH_BATCH:
-                self._collect(pending.pop(0), out)
+                prs.append((i1, i2))
+                items.append((features[i1], features[i2], m, intrinsics[i1], intrinsics[i2]))
+            if items:  # this chunk's verification: one call on its own stream / thread under the next chunk's matching
+                pending.append((prs, [it[2] for it in items], self.fe.verify_many_async(items, self.threshold_px, self.seed)))
+            while len(pending) > 1:
+                self._collect_chunk(pending.pop(0), out)
         for p in pending:
-            self._collect(p, out)
+            self._collect_chunk(p, out)
         return out
 
+    @classmethod
+    def _collect_chunk(cls, chunk, out) -> None:
+        prs, ms, fut = chunk
+        for pair, m, r in zip(prs, ms, fut.result()):
+            cls._collect_one(pair, m, r, out)
+
     @staticmethod
-    def _collect(item, out) -> None:
-        pair, m, fut = item
-        E, R, t, n_inl, mask = fut.result()
+    def _collect_one(pair, m, result, out) -> None:
+        E, R, t, n_inl, mask = result
         k = int(m.shape[0])
         if E is None:
             out[pair] = _failure(k)

@@ -8,7 +8,7 @@ delegates to OpenCV runs in libgtsfm_b200.so (CUDA).
 """
 from __future__ import annotations
 
-from typing import Optional, Tuple
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -32,6 +32,29 @@ def normalize_coordinates(coordinates: np.ndarray, intrinsics) -> np.ndarray:
         K = intrinsics.K()
         return np.stack([(c[:, 0] - K[0, 2]) / K[0, 0], (c[:, 1] - K[1, 2]) / K[1, 1]], -1)
     return np.vstack([intrinsics.calibrate(x[:2].reshape(2, 1)).ravel() for x in c])
+
+
+def pinhole_cal(intrinsics) -> Optional[Tuple[float, float, float]]:
+    """(f, u0, v0) when `intrinsics` is a distortion-free pinhole model with one focal length and no skew, which is what the
+    device calibrates with (`k_rs_gather` computes the same (u - u0) / f in double as `normalize_coordinates`); else None."""
+    k1 = intrinsics.k1() if hasattr(intrinsics, "k1") else 0.0
+    k2 = intrinsics.k2() if hasattr(intrinsics, "k2") else 0.0
+    if k1 != 0.0 or k2 != 0.0 or not hasattr(intrinsics, "px"):
+        return None
+    K = np.asarray(intrinsics.K(), np.float64)
+    if K[0, 0] != K[1, 1] or K[0, 1] != 0.0 or not K[0, 0] > 0.0:
+        return None
+    return float(K[0, 0]), float(K[0, 2]), float(K[1, 2])
+
+
+def ransac_problem(k: int, mode: int, threshold: float, max_iters: int, mask=None, kp1=None, kp2=None, matches=None, x1=None,
+                   x2=None, cal1=(1.0, 0.0, 0.0), cal2=(1.0, 0.0, 0.0)) -> "_lib.RansacProblem":
+    """One b2_ransac_problem.  Array arguments are device tensors or addresses; the caller keeps them alive over the call."""
+    p = _lib.RansacProblem()
+    p.kp1, p.kp2, p.matches, p.x1, p.x2, p.mask = (_lib.ptr(a) for a in (kp1, kp2, matches, x1, x2, mask))
+    p.k, p.mode, p.max_iters, p.threshold = int(k), int(mode), int(min(max_iters, 2**31 - 1)), float(threshold)
+    p.cal1[:], p.cal2[:] = [float(c) for c in cal1], [float(c) for c in cal2]
+    return p
 
 
 class RansacEngine:
@@ -73,6 +96,19 @@ class RansacEngine:
         if rc == 1:
             return None, mask[:k]
         return F.reshape(3, 3), mask[:k]
+
+    def verify_batched_dev(self, problems: Sequence["_lib.RansacProblem"], confidence=RANSAC_SUCCESS_PROB, seed=DEFAULT_SEED,
+                           stream=None):
+        """b2_ransac_verify_batched_dev: every problem of the list in one call -> ctypes array of b2_ransac_result.
+        `stream`: a raw CUDA stream handle (None / 0: the legacy default stream)."""
+        n = len(problems)
+        arr = (_lib.RansacProblem * max(n, 1))(*problems)
+        res = (_lib.RansacResult * max(n, 1))()
+        prm = _lib.RansacParams(0.0, confidence, 0, seed)
+        rc = self.ctx.lib.b2_ransac_verify_batched_dev(self.ctx.handle, arr, n, _lib.C.byref(prm), res, _lib.C.c_void_p(stream or 0))
+        self.ctx.check(rc, "ransac_verify_batched_dev")
+        self.d2h_bytes += n * _lib.C.sizeof(_lib.RansacResult)
+        return res
 
     def recover_pose(self, E, x1, x2):
         E = np.ascontiguousarray(E, np.float64)
@@ -136,3 +172,69 @@ class B200Ransac(VerifierBase):
         v_corr_idxs = match_indices[inlier_idxs]
         inlier_ratio_est_model = float(np.mean(mask))
         return Rot3(R), Unit3(t), v_corr_idxs, inlier_ratio_est_model
+
+    def verify_many(self, items: Sequence[tuple]) -> List[Tuple[Optional[Rot3], Optional[Unit3], np.ndarray, float]]:
+        """`verify` for a list of its argument tuples in ONE library call: `verify_many(items)[i]` is what
+        `verify(*items[i])` returns (rows and ratio equal; the pose equal for E, and for F up to the rounding of
+        E = K2^T F K1, which the device forms itself).  Keypoints and rows are uploaded once per distinct array and the
+        device gathers and calibrates them; a pair whose intrinsics are not a plain pinhole model (distortion, two focal
+        lengths) is normalised on the host as in `verify` (E) or verified on its own (F)."""
+        out: list = [None] * len(items)
+        live = []
+        for i, (kp1, kp2, rows, _, _) in enumerate(items):
+            n = rows.shape[0]
+            if n < self._min_matches or (self._use_intrinsics_in_verification and n < 6):  # opencv_verifier_base.py:70-79
+                out[i] = self._failure_result
+            else:
+                live.append(i)
+        if not live:
+            return out
+        import torch
+
+        eng = self._ensure_engine()
+        dev = torch.device("cuda", self._device)
+        uploaded = {}
+
+        def up(a: np.ndarray, dtype):  # one device copy per distinct host array
+            key = (id(a), dtype)
+            if key not in uploaded:
+                uploaded[key] = (a, torch.from_numpy(np.ascontiguousarray(a, dtype)).to(dev))
+            return uploaded[key][1]
+
+        mode = 0 if self._use_intrinsics_in_verification else 1
+        batch, problems = [], []
+        masks = torch.zeros(sum(items[i][2].shape[0] for i in live) + 1, dtype=torch.uint8, device=dev)
+        off = 0
+        for i in live:
+            kp1, kp2, rows, intr1, intr2 = items[i]
+            k = rows.shape[0]
+            c1, c2 = pinhole_cal(intr1), pinhole_cal(intr2)
+            xy1, xy2 = np.asarray(kp1.coordinates), np.asarray(kp2.coordinates)
+            gather = xy1.dtype == np.float32 and xy2.dtype == np.float32 and c1 is not None and c2 is not None
+            if mode == 1 and (c1 is None or c2 is None):
+                out[i] = self.verify(*items[i])
+                continue
+            thr = self._estimation_threshold_px / max(intr1.K()[0, 0], intr2.K()[0, 0]) if mode == 0 else self._estimation_threshold_px
+            args = dict(mask=masks[off:off + k], cal1=c1 or (1.0, 0.0, 0.0), cal2=c2 or (1.0, 0.0, 0.0))
+            if gather:
+                args.update(kp1=up(xy1, np.float32), kp2=up(xy2, np.float32), matches=up(rows, np.int64))
+            else:
+                idx1, idx2 = rows[:, 0].astype(np.int64), rows[:, 1].astype(np.int64)
+                if mode == 0:
+                    p1, p2 = normalize_coordinates(xy1[idx1], intr1), normalize_coordinates(xy2[idx2], intr2)
+                else:
+                    p1, p2 = xy1.astype(np.float64)[idx1], xy2.astype(np.float64)[idx2]
+                args.update(x1=up(p1, np.float64), x2=up(p2, np.float64))
+            problems.append(ransac_problem(k, mode, thr, E_MAX_ITERS if mode == 0 else F_MAX_ITERS, **args))
+            batch.append((i, off))
+            off += k
+        res = eng.verify_batched_dev(problems, seed=self._seed, stream=torch.cuda.current_stream(dev).cuda_stream)
+        masks_h = masks.cpu().numpy()
+        for (i, o), r in zip(batch, res):
+            if r.status != 0:
+                out[i] = self._failure_result
+                continue
+            rows = items[i][2]
+            mask = masks_h[o:o + rows.shape[0]]
+            out[i] = (Rot3(np.array(r.R).reshape(3, 3)), Unit3(np.array(r.t)), rows[np.where(mask == 1)[0]], float(np.mean(mask)))
+        return out

@@ -50,6 +50,8 @@ uint64_t b2_h2d_bytes(const b2_context* ctx);
  * "lightglue_batch" = 0..8: pairs per lock-step batch of b2_lightglue_match_batched_dev (0 = 8, the maximum).
  * "force_simt" = 0 | 1: models whose weights are set afterwards run the exact-fp32 SIMT kernels instead of the wgmma
  * split-fp16 ones (the on-device cross-check of the tensor-core path; tests only).
+ * "ransac_workspace_mb" = 1..: device workspace one sub-batch of b2_ransac_verify_batched_dev may use (default 1024); a call with
+ * more problems than fit is cut into consecutive sub-batches, which changes no result.
  * "superpoint_graph" = 0 (default) | 1: launch every kernel of the SuperPoint network directly / replay the ~21 launches as one
  * CUDA graph per (image shape, parameters, buffers) key (the path is GPU-bound, not launch-bound).
  * "feature_cache" = 0 | 1: drop every cached device copy of host feature arrays and (0, default) copy on every call like the
@@ -270,6 +272,51 @@ int b2_ransac_fundamental_host(b2_context* ctx, const double* x1, const double* 
 int b2_ransac_essential_dev(b2_context* ctx, const float* kp1, const float* kp2, const int64_t* matches, int k,
                             const double* cal1, const double* cal2, const b2_ransac_params* params, double* out_model,
                             uint8_t* out_mask_dev, int* out_num_inliers, double* out_R, double* out_t, void* stream);
+/* Batched verification: n independent problems, every stage launched once for all of them, results equal bit for bit to
+ * what the per-pair entry points return for each problem alone (same seed, same kernels, fixed-order reductions).
+ * Points: either x1 / x2, DEVICE [k][2] double ready to use (calibrated for mode 0, pixels for mode 1), or, when both are
+ * NULL, kp1 / kp2 DEVICE [n][2] float pixel coordinates + matches DEVICE [k][2] int64 rows, which the library gathers and,
+ * for mode 0, calibrates with cal1 / cal2 = {f, u0, v0} as b2_ransac_essential_dev does.  Mode 1 estimates F on pixels and
+ * then recovers the pose on the device as well: E = K2^T F K1 and the inliers calibrated with each side's cal
+ * (gtsfm/utils/verification.py:54-112), so cal is required for mode 1 and for gathered mode 0 problems (f > 0).
+ * threshold / max_iters: as in b2_ransac_params, per problem (thr_px / max(f) differs per pair; E callers pass 1000, F callers
+ * 10^6).  mask: DEVICE [k] uint8, written; may be NULL. */
+typedef struct b2_ransac_problem {
+  const float* kp1;
+  const float* kp2;
+  const int64_t* matches;
+  const double* x1;
+  const double* x2;
+  int k;
+  int mode;          /* 0 = essential (5-point), 1 = fundamental (8-point) */
+  int max_iters;
+  double cal1[3];
+  double cal2[3];
+  double threshold;
+  uint8_t* mask;
+} b2_ransac_problem;
+typedef struct b2_ransac_result {
+  int status;        /* 0 ok, 1 no model (k below the minimal sample or nothing valid; mask all zero), as the per-pair return value */
+  int num_inliers;
+  double model[9];   /* E (mode 0) or F (mode 1), row-major */
+  double R[9];       /* i2Ri1 row-major, t unit i2ti1 (cv2.recoverPose semantics) */
+  double t[3];
+} b2_ransac_result;
+/* `params` gives the confidence and the seed of the whole call (its threshold and max_iters are not read); `results` is a
+ * HOST array of n.  n = 0 and k = 0 problems are legal.  Bad arguments return B2_ERR_ARG before anything is launched.  The
+ * results of a sub-batch arrive in one copy and the call synchronises `stream` once per sub-batch, plus once per further
+ * sampling round where a problem's budget exceeds one round of 16 384 hypotheses (mode 1 at 10^6: the flags of all problems
+ * are read together and the problems whose confidence bound is met leave the later rounds). */
+int b2_ransac_verify_batched_dev(b2_context* ctx, const b2_ransac_problem* problems, int n, const b2_ransac_params* params,
+                                 b2_ransac_result* results, void* stream);
+/* Device workspace one problem takes in a batched call, and the cut of n problems into consecutive sub-batches under
+ * `budget_bytes` that b2_ransac_verify_batched_dev makes: out_first[i] is the first problem of sub-batch i, out_first[count] =
+ * n (room for n + 1), returns count.  A problem that alone exceeds the budget forms a sub-batch of its own.  Pure host
+ * functions (pointer fields are only tested for NULL). */
+size_t b2_ransac_workspace_bytes(const b2_ransac_problem* problem);
+int b2_ransac_plan(const b2_ransac_problem* problems, int n, size_t budget_bytes, int* out_first);
+/* Stream synchronisations the RANSAC entry points have performed through `ctx` since creation. */
+uint64_t b2_ransac_sync_count(const b2_context* ctx);
 /* cv2.recoverPose restated: decompose E, pick (R, t) with most points in front of both cameras. */
 int b2_recover_pose_host(b2_context* ctx, const double* E, const double* x1, const double* x2, int k, double* out_R,
                          double* out_t, int* out_num_good);
