@@ -4,6 +4,11 @@ This is the L2 seam of SURVEY.md §8b (`CorrespondenceGeneratorBase.generate_cor
 per image and per pair, each pickling ~5 MB of features (det_desc_correspondence_generator.py:65-85), one process per
 GPU walks its shard of the visibility graph and only small results (match index arrays, E / R / t) leave the device.
 PyTorch is used for device buffers and the stream only; all arithmetic is libgtsfm_b200.so through the `*_dev` C ABI.
+
+Besides its own library context, a front end runs "lanes": more contexts, each with its own work buffers, stream and (for
+the roles driven from host threads) one host thread, so that independent images or pairs overlap on the GPU.  `detect_many`
+uses DETECT_LANES of them, `match_superglue_many` SG_LANES and verification one.  Every lane is configured like the front
+end's context: its recorded options are replayed onto the lane before the lane loads its model's weights.
 """
 from __future__ import annotations
 
@@ -11,6 +16,7 @@ import contextlib
 import itertools
 import os
 import threading
+from concurrent.futures import ThreadPoolExecutor
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -36,15 +42,24 @@ class DeviceFeatures:
         return int(self.kp.shape[0])
 
 
-# concurrent LightGlue instances used by match_many.  Default 1: the matcher's persistent kernels already fill the GPU (H100,
-# 40-pair steps of 5000 x 5000 keypoints: 99-105 pairs/s for 1 to 4 lanes, within run-to-run spread)
-MATCH_LANES = int(os.environ.get("B2_MATCH_LANES", "1"))
 SG_LANES = int(os.environ.get("B2_SG_LANES", "3"))  # concurrent SuperGlue instances used by match_superglue_many
 DETECT_LANES = int(os.environ.get("B2_DETECT_LANES", "4"))  # concurrent SuperPoint instances used by detect_many
 # SMs the matcher's persistent kernels leave to the concurrent RANSAC kernels.  H100 (132 SMs), 40-pair LightGlue steps:
 # 99 pairs/s reserving 8, 103-107 reserving 0-4; 4 keeps k_rs_hyp_E's CTAs off the matcher's SMs at no measured cost
 RESERVE_SMS_FOR_VERIFY = int(os.environ.get("B2_RESERVE_SMS", "4"))
 _FRONT_END_SERIAL = itertools.count()  # one per DeviceFrontEnd: an image's LightGlue encoding is only valid for the one that made it
+# model -> (weights packer, the library entry point that loads the packed weights onto a context)
+_MODELS = {"superpoint": (weights.pack_superpoint, "b2_superpoint_set_weights"),
+           "lightglue": (weights.pack_lightglue, "b2_lightglue_set_weights"),
+           "superglue": (weights.pack_superglue, "b2_superglue_set_weights")}
+
+
+@dataclass
+class _Lane:
+    """A library context (own work buffers), the stream its work is enqueued on and, if its role needs one, a host thread."""
+    ctx: _lib.Context
+    stream: Optional[torch.cuda.Stream] = None  # None: the caller's current stream (the front end's own context)
+    pool: Optional[ThreadPoolExecutor] = None  # the lane's host thread, for the roles that drive lanes from threads
 
 
 class DeviceFrontEnd:
@@ -58,38 +73,66 @@ class DeviceFrontEnd:
         self.max_keypoints = max_keypoints
         self.prune_min = -1 if cpu_semantics else 1536
         self.fp16_attention = 1 if fp16_attention else 0  # opt-in: the reference's CUDA numerics (lightglue.py:116-121)
-        blob = weights.pack_superpoint(weights.load_state_dict(superpoint_sd))
-        self._sp_blob = blob
-        self._lanes = []  # extra (context, stream) SuperPoint lanes of detect_many
         self._counts = None
-        self.ctx.check(self.lib.b2_superpoint_set_weights(self.ctx.handle, _lib.ptr(blob), blob.size), "superpoint_set_weights")
-        self._lg_blob = None
-        self._mlanes = []  # extra (context, stream, executor) LightGlue lanes of match_many
-        self._mpool0 = None
-        self._reserve_sms = 0
         self._serial = next(_FRONT_END_SERIAL)
-        # the kernel path (force_simt) LightGlue's weights are loaded under; the extra match_many lanes load them the same way
-        self._lg_simt = self.ctx.options.get("force_simt")
-        if lightglue_sd is not None:
-            blob = weights.pack_lightglue(weights.load_state_dict(lightglue_sd))
-            self._lg_blob = blob
-            self.ctx.check(self.lib.b2_lightglue_set_weights(self.ctx.handle, _lib.ptr(blob), blob.size), "lightglue_set_weights")
-        self._sg_blob = None
-        self._sglanes = []  # (context, stream, executor) SuperGlue lanes of match_superglue_many (lane 0 = self.ctx)
-        if superglue_sd is not None:
-            blob = weights.pack_superglue(weights.load_state_dict(superglue_sd))
-            self._sg_blob = blob
-            self.ctx.check(self.lib.b2_superglue_set_weights(self.ctx.handle, _lib.ptr(blob), blob.size), "superglue_set_weights")
-        # verification runs on its own context + stream + host thread so that the (latency-bound, 16-CTA) RANSAC kernels of
-        # pair p overlap the matcher kernels of pair p+1 (ctypes calls release the GIL)
-        self._vctx: Optional[_lib.Context] = None
-        self._vstream: Optional[torch.cuda.Stream] = None
-        self._vpool = None
-        self._vlock = threading.Lock()
+        self._blobs = {}  # model -> packed weights, kept for the lanes that run the model
+        for model, sd in (("superpoint", superpoint_sd), ("lightglue", lightglue_sd), ("superglue", superglue_sd)):
+            if sd is not None:
+                self._blobs[model] = _MODELS[model][0](weights.load_state_dict(sd))
+                self._set_weights(self.ctx, model)
+        self._lanes: Dict[str, List[_Lane]] = {"superpoint": [], "superglue": []}  # model -> its lanes, made by _role_lanes
+        # verification runs on its own lane so that the (latency-bound, 16-CTA) RANSAC kernels of pair p overlap the matcher
+        # kernels of pair p+1 (ctypes calls release the GIL)
+        self._vlane: Optional[_Lane] = None
+        self._lane_lock = threading.RLock()  # verify_async makes the verification lane from matcher callback threads
+
+    def _set_weights(self, ctx: _lib.Context, model: str) -> None:
+        blob, entry = self._blobs[model], _MODELS[model][1]
+        ctx.check(getattr(self.lib, entry)(ctx.handle, _lib.ptr(blob), blob.size), entry.removeprefix("b2_"))
+
+    def _new_lane(self, model: Optional[str], threaded: bool) -> _Lane:
+        """Another library context on this device, configured like the front end's: its options are replayed first, because
+        force_simt only applies to models loaded after it, then `model`'s weights are loaded (None: no model)."""
+        ctx = _lib.Context(self.device.index)
+        for name, value in self.ctx.options.items():
+            ctx.set_option(name, value)
+        if model is not None:
+            self._set_weights(ctx, model)
+        return _Lane(ctx, torch.cuda.Stream(self.device), ThreadPoolExecutor(max_workers=1) if threaded else None)
+
+    def _role_lanes(self, model: str, n: int, threaded: bool = False) -> List[_Lane]:
+        """The first `n` lanes that run `model`, made on first use (with a host thread each if the role is `threaded`).  Lane 0
+        is the front end's own context on the caller's stream."""
+        with self._lane_lock:
+            lanes = self._lanes[model]
+            while len(lanes) < n:
+                lanes.append(self._new_lane(model, threaded) if lanes else
+                             _Lane(self.ctx, pool=ThreadPoolExecutor(max_workers=1) if threaded else None))
+            return lanes[:n]
+
+    def _verify_lane(self) -> _Lane:
+        with self._lane_lock:
+            if self._vlane is None:
+                # the matcher's persistent kernels (one CTA per SM) leave a few SMs to the concurrent RANSAC kernels: a CTA
+                # that finds its SM occupied would wait for a whole CTA lifetime and double the kernel's duration
+                self._set_option("reserve_sms", RESERVE_SMS_FOR_VERIFY)
+                self._vlane = self._new_lane(None, threaded=True)
+            return self._vlane
+
+    def _set_option(self, name: str, value: int) -> None:
+        """b2_set_option on the front end's context and on every lane made so far; lanes made later get it by the replay."""
+        with self._lane_lock:
+            for ctx in self._all_ctx() + ([self._vlane.ctx] if self._vlane is not None else []):
+                ctx.set_option(name, value)
+
+    @property
+    def _vctx(self) -> Optional[_lib.Context]:
+        """The verification lane's context, None until verification has been used."""
+        return self._vlane.ctx if self._vlane is not None else None
 
     # measurement helpers over every context that runs SuperPoint / matcher kernels for this front end (bench.py)
     def _all_ctx(self):
-        return [self.ctx] + [c for c, _ in self._lanes] + [l[0] for l in self._mlanes] + [l[0] for l in self._sglanes[1:]]
+        return [self.ctx] + [lane.ctx for lanes in self._lanes.values() for lane in lanes[1:]]
 
     def launch_count(self) -> int:
         return sum(c.launch_count() for c in self._all_ctx())
@@ -159,8 +202,9 @@ class DeviceFrontEnd:
     def detect_many(self, images) -> list:
         """`detect` for a list of images with every image enqueued before the first result is read: no host synchronisation
         between images (b2_superpoint_extract_async_dev), one at the end (b2_superpoint_finish_dev).  Images alternate between
-        DETECT_LANES library contexts on as many streams, so one image's narrow kernels (80-CTA layers, the one-block top-k / scan) and
-        launch gaps are filled by the other's.  Same outputs as [detect(im) for im in images]."""
+        DETECT_LANES lanes (library contexts configured like the front end's) on as many streams, so one image's narrow kernels
+        (80-CTA layers, the one-block top-k / scan) and launch gaps are filled by the other's.  Same outputs as
+        [detect(im) for im in images]."""
         if len(images) == 0:
             return []
         kp_all, score_all, desc_all, counts, shapes = self.detect_pool(images)
@@ -174,27 +218,23 @@ class DeviceFrontEnd:
             self._counts = torch.zeros(max(64, len(images)), dtype=torch.int32).pin_memory()
         counts = self._counts
         outs = []
-        lanes = [(self.ctx, torch.cuda.current_stream(self.device))]
-        for j in range(1, min(DETECT_LANES, max(1, len(images)))):
-            if len(self._lanes) < j:  # another SuperPoint instance (own work buffers) + its stream
-                ctx = _lib.Context(self.device.index or 0)
-                ctx.check(self.lib.b2_superpoint_set_weights(ctx.handle, _lib.ptr(self._sp_blob), self._sp_blob.size), "superpoint_set_weights")
-                self._lanes.append((ctx, torch.cuda.Stream(self.device)))
-            self._lanes[j - 1][1].wait_stream(lanes[0][1])  # the images were produced on the caller's stream
-            lanes.append(self._lanes[j - 1])
+        lanes = self._role_lanes("superpoint", min(DETECT_LANES, max(1, len(images))))
+        main = torch.cuda.current_stream(self.device)
+        streams = [main] + [lane.stream for lane in lanes[1:]]
         # ONE allocation per output kind for the whole list (a fresh 5 MB descriptor block per image is a cudaMalloc each when the
         # caller keeps every image's features alive: 360 of them cost 0.7 s for 120 frames), sliced per image
         nimg = max(len(images), slots or 0)
         kp_all = torch.empty((nimg, k, 2), dtype=torch.float32, device=self.device)
         score_all = torch.empty((nimg, k), dtype=torch.float32, device=self.device)
         desc_all = torch.empty((nimg, k, 256), dtype=torch.float32, device=self.device)
-        for _, stream in lanes[1:]:
-            stream.wait_stream(lanes[0][1])  # the pool's previous owner (caching allocator) finished on the caller's stream
+        for stream in streams[1:]:
+            # the images, and the previous owner of the output blocks (caching allocator), are done on the caller's stream
+            stream.wait_stream(main)
             for t in (kp_all, score_all, desc_all):
                 t.record_stream(stream)
         for i, image in enumerate(images):
             assert image.dtype == torch.uint8 and image.is_cuda and image.is_contiguous()
-            ctx, stream = lanes[i % len(lanes)]
+            ctx, stream = lanes[i % len(lanes)].ctx, streams[i % len(lanes)]
             h, w = int(image.shape[0]), int(image.shape[1])
             ch = 1 if image.dim() == 2 else int(image.shape[2])
             kp, score, desc = kp_all[i], score_all[i], desc_all[i]
@@ -203,8 +243,8 @@ class DeviceFrontEnd:
                                                           _lib.C.c_void_p(counts.data_ptr() + 4 * i), _lib.C.c_void_p(stream.cuda_stream))
             ctx.check(rc, "superpoint_extract_async_dev")
             outs.append((h, w))
-        for ctx, stream in lanes:
-            ctx.check(self.lib.b2_superpoint_finish_dev(ctx.handle, _lib.C.c_void_p(stream.cuda_stream)), "superpoint_finish_dev")
+        for lane, stream in zip(lanes, streams):
+            lane.ctx.check(self.lib.b2_superpoint_finish_dev(lane.ctx.handle, _lib.C.c_void_p(stream.cuda_stream)), "superpoint_finish_dev")
         return kp_all, score_all, desc_all, counts[: len(images)].tolist(), outs
 
     def _detect_masked(self, image: torch.Tensor, h: int, w: int, ch: int, mask: np.ndarray) -> DeviceFeatures:
@@ -241,50 +281,32 @@ class DeviceFrontEnd:
         return out[: k.value], stop.value
 
     def match_superglue_many(self, pairs: Sequence[Tuple[DeviceFeatures, DeviceFeatures]], on_pair=None, **kw) -> List[torch.Tensor]:
-        """`match_superglue` over a list of pairs, dealt round-robin to SG_LANES library contexts (own SuperGlue instance, stream
-        and host thread each): SuperGlue runs pair by pair with many narrow kernels (2000-keypoint GNN layers, one-block
-        filters), which concurrent pairs fill.  `on_pair(index, matches)` is called from the lane's thread as a pair completes."""
-        from concurrent.futures import ThreadPoolExecutor
-
-        lanes = min(SG_LANES, len(pairs))
-        if lanes <= 1:
-            out = []
-            for i, (a, b) in enumerate(pairs):
-                m = self.match_superglue(a, b, **kw)
-                if on_pair:
-                    on_pair(i, m)
-                out.append(m)
-            return out
-        while len(self._sglanes) < lanes:  # lane 0 included: every lane has its own host thread
-            if not self._sglanes:
-                ctx = self.ctx
-            else:
-                ctx = _lib.Context(self.device.index or 0)
-                ctx.check(self.lib.b2_superglue_set_weights(ctx.handle, _lib.ptr(self._sg_blob), self._sg_blob.size), "superglue_set_weights")
-                ctx.set_option("reserve_sms", self._reserve_sms)
-            self._sglanes.append((ctx, torch.cuda.Stream(self.device) if self._sglanes else None, ThreadPoolExecutor(max_workers=1)))
+        """`match_superglue` over a list of pairs, dealt round-robin to SG_LANES lanes (library contexts configured like the front
+        end's, with their own SuperGlue instance, stream and host thread each): SuperGlue runs pair by pair with many narrow
+        kernels (2000-keypoint GNN layers, one-block filters), which concurrent pairs fill.  `on_pair(index, matches)` is called
+        from the lane's thread as a pair completes.  Results in input order."""
+        if len(pairs) == 0:
+            return []
+        lanes = self._role_lanes("superglue", max(1, min(SG_LANES, len(pairs))), threaded=True)
         main = torch.cuda.current_stream(self.device)
 
-        def work(lane, idxs):
-            ctx, stream, _ = self._sglanes[lane]
-            res = []
-            with torch.cuda.stream(stream if stream is not None else main):
-                for i in idxs:
-                    m = self.match_superglue(*pairs[i], ctx=ctx, **kw)
-                    if stream is not None:
+        def work(j):
+            lane, res = lanes[j], []
+            with torch.cuda.stream(lane.stream if lane.stream is not None else main):
+                for i in range(j, len(pairs), len(lanes)):
+                    m = self.match_superglue(*pairs[i], ctx=lane.ctx, **kw)
+                    if lane.stream is not None:
                         m.record_stream(main)
                     if on_pair:
                         on_pair(i, m)
-                    res.append((i, m))
+                    res.append(m)
             return res
 
-        for _, stream, _ in self._sglanes[1:lanes]:
-            stream.wait_stream(main)  # the features were produced on the caller's stream
-        futs = [self._sglanes[l][2].submit(work, l, list(range(l, len(pairs), lanes))) for l in range(lanes)]
+        for lane in lanes[1:]:
+            lane.stream.wait_stream(main)  # the features were produced on the caller's stream
         out: List[Optional[torch.Tensor]] = [None] * len(pairs)
-        for f in futs:
-            for i, m in f.result():
-                out[i] = m
+        for j, f in enumerate([lane.pool.submit(work, j) for j, lane in enumerate(lanes)]):
+            out[j::len(lanes)] = f.result()
         return out  # type: ignore[return-value]
 
     def match_superglue(self, a: DeviceFeatures, b: DeviceFeatures, sinkhorn_iters: int = 20, match_threshold: float = 0.2,
@@ -301,70 +323,28 @@ class DeviceFrontEnd:
         return out[: k.value].to(torch.int64)
 
     def match_many(self, pairs: Sequence[Tuple[DeviceFeatures, DeviceFeatures]], on_chunk=None, **kw) -> List[Tuple[torch.Tensor, int]]:
-        """`match_batch` over any number of pairs: lock-step batches of 8, dealt to MATCH_LANES library contexts (own LightGlue
-        instance, stream and host thread each) so that one batch's per-layer host syncs, small glue kernels and launch gaps
-        are filled by another batch's kernels.  `on_chunk(first_pair_index, results)` is called (from the lane's thread) as soon
-        as a batch is complete - the hook bench.py uses to start verification early.  Results in input order."""
-        from concurrent.futures import ThreadPoolExecutor
-
-        self.encode([f for p in pairs for f in p])  # on the caller's stream, before the lanes wait for it
-        chunks = [(c0, pairs[c0:c0 + 8]) for c0 in range(0, len(pairs), 8)]
-        lanes = min(MATCH_LANES, len(chunks))
-        if lanes <= 1:
-            out = []
-            for c0, ch in chunks:
-                r = self.match_batch(ch, **kw)
-                if on_chunk:
-                    on_chunk(c0, r)
-                out += r
-            return out
-        while len(self._mlanes) < lanes - 1:  # extra lanes: context + LightGlue weights + stream + a one-thread executor
-            ctx = _lib.Context(self.device.index or 0)
-            if self._lg_simt is not None:
-                ctx.set_option("force_simt", self._lg_simt)
-            ctx.check(self.lib.b2_lightglue_set_weights(ctx.handle, _lib.ptr(self._lg_blob), self._lg_blob.size), "lightglue_set_weights")
-            ctx.set_option("reserve_sms", self._reserve_sms)
-            self._mlanes.append((ctx, torch.cuda.Stream(self.device), ThreadPoolExecutor(max_workers=1)))
-        if self._mpool0 is None:
-            self._mpool0 = ThreadPoolExecutor(max_workers=1)
-        main = torch.cuda.current_stream(self.device)
-
-        def work(lane, c0, ch):
-            if lane == 0:
-                with torch.cuda.stream(main):
-                    r = self.match_batch(ch, **kw)
-            else:
-                ctx, stream, _ = self._mlanes[lane - 1]
-                with torch.cuda.stream(stream):
-                    r = self.match_batch(ch, ctx=ctx, **kw)
-                for m, _ in r:
-                    m.record_stream(main)
+        """`match_batch` over any number of pairs in lock-step batches of 8, every image encoded once up front (one LightGlue
+        instance: the matcher's persistent kernels already fill the GPU, so concurrent instances measured no gain).
+        `on_chunk(first_pair_index, results)` is called as soon as a batch is complete - the hook bench.py uses to start
+        verification early.  Results in input order."""
+        self.encode([f for p in pairs for f in p])
+        out = []
+        for c0 in range(0, len(pairs), 8):
+            r = self.match_batch(pairs[c0:c0 + 8], **kw)
             if on_chunk:
                 on_chunk(c0, r)
-            return r
-
-        for _, stream, _ in self._mlanes[: lanes - 1]:
-            stream.wait_stream(main)  # the features were produced on the caller's stream
-        futs = []
-        for i, (c0, ch) in enumerate(chunks):
-            lane = i % lanes
-            ex = self._mpool0 if lane == 0 else self._mlanes[lane - 1][2]
-            futs.append(ex.submit(work, lane, c0, ch))
-        out = []
-        for f in futs:
-            out += f.result()
+            out += r
         return out
 
     def match_batch(self, pairs: Sequence[Tuple[DeviceFeatures, DeviceFeatures]], depth_confidence=0.95, width_confidence=0.99,
-                    filter_threshold=0.1, ctx: Optional[_lib.Context] = None) -> List[Tuple[torch.Tensor, int]]:
+                    filter_threshold=0.1) -> List[Tuple[torch.Tensor, int]]:
         """LightGlue over a list of pairs through `b2_lightglue_match_batched_dev`: the library walks up to 8 pairs in
         lock-step (one launch per layer step for all their images), starting every image from its encoding (`encode`).
         -> [(matches (k, 2) int64 device tensor, stop layer)]."""
         n = len(pairs)
         if n == 0:
             return []
-        ctx = ctx or self.ctx
-        key = self.encode([f for p in pairs for f in p], ctx=ctx)
+        key = self.encode([f for p in pairs for f in p])
         arr = (_lib.LightGluePair * n)()
         outs = []
         for i, (a, b) in enumerate(pairs):
@@ -374,8 +354,8 @@ class DeviceFrontEnd:
             arr[i].kp1, arr[i].desc1, arr[i].n1, arr[i].enc1 = b.kp.data_ptr(), b.desc.data_ptr(), len(b), b.enc[key].data_ptr()
             arr[i].out_matches, arr[i].out_scores = out.data_ptr(), None
         prm = _lib.LightGlueParams(depth_confidence, width_confidence, filter_threshold, self.prune_min, self.fp16_attention)
-        rc = self.lib.b2_lightglue_match_batched_dev(ctx.handle, arr, n, _lib.C.byref(prm), self._stream())
-        ctx.check(rc, "lightglue_match_batched_dev")
+        rc = self.lib.b2_lightglue_match_batched_dev(self.ctx.handle, arr, n, _lib.C.byref(prm), self._stream())
+        self.ctx.check(rc, "lightglue_match_batched_dev")
         return [(outs[i][: arr[i].out_k], int(arr[i].out_stop_layer)) for i in range(n)]
 
     def _enc_key(self) -> tuple:
@@ -383,7 +363,7 @@ class DeviceFrontEnd:
         # that made it, and under the attention numerics it was made with
         return self._serial, self.fp16_attention
 
-    def encode(self, feats: Sequence[DeviceFeatures], ctx: Optional[_lib.Context] = None) -> tuple:
+    def encode(self, feats: Sequence[DeviceFeatures]) -> tuple:
         """Give every image in `feats` that has none its LightGlue encoding under this front end (the state after layer 0's
         self block, which does not depend on the partner image): one b2_lightglue_encode_batched_dev call on the current
         stream for all of them, so that an image matched against many partners runs that block once.  -> the encoding key."""
@@ -396,9 +376,8 @@ class DeviceFrontEnd:
         for i, (f, buf) in enumerate(zip(todo, bufs)):
             imgs[i].kp, imgs[i].desc, imgs[i].n, imgs[i].out = f.kp.data_ptr(), f.desc.data_ptr(), len(f), buf.data_ptr()
         prm = _lib.LightGlueParams(0.0, 0.0, 0.0, self.prune_min, self.fp16_attention)
-        ctx = ctx or self.ctx
-        ctx.check(self.lib.b2_lightglue_encode_batched_dev(ctx.handle, imgs, len(todo), _lib.C.byref(prm), self._stream()),
-                  "lightglue_encode_batched_dev")
+        self.ctx.check(self.lib.b2_lightglue_encode_batched_dev(self.ctx.handle, imgs, len(todo), _lib.C.byref(prm), self._stream()),
+                       "lightglue_encode_batched_dev")
         for f, buf in zip(todo, bufs):
             f.enc[key] = buf
         return key
@@ -407,24 +386,8 @@ class DeviceFrontEnd:
                      seed: int = DEFAULT_SEED):
         """Same as verify() but returns a concurrent.futures.Future; `matches` must already be complete on the device
         (match() synchronises its stream before returning)."""
-        from concurrent.futures import ThreadPoolExecutor
-
-        with self._vlock:
-            self._ensure_verify_lane()
-        return self._vpool.submit(self.verify, a, b, matches, cal1, cal2, threshold_px, seed, self._vctx, self._vstream)
-
-    def _ensure_verify_lane(self):
-        from concurrent.futures import ThreadPoolExecutor
-
-        if self._vpool is None:
-            self._vctx = _lib.Context(self.device.index)
-            self._vstream = torch.cuda.Stream(self.device)
-            self._vpool = ThreadPoolExecutor(max_workers=1)
-            # the matcher's persistent kernels (one CTA per SM) leave a few SMs to the concurrent RANSAC kernels: a CTA
-            # that finds its SM occupied would wait for a whole CTA lifetime and double the kernel's duration
-            self._reserve_sms = RESERVE_SMS_FOR_VERIFY
-            for c in [self.ctx] + [l[0] for l in self._mlanes] + [l[0] for l in self._sglanes[1:]]:
-                c.set_option("reserve_sms", RESERVE_SMS_FOR_VERIFY)
+        lane = self._verify_lane()
+        return lane.pool.submit(self.verify, a, b, matches, cal1, cal2, threshold_px, seed, lane.ctx, lane.stream)
 
     def verify(self, a: DeviceFeatures, b: DeviceFeatures, matches: torch.Tensor, cal1: Sequence[float], cal2: Sequence[float],
                threshold_px: float = 4.0, seed: int = DEFAULT_SEED, ctx: Optional[_lib.Context] = None,
@@ -454,9 +417,8 @@ class DeviceFrontEnd:
         """Same as verify_many() but returns ONE concurrent.futures.Future for the whole list, run on the verification lane
         (its own context, stream and thread, under the matcher's kernels); every `matches` must already be complete on the
         device."""
-        with self._vlock:
-            self._ensure_verify_lane()
-        return self._vpool.submit(self.verify_many, items, threshold_px, seed, self._vctx, self._vstream)
+        lane = self._verify_lane()
+        return lane.pool.submit(self.verify_many, items, threshold_px, seed, lane.ctx, lane.stream)
 
     def verify_many(self, items: Sequence[tuple], threshold_px: float = 4.0, seed: int = DEFAULT_SEED,
                     ctx: Optional[_lib.Context] = None, stream: Optional[torch.cuda.Stream] = None) -> list:

@@ -43,8 +43,8 @@ def main():
     from oracle import verifier_ref as vr
 
     fe = DeviceFrontEnd(syn.superpoint_state_dict(0))
-    fe._ensure_verify_lane()
-    vctx = fe._vctx
+    vlane = fe._verify_lane()
+    vctx = vlane.ctx
 
     def scenes(k, ratio):
         out = []
@@ -60,7 +60,7 @@ def main():
         return None if r[0] is None else (r[0].tobytes(), r[1].tobytes(), r[2].tobytes(), r[3], r[4].cpu().numpy().tobytes())
 
     def arm_loop(items):
-        return [fe.verify(*it, ctx=vctx, stream=fe._vstream) for it in items]
+        return [fe.verify(*it, ctx=vctx, stream=vlane.stream) for it in items]
 
     def arm_async(items):
         return [f.result() for f in [fe.verify_async(*it) for it in items]]
@@ -104,7 +104,7 @@ def main():
                     ms = {}
                     for label, chunk in (("batch32", items[:32]), ("one_pair", items[:1])):
                         vctx.profile_start(s)
-                        fe.verify_many(chunk, ctx=vctx, stream=fe._vstream)
+                        fe.verify_many(chunk, ctx=vctx, stream=vlane.stream)
                         ms[label] = round(vctx.profile_stop()[0], 4)
                     stage[s] = ms
                 print(stage, flush=True)

@@ -103,8 +103,9 @@ def test_detect_many_and_graph_replay_equal_detect(b200_ctx):
         assert torch.equal(got.kp, r.kp) and torch.equal(got.score, r.score) and torch.equal(got.desc, r.desc)
 
 
-def test_concurrent_matcher_lanes_equal_sequential(b200_ctx, monkeypatch):
-    """match_many / match_superglue_many with several library contexts on several streams return what the single-lane calls do."""
+def test_superglue_lanes_and_lightglue_batches_equal_sequential(b200_ctx, monkeypatch):
+    """match_superglue_many with several library contexts on several streams returns what the single-lane calls do, and
+    match_many's lock-step batches return what one pair per batch does."""
     from gtsfm_b200 import pipeline
 
     sp_sd, lg_sd, sg_sd = syn.superpoint_state_dict(0), syn.lightglue_state_dict(2, "sharp"), syn.superglue_state_dict(1, "sharp")
@@ -114,12 +115,11 @@ def test_concurrent_matcher_lanes_equal_sequential(b200_ctx, monkeypatch):
     pairs = [(feats[i], feats[j]) for i in range(5) for j in range(i + 1, 5)] * 2  # 20 pairs = 3 lock-step batches
     ref_lg = [fe.match_batch([p])[0] for p in pairs[:10]]
     ref_sg = [fe.match_superglue(*p) for p in pairs[:10]]
-    monkeypatch.setattr(pipeline, "MATCH_LANES", 2)
     monkeypatch.setattr(pipeline, "SG_LANES", 3)
     seen = []
     got_lg = fe.match_many(pairs, on_chunk=lambda c0, res: seen.append((c0, len(res))))
     got_sg = fe.match_superglue_many(pairs)
-    assert sorted(seen) == [(0, 8), (8, 8), (16, 4)] and len(fe._mlanes) == 1 and len(fe._sglanes) == 3
+    assert sorted(seen) == [(0, 8), (8, 8), (16, 4)] and len(fe._lanes["superglue"]) == 3
     for i in range(20):
         assert torch.equal(got_lg[i][0], ref_lg[i % 10][0]) and got_lg[i][1] == ref_lg[i % 10][1]
         assert torch.equal(got_sg[i], ref_sg[i % 10])
