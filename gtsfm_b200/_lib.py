@@ -92,6 +92,16 @@ class RansacTrace(C.Structure):  # b2_ransac_trace (tests only)
                 ("mask_count", C.c_int), ("votes", C.c_int * 4), ("winner", C.c_int), ("pose_cands", C.c_double * 21)]
 
 
+class LmedsParams(C.Structure):  # b2_lmeds_params
+    _fields_ = [("confidence", C.c_double * 2)]
+
+
+class LmedsTrace(C.Structure):  # b2_lmeds_trace (tests only)
+    _fields_ = [("cap", C.c_int), ("idx", C.c_void_p), ("nsol", C.c_void_p), ("models", C.c_void_p), ("medians", C.c_void_p),
+                ("niters", C.c_int), ("drawn", C.c_int), ("slot", C.c_int), ("min_median", C.c_float), ("sigma", C.c_double),
+                ("thr", C.c_float), ("count", C.c_int)]
+
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 
@@ -150,6 +160,10 @@ SIGNATURES = {
     "b2_ransac_verify_batched_dev": (_i, [_vp, C.POINTER(RansacProblem), _i, C.POINTER(RansacParams), C.POINTER(RansacResult), _vp]),
     "b2_ransac_workspace_bytes": (_sz, [C.POINTER(RansacProblem)]),
     "b2_ransac_plan": (_i, [C.POINTER(RansacProblem), _i, _sz, _ip]),
+    "b2_lmeds_verify_batched_dev": (_i, [_vp, C.POINTER(RansacProblem), _i, C.POINTER(LmedsParams), C.POINTER(RansacResult), _vp]),
+    "b2_lmeds_workspace_bytes": (_sz, [C.POINTER(RansacProblem), C.POINTER(LmedsParams)]),
+    "b2_lmeds_plan": (_i, [C.POINTER(RansacProblem), _i, C.POINTER(LmedsParams), _sz, _ip]),
+    "b2_debug_lmeds_trace_host": (_i, [_vp, _i, _vp, _vp, _i, C.POINTER(LmedsParams), _i, C.POINTER(LmedsTrace), C.POINTER(RansacResult), _vp]),
     "b2_ransac_sync_count": (C.c_uint64, [_vp]),
     "b2_recover_pose_host": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _ip]),
     "b2_debug_ransac_trace_host": (_i, [_vp, _i, _vp, _vp, _i, C.POINTER(RansacParams), C.POINTER(RansacTrace), _vp, _vp, _ip, _vp, _vp]),

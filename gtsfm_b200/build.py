@@ -23,6 +23,9 @@ NVCC_FLAGS = [
     # builds both variants on the host
     "-DB2_FIVEPT_QR",
 ]
+# per-source additions: the LMedS verifier replays cv2's double arithmetic, so its products and sums are not contracted
+# into FMAs (its solvers then round as the host build in tests/cpp/lmeds_shim.cpp does)
+NVCC_FLAGS_FOR = {"lmeds.cu": ["-fmad=false"]}
 
 
 def nvcc() -> str:
@@ -51,7 +54,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
 
     def compile_one(job):
         s, o = job
-        cmd = [nvcc(), *NVCC_FLAGS, "-c", str(s), "-o", str(o)]
+        cmd = [nvcc(), *NVCC_FLAGS, *NVCC_FLAGS_FOR.get(s.name, []), "-c", str(s), "-o", str(o)]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"nvcc failed on {s.name}:\n{r.stdout}\n{r.stderr}")

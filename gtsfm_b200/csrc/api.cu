@@ -33,6 +33,7 @@ extern "C" void b2_destroy(b2_context* ctx) {
   lg_destroy(ctx);
   sg_destroy(ctx);
   rs_destroy(ctx);
+  lm_destroy(ctx);
   rt_destroy(ctx);
   nv_destroy(ctx);
   mn_destroy(ctx);

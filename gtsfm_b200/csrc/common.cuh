@@ -94,6 +94,7 @@ struct SuperPointState;
 struct LightGlueState;
 struct SuperGlueState;
 struct RansacState;
+struct LmedsState;
 struct RetrievalState;
 struct NetVladState;
 struct MnnState;
@@ -135,6 +136,7 @@ struct b2_context {
   LightGlueState* lg = nullptr;
   SuperGlueState* sg = nullptr;
   RansacState* rs = nullptr;
+  LmedsState* lm = nullptr;
   RetrievalState* rt = nullptr;
   NetVladState* nv = nullptr;
   MnnState* mn = nullptr;
@@ -207,6 +209,7 @@ void sp_destroy(b2_context* ctx);
 void lg_destroy(b2_context* ctx);
 void sg_destroy(b2_context* ctx);
 void rs_destroy(b2_context* ctx);
+void lm_destroy(b2_context* ctx);
 void rt_destroy(b2_context* ctx);
 void nv_destroy(b2_context* ctx);
 void mn_destroy(b2_context* ctx);

@@ -274,9 +274,69 @@ RM_HDN int upoly_real_roots(const double* p, int deg, double* roots, int max_roo
   return n;
 }
 
+// EVERY real root of p (degree <= 10) in [-1, 1], ascending.  Between two consecutive real roots of p' the polynomial is
+// monotone, so the roots of p' split [-1, 1] into intervals holding at most one root each; the roots of p' come from p''
+// the same way, down to the linear derivative.  Unlike sampling for sign changes this finds close pairs of roots (a pair
+// closer than the sampling step gives no sign change at the samples, but the root of p' between them separates it).
+RM_HDN int upoly_roots_in_unit(const double* p, int deg, double* roots) {
+  double d[11][11];  // d[j] = j-th derivative / j!, ascending, degree deg - j
+  double crit[12], nxt[12];
+  for (int i = 0; i <= deg; ++i) d[0][i] = p[i];
+  for (int j = 1; j <= deg; ++j)
+    for (int i = 0; i <= deg - j; ++i) d[j][i] = d[j - 1][i + 1] * (double)(i + 1);
+  int nc = 0;  // roots of the current derivative in (-1, 1), ascending
+  for (int j = deg - 1; j >= 0; --j) {
+    const double* q = d[j];
+    const int dq = deg - j;
+    double a = -1.0, fa = upoly_eval(q, dq, a);
+    int nn = 0;
+    for (int s = 0; s <= nc; ++s) {
+      const double b = s < nc ? crit[s] : 1.0, fb = upoly_eval(q, dq, b);
+      if (fa == 0.0) {
+        if (nn == 0 || nxt[nn - 1] != a) nxt[nn++] = a;
+      } else if (fb != 0.0 && (fa < 0) != (fb < 0)) {
+        double lo = a, hi = b, flo = fa;
+        for (int it = 0; it < 200; ++it) {
+          const double mid = 0.5 * (lo + hi);
+          if (mid == lo || mid == hi) break;
+          const double fm = upoly_eval(q, dq, mid);
+          if (fm == 0.0) {
+            lo = hi = mid;
+            break;
+          }
+          if ((fm < 0) == (flo < 0)) lo = mid, flo = fm;
+          else hi = mid;
+        }
+        nxt[nn++] = 0.5 * (lo + hi);
+      }
+      a = b, fa = fb;
+    }
+    if (fa == 0.0 && (nn == 0 || nxt[nn - 1] != a)) nxt[nn++] = a;  // a root at +1
+    for (int i = 0; i < nn; ++i) crit[i] = nxt[i];
+    nc = nn;
+  }
+  for (int i = 0; i < nc; ++i) roots[i] = crit[i];
+  return nc;
+}
+// every real root of p: [-1, 1] directly, |z| > 1 as 1 / z of the reversed polynomial's roots in (-1, 1) \ {0}.
+RM_HDN int upoly_all_real_roots(const double* p, int deg, double* roots) {
+  int n = upoly_roots_in_unit(p, deg, roots);
+  double rev[11], rr[10];
+  for (int i = 0; i <= deg; ++i) rev[i] = p[deg - i];
+  const int nr = upoly_roots_in_unit(rev, deg, rr);
+  for (int i = 0; i < nr; ++i)
+    if (rr[i] != 0.0 && fabs(rr[i]) < 1.0) roots[n++] = 1.0 / rr[i];
+  return n;
+}
+
 // ---- 5-point essential-matrix solver (Nister 2004) -------------------------------------------------------------
 // x1, x2: 5 normalised correspondences; E_out: up to 10 solutions, row-major, x2^T E x1 = 0, Frobenius norm 1.
-RM_HDN int fivept_solve(const double (*x1)[2], const double (*x2)[2], double (*E_out)[9]) {
+// kAllRoots = false (fivept_solve, the RANSAC verifier): the degree-10 polynomial's roots are bracketed by sign changes at
+// 161 samples, which can miss a close pair.  kAllRoots = true (fivept_solve_all, the LMedS verifier, which must visit
+// every solution cv2 visits): upoly_all_real_roots.
+// poly_out (kAllRoots only, may be null): receives the scaled degree-10 polynomial in z, ascending (for tests).
+template <bool kAllRoots>
+RM_HDN int fivept_solve_t(const double (*x1)[2], const double (*x2)[2], double (*E_out)[9], double* poly_out = nullptr) {
 #ifdef B2_FIVEPT_QR
   // (opt-in, host-validated, not yet run on the GPU: see DESIGN.md section 8) null space of the 5 x 9 epipolar constraint
   // matrix A by Householder QR of A^T (9 x 5): A^T = Q [R; 0], columns 5..8 of Q are an orthonormal basis of null(A).
@@ -457,8 +517,10 @@ RM_HDN int fivept_solve(const double (*x1)[2], const double (*x2)[2], double (*E
   for (int i = 0; i <= 10; ++i) scale = fabs(detp[i]) > scale ? fabs(detp[i]) : scale;
   if (!(scale > 0.0) || !(scale < 1e300)) return 0;
   for (int i = 0; i <= 10; ++i) detp[i] /= scale;
+  if (kAllRoots && poly_out)
+    for (int i = 0; i <= 10; ++i) poly_out[i] = detp[i];
   double roots[10];
-  int nr = upoly_real_roots(detp, 10, roots, 10);
+  int nr = kAllRoots ? upoly_all_real_roots(detp, 10, roots) : upoly_real_roots(detp, 10, roots, 10);
   int ns = 0;
   for (int ri = 0; ri < nr; ++ri) {
     double z = roots[ri];
@@ -492,6 +554,190 @@ RM_HDN int fivept_solve(const double (*x1)[2], const double (*x2)[2], double (*E
     ++ns;
   }
   return ns;
+}
+RM_HDN int fivept_solve(const double (*x1)[2], const double (*x2)[2], double (*E_out)[9]) {
+  return fivept_solve_t<false>(x1, x2, E_out);
+}
+RM_HDN int fivept_solve_all(const double (*x1)[2], const double (*x2)[2], double (*E_out)[9]) {
+  return fivept_solve_t<true>(x1, x2, E_out);
+}
+
+// ---- cv2's LMedS arithmetic (the LMedS verifier, lmeds.cu) ------------------------------------------------------------
+// Products and sums rounded one at a time (no FMA contraction on the device), so the float cast of an error sees the
+// double cv2 computes.
+#if defined(__CUDA_ARCH__)
+#define RM_MUL(a, b) __dmul_rn((a), (b))
+#define RM_ADD(a, b) __dadd_rn((a), (b))
+#else
+#define RM_MUL(a, b) ((a) * (b))
+#define RM_ADD(a, b) ((a) + (b))
+#endif
+// squared Sampson error of cv2's EMEstimatorCallback::computeError, as float
+RM_HD float sampson_sq_cv(const double* E, double x1, double y1, double x2, double y2) {
+  const double e0 = RM_ADD(RM_ADD(RM_MUL(E[0], x1), RM_MUL(E[1], y1)), E[2]);
+  const double e1 = RM_ADD(RM_ADD(RM_MUL(E[3], x1), RM_MUL(E[4], y1)), E[5]);
+  const double e2 = RM_ADD(RM_ADD(RM_MUL(E[6], x1), RM_MUL(E[7], y1)), E[8]);
+  const double t0 = RM_ADD(RM_ADD(RM_MUL(E[0], x2), RM_MUL(E[3], y2)), E[6]);
+  const double t1 = RM_ADD(RM_ADD(RM_MUL(E[1], x2), RM_MUL(E[4], y2)), E[7]);
+  const double r = RM_ADD(RM_ADD(RM_MUL(x2, e0), RM_MUL(y2, e1)), e2);
+  const double den = RM_ADD(RM_ADD(RM_ADD(RM_MUL(e0, e0), RM_MUL(e1, e1)), RM_MUL(t0, t0)), RM_MUL(t1, t1));
+  return (float)(RM_MUL(r, r) / den);
+}
+// symmetric squared epipolar-line error of cv2's FMEstimatorCallback::computeError (points already float-valued), as float
+RM_HD float epiline_sq_cv(const double* F, double x1, double y1, double x2, double y2) {
+  double a = RM_ADD(RM_ADD(RM_MUL(F[0], x1), RM_MUL(F[1], y1)), F[2]);
+  double b = RM_ADD(RM_ADD(RM_MUL(F[3], x1), RM_MUL(F[4], y1)), F[5]);
+  double c = RM_ADD(RM_ADD(RM_MUL(F[6], x1), RM_MUL(F[7], y1)), F[8]);
+  const double s2 = 1. / RM_ADD(RM_MUL(a, a), RM_MUL(b, b));
+  const double d2 = RM_ADD(RM_ADD(RM_MUL(x2, a), RM_MUL(y2, b)), c);
+  a = RM_ADD(RM_ADD(RM_MUL(F[0], x2), RM_MUL(F[3], y2)), F[6]);
+  b = RM_ADD(RM_ADD(RM_MUL(F[1], x2), RM_MUL(F[4], y2)), F[7]);
+  c = RM_ADD(RM_ADD(RM_MUL(F[2], x2), RM_MUL(F[5], y2)), F[8]);
+  const double s1 = 1. / RM_ADD(RM_MUL(a, a), RM_MUL(b, b));
+  const double d1 = RM_ADD(RM_ADD(RM_MUL(x1, a), RM_MUL(y1, b)), c);
+  const double u = RM_MUL(RM_MUL(d1, d1), s1), v = RM_MUL(RM_MUL(d2, d2), s2);
+  return (float)(u < v ? v : u);
+}
+// cv2's haveCollinearPoints for the last of the first `count` points of p [.][2] (float-valued): is it on a line through two
+// earlier points (or on top of one)?
+RM_HD bool collinear_last(const double (*p)[2], int count) {
+  const int i = count - 1;
+  const double eps = 1.1920928955078125e-07;  // FLT_EPSILON
+  for (int j = 0; j < i; ++j) {
+    const double dx1 = (double)(float)(p[j][0] - p[i][0]), dy1 = (double)(float)(p[j][1] - p[i][1]);
+    for (int k = 0; k < j; ++k) {
+      const double dx2 = (double)(float)(p[k][0] - p[i][0]), dy2 = (double)(float)(p[k][1] - p[i][1]);
+      if (fabs(RM_ADD(RM_MUL(dx2, dy1), -RM_MUL(dy2, dx1))) <= eps * (fabs(dx1) + fabs(dy1) + fabs(dx2) + fabs(dy2))) return true;
+    }
+  }
+  return false;
+}
+
+// 7-point fundamental-matrix solver (Hartley & Zisserman 11.1.2) on float-valued pixels: Hartley normalisation, the
+// two-dimensional null space of the 7 x 9 constraint matrix (F = lambda f1 + (1 - lambda) f2), det F = 0 as a cubic in
+// lambda, every real root, de-normalised and scaled so that F33 = 1 (as cv2's run7Point).  Returns 0..3 solutions.
+RM_HDN int sevenpt_solve(const double (*x1)[2], const double (*x2)[2], double (*F_out)[9]) {
+  double c1x = 0, c1y = 0, c2x = 0, c2y = 0;
+  for (int i = 0; i < 7; ++i) c1x += x1[i][0], c1y += x1[i][1], c2x += x2[i][0], c2y += x2[i][1];
+  const double t = 1. / 7;
+  c1x *= t, c1y *= t, c2x *= t, c2y *= t;
+  double s1 = 0, s2 = 0;
+  for (int i = 0; i < 7; ++i) {
+    s1 += sqrt((x1[i][0] - c1x) * (x1[i][0] - c1x) + (x1[i][1] - c1y) * (x1[i][1] - c1y));
+    s2 += sqrt((x2[i][0] - c2x) * (x2[i][0] - c2x) + (x2[i][1] - c2y) * (x2[i][1] - c2y));
+  }
+  s1 *= t, s2 *= t;
+  if (s1 < 1.1920928955078125e-07 || s2 < 1.1920928955078125e-07) return 0;
+  s1 = 1.4142135623730951 / s1, s2 = 1.4142135623730951 / s2;
+  double A[81];
+  for (int i = 0; i < 81; ++i) A[i] = 0;
+  for (int p = 0; p < 7; ++p) {
+    const double ax = (x1[p][0] - c1x) * s1, ay = (x1[p][1] - c1y) * s1;
+    const double bx = (x2[p][0] - c2x) * s2, by = (x2[p][1] - c2y) * s2;
+    const double q[9] = {bx * ax, bx * ay, bx, by * ax, by * ay, by, ax, ay, 1.0};
+    for (int i = 0; i < 9; ++i)
+      for (int j = 0; j < 9; ++j) A[i * 9 + j] += q[i] * q[j];
+  }
+  double V[81], w[9];
+  jacobi_eig<9>(A, V, w);
+  int o0 = 0, o1 = -1;  // the two smallest eigenvalues span the null space
+  for (int i = 1; i < 9; ++i)
+    if (w[i] < w[o0]) o0 = i;
+  for (int i = 0; i < 9; ++i)
+    if (i != o0 && (o1 < 0 || w[i] < w[o1])) o1 = i;
+  double f1[9], f2[9];
+  for (int i = 0; i < 9; ++i) f2[i] = V[i * 9 + o1], f1[i] = V[i * 9 + o0] - f2[i];
+  // det(lambda f1 + f2) = c3 lambda^3 + c2 lambda^2 + c1 lambda + c0, ascending in cf
+  double cf[4];
+  {
+    double t0 = f2[4] * f2[8] - f2[5] * f2[7], t1 = f2[3] * f2[8] - f2[5] * f2[6], t2 = f2[3] * f2[7] - f2[4] * f2[6];
+    cf[0] = f2[0] * t0 - f2[1] * t1 + f2[2] * t2;
+    cf[1] = f1[0] * t0 - f1[1] * t1 + f1[2] * t2 - f1[3] * (f2[1] * f2[8] - f2[2] * f2[7]) + f1[4] * (f2[0] * f2[8] - f2[2] * f2[6]) -
+            f1[5] * (f2[0] * f2[7] - f2[1] * f2[6]) + f1[6] * (f2[1] * f2[5] - f2[2] * f2[4]) -
+            f1[7] * (f2[0] * f2[5] - f2[2] * f2[3]) + f1[8] * (f2[0] * f2[4] - f2[1] * f2[3]);
+    t0 = f1[4] * f1[8] - f1[5] * f1[7], t1 = f1[3] * f1[8] - f1[5] * f1[6], t2 = f1[3] * f1[7] - f1[4] * f1[6];
+    cf[2] = f2[0] * t0 - f2[1] * t1 + f2[2] * t2 - f2[3] * (f1[1] * f1[8] - f1[2] * f1[7]) + f2[4] * (f1[0] * f1[8] - f1[2] * f1[6]) -
+            f2[5] * (f1[0] * f1[7] - f1[1] * f1[6]) + f2[6] * (f1[1] * f1[5] - f1[2] * f1[4]) -
+            f2[7] * (f1[0] * f1[5] - f1[2] * f1[3]) + f2[8] * (f1[0] * f1[4] - f1[1] * f1[3]);
+    cf[3] = f1[0] * t0 - f1[1] * t1 + f1[2] * t2;
+  }
+  double scale = 0.0;
+  for (int i = 0; i < 4; ++i) scale = fabs(cf[i]) > scale ? fabs(cf[i]) : scale;
+  if (!(scale > 0.0) || !(scale < 1e300)) return 0;
+  for (int i = 0; i < 4; ++i) cf[i] /= scale;
+  double r[6];
+  const int n = upoly_all_real_roots(cf, 3, r);
+  const double T1[9] = {s1, 0, -s1 * c1x, 0, s1, -s1 * c1y, 0, 0, 1}, T2t[9] = {s2, 0, 0, 0, s2, 0, -s2 * c2x, -s2 * c2y, 1};
+  int ns = 0;
+  for (int k = 0; k < n && ns < 3; ++k) {
+    double lambda = r[k], mu = 1.0, Fn[9];
+    const double s = f1[8] * r[k] + f2[8];
+    if (fabs(s) > 2.220446049250313e-16) {
+      mu = 1. / s, lambda *= mu, Fn[8] = 1.0;
+    } else {
+      Fn[8] = 0.0;
+    }
+    for (int i = 0; i < 8; ++i) Fn[i] = f1[i] * lambda + f2[i] * mu;
+    double tmp[9], F[9];
+    mat3_mul(T2t, Fn, tmp);
+    mat3_mul(tmp, T1, F);
+    if (fabs(F[8]) > 1.1920928955078125e-07) {
+      const double inv = 1. / F[8];
+      for (int i = 0; i < 9; ++i) F[i] *= inv;
+    }
+    for (int i = 0; i < 9; ++i) F_out[ns][i] = F[i];
+    ++ns;
+  }
+  return ns;
+}
+
+// ---- cv2's RNG (cv::RNG, multiply-with-carry) and its LMedS subset draw -------------------------------------------
+RM_HD unsigned cvrng_next(unsigned long long& state) {
+  state = (unsigned long long)(unsigned)state * 4164903690ull + (unsigned)(state >> 32);
+  return (unsigned)state;
+}
+// cv2's LMeDS sample table: `niters` subsets of m = 5 (mode 0) or 7 (mode 1) indices of [0, k), one RNG stream seeded with
+// 2^64 - 1.  An index equal to an earlier one of its subset is drawn again.  Mode 1 rejects a subset whose last point is
+// collinear with two earlier ones in either image and draws a whole new one, at most 1000 times per subset.  Returns the
+// subsets drawn: niters, fewer when the attempts ran out (cv2 stops sampling there), 0 when that happened on the first.
+RM_HDN int lmeds_subsets(const double* x1, const double* x2, int k, int mode, int niters, int* idx) {
+  const int m = mode == 0 ? 5 : 7;
+  unsigned long long st = ~0ull;
+  for (int it = 0; it < niters; ++it) {
+    int* s = idx + (size_t)it * m;
+    int attempt = 0;
+    for (; attempt < 1000; ++attempt) {
+      for (int i = 0; i < m; ++i) {
+        int v;
+        bool dup;
+        do {
+          v = (int)(cvrng_next(st) % (unsigned)k);
+          dup = false;
+          for (int j = 0; j < i; ++j) dup |= s[j] == v;
+        } while (dup);
+        s[i] = v;
+      }
+      if (mode == 0) break;
+      double p1[7][2], p2[7][2];
+      for (int i = 0; i < 7; ++i)  // cv2 casts F's points to float32
+        for (int c = 0; c < 2; ++c) p1[i][c] = (double)(float)x1[2 * s[i] + c], p2[i][c] = (double)(float)x2[2 * s[i] + c];
+      if (!collinear_last(p1, 7) && !collinear_last(p2, 7)) break;
+    }
+    if (attempt == 1000) return it;
+  }
+  return niters;
+}
+// cv2's RANSACUpdateNumIters(confidence, 0.45, m, max_iters), at least 3 (LMeDSPointSetRegistrator::run)
+RM_HD int lmeds_niters(double confidence, int m, int max_iters) {
+  const double num = log(fmax(1. - confidence, 2.2250738585072014e-308));
+  const double denom = 1. - pow(0.55, (double)m);
+  int n;
+  if (denom < 2.2250738585072014e-308) n = 0;
+  else {
+    const double ld = log(denom);
+    n = (ld >= 0 || -num >= max_iters * (-ld)) ? max_iters : (int)floor(num / ld + 0.5);
+  }
+  return n > 3 ? n : 3;
 }
 
 // ---- linear (8+ point) estimation helpers ---------------------------------------------------------------------------

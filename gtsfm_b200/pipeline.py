@@ -25,7 +25,7 @@ import torch
 
 from . import _lib, weights
 from .detector_descriptor import KEYPOINT_THRESHOLD, NMS_RADIUS, REMOVE_BORDERS, SuperPointEngine
-from .verifier import DEFAULT_SEED, E_MAX_ITERS, RANSAC_SUCCESS_PROB, ransac_problem
+from .verifier import DEFAULT_SEED, E_MAX_ITERS, LMEDS_MAX_ITERS, RANSAC_SUCCESS_PROB, lmeds_params, ransac_problem
 
 
 @dataclass
@@ -413,18 +413,21 @@ class DeviceFrontEnd:
             return None, None, None, 0, mask[:k]
         return E.reshape(3, 3), R.reshape(3, 3), t, n.value, mask[:k]
 
-    def verify_many_async(self, items: Sequence[tuple], threshold_px: float = 4.0, seed: int = DEFAULT_SEED):
+    def verify_many_async(self, items: Sequence[tuple], threshold_px: float = 4.0, seed: int = DEFAULT_SEED, method: str = "ransac"):
         """Same as verify_many() but returns ONE concurrent.futures.Future for the whole list, run on the verification lane
         (its own context, stream and thread, under the matcher's kernels); every `matches` must already be complete on the
         device."""
+        _check_method(method)
         lane = self._verify_lane()
-        return lane.pool.submit(self.verify_many, items, threshold_px, seed, lane.ctx, lane.stream)
+        return lane.pool.submit(self.verify_many, items, threshold_px, seed, lane.ctx, lane.stream, method)
 
     def verify_many(self, items: Sequence[tuple], threshold_px: float = 4.0, seed: int = DEFAULT_SEED,
-                    ctx: Optional[_lib.Context] = None, stream: Optional[torch.cuda.Stream] = None) -> list:
+                    ctx: Optional[_lib.Context] = None, stream: Optional[torch.cuda.Stream] = None, method: str = "ransac") -> list:
         """verify() for a list of (a, b, matches, cal1, cal2) in one b2_ransac_verify_batched_dev call: every stage is
         launched once for all pairs and the call synchronises once.  -> the list of verify()'s tuples, equal to them bit
-        for bit."""
+        for bit.  method="lmeds": cv2's LMeDS (the reference's LMEDS verifier, 5-point E) in one
+        b2_lmeds_verify_batched_dev call instead; `threshold_px` and `seed` are not used there (LMeDS has neither)."""
+        _check_method(method)
         ctx = ctx or self.ctx
         sptr = _lib.C.c_void_p(stream.cuda_stream) if stream is not None else self._stream()
         ks = [int(m.shape[0]) for _, _, m, _, _ in items]
@@ -440,19 +443,29 @@ class DeviceFrontEnd:
             m = m.contiguous()
             keep.append(m)  # alive until the C call has returned
             live.append(len(out) - 1)
-            problems.append(ransac_problem(k, 0, threshold_px / max(float(cal1[0]), float(cal2[0])), E_MAX_ITERS, mask=mask, kp1=a.kp,
+            thr = threshold_px / max(float(cal1[0]), float(cal2[0])) if method == "ransac" else 0.0
+            problems.append(ransac_problem(k, 0, thr, E_MAX_ITERS if method == "ransac" else LMEDS_MAX_ITERS, mask=mask, kp1=a.kp,
                                            kp2=b.kp, matches=m, cal1=cal1, cal2=cal2))
         if not problems:
             return out
         arr = (_lib.RansacProblem * len(problems))(*problems)
         res = (_lib.RansacResult * len(problems))()
-        prm = _lib.RansacParams(0.0, RANSAC_SUCCESS_PROB, 0, seed)
-        ctx.check(self.lib.b2_ransac_verify_batched_dev(ctx.handle, arr, len(problems), _lib.C.byref(prm), res, sptr),
-                  "ransac_verify_batched_dev")
+        if method == "ransac":
+            prm = _lib.RansacParams(0.0, RANSAC_SUCCESS_PROB, 0, seed)
+            ctx.check(self.lib.b2_ransac_verify_batched_dev(ctx.handle, arr, len(problems), _lib.C.byref(prm), res, sptr),
+                      "ransac_verify_batched_dev")
+        else:
+            ctx.check(self.lib.b2_lmeds_verify_batched_dev(ctx.handle, arr, len(problems), _lib.C.byref(lmeds_params()), res, sptr),
+                      "lmeds_verify_batched_dev")
         for i, r in zip(live, res):
             if r.status == 0:
                 out[i] = (np.array(r.model).reshape(3, 3), np.array(r.R).reshape(3, 3), np.array(r.t), r.num_inliers, out[i][4])
         return out
+
+
+def _check_method(method: str) -> None:
+    if method not in ("ransac", "lmeds"):
+        raise ValueError(f"verification method must be 'ransac' or 'lmeds', not {method!r}")
 
 
 from .distributed import shard_pairs  # noqa: E402,F401  (re-export: `p mod world` partitioner)

@@ -40,15 +40,20 @@ def _failure(num_putative: int) -> TwoViewResult:  # verifier_base.py:60-64
 
 
 class B200TwoViewBatch:
-    """match (optional) -> calibrate -> RANSAC-5pt -> recoverPose for a list of pairs, device-resident.
+    """match (optional) -> calibrate -> RANSAC-5pt (or LMedS-5pt) -> recoverPose for a list of pairs, device-resident.
 
     `intrinsics[i]` = (f, u0, v0) of image i (Cal3Bundler without distortion: what GTSfM's deep front-end configs use).
+    `method`: "ransac" (the reference's Ransac verifier) or "lmeds" (its LMEDS verifier; the threshold and seed are unused).
     """
 
-    def __init__(self, front_end: DeviceFrontEnd, estimation_threshold_px: float = 4.0, seed: int = DEFAULT_SEED):
+    def __init__(self, front_end: DeviceFrontEnd, estimation_threshold_px: float = 4.0, seed: int = DEFAULT_SEED,
+                 method: str = "ransac"):
+        if method not in ("ransac", "lmeds"):
+            raise ValueError(f"verification method must be 'ransac' or 'lmeds', not {method!r}")
         self.fe = front_end
         self.threshold_px = float(estimation_threshold_px)
         self.seed = int(seed)
+        self.method = method
 
     def run(self, features: Mapping[int, DeviceFeatures], pairs: Iterable[Tuple[int, int]], intrinsics: Mapping[int, Sequence[float]],
             putative: Optional[Mapping[Tuple[int, int], torch.Tensor]] = None) -> Dict[Tuple[int, int], TwoViewResult]:
@@ -70,7 +75,7 @@ class B200TwoViewBatch:
                 prs.append((i1, i2))
                 items.append((features[i1], features[i2], m, intrinsics[i1], intrinsics[i2]))
             if items:  # this chunk's verification: one call on its own stream / thread under the next chunk's matching
-                pending.append((prs, [it[2] for it in items], self.fe.verify_many_async(items, self.threshold_px, self.seed)))
+                pending.append((prs, [it[2] for it in items], self.fe.verify_many_async(items, self.threshold_px, self.seed, self.method)))
             while len(pending) > 1:
                 self._collect_chunk(pending.pop(0), out)
         for p in pending:

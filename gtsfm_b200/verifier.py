@@ -238,3 +238,122 @@ class B200Ransac(VerifierBase):
             mask = masks_h[o:o + rows.shape[0]]
             out[i] = (Rot3(np.array(r.R).reshape(3, 3)), Unit3(np.array(r.t)), rows[np.where(mask == 1)[0]], float(np.mean(mask)))
         return out
+
+
+LMEDS_E_CONFIDENCE = 0.999  # cv2.findEssentialMat's default prob (lmeds.py:36-41 passes none)
+LMEDS_F_CONFIDENCE = 0.99  # cv2.findFundamentalMat's default confidence (lmeds.py:58-62)
+LMEDS_MAX_ITERS = 1000  # cv2's default maxIters for both
+
+
+def lmeds_params(e_confidence: float = LMEDS_E_CONFIDENCE, f_confidence: float = LMEDS_F_CONFIDENCE) -> "_lib.LmedsParams":
+    prm = _lib.LmedsParams()
+    prm.confidence[:] = [float(e_confidence), float(f_confidence)]
+    return prm
+
+
+def lmeds_verify_batched_dev(ctx: "_lib.Context", problems: Sequence["_lib.RansacProblem"], params=None, stream=None):
+    """b2_lmeds_verify_batched_dev: every problem of the list in one call -> ctypes array of b2_ransac_result.
+    `stream`: a raw CUDA stream handle (None / 0: the legacy default stream)."""
+    n = len(problems)
+    arr = (_lib.RansacProblem * max(n, 1))(*problems)
+    res = (_lib.RansacResult * max(n, 1))()
+    prm = params if params is not None else lmeds_params()
+    rc = ctx.lib.b2_lmeds_verify_batched_dev(ctx.handle, arr, n, _lib.C.byref(prm), res, _lib.C.c_void_p(stream or 0))
+    ctx.check(rc, "lmeds_verify_batched_dev")
+    return res
+
+
+class B200LMEDS(VerifierBase):
+    """cv2's LMeDS (gtsfm/frontend/verifier/lmeds.py, `LMEDS`) on sm_90a kernels behind GTSfM's VerifierBase.
+
+    Same constructor as the reference; `estimation_threshold_px` is accepted and not used, as there: the inlier threshold
+    comes from the best model's median error.  E (5-point) on calibrated points with cv2's defaults (prob 0.999, 1000
+    iterations), or F (7-point) on pixels (confidence 0.99); the inlier mask is cv2's bit for bit on the scenes
+    tests/test_lmeds_cpu.py checks, and the pose is recovered on the device as for `B200Ransac`."""
+
+    def __init__(self, use_intrinsics_in_verification: bool, estimation_threshold_px: float, device: int = 0) -> None:
+        super().__init__(use_intrinsics_in_verification, estimation_threshold_px)
+        self._device = device
+        self._engine: Optional[RansacEngine] = None
+
+    def __getstate__(self):
+        st = dict(self.__dict__)
+        st["_engine"] = None
+        return st
+
+    def _ensure_engine(self) -> RansacEngine:
+        if self._engine is None:
+            self._engine = RansacEngine(self._device)
+        return self._engine
+
+    def verify(self, keypoints_i1: Keypoints, keypoints_i2: Keypoints, match_indices: np.ndarray, camera_intrinsics_i1,
+               camera_intrinsics_i2) -> Tuple[Optional[Rot3], Optional[Unit3], np.ndarray, float]:
+        return self.verify_many([(keypoints_i1, keypoints_i2, match_indices, camera_intrinsics_i1, camera_intrinsics_i2)])[0]
+
+    def verify_many(self, items: Sequence[tuple]) -> List[Tuple[Optional[Rot3], Optional[Unit3], np.ndarray, float]]:
+        """`verify` for a list of its argument tuples in ONE library call.  Keypoints and rows are uploaded once per
+        distinct array and the device gathers and calibrates them; a pair whose intrinsics are not a plain pinhole model
+        is normalised on the host (E), or has its pose recovered from E = K2^T F K1 on the host (F)."""
+        out: list = [None] * len(items)
+        live = []
+        for i, (kp1, kp2, rows, _, _) in enumerate(items):
+            n = rows.shape[0]
+            if n < self._min_matches or (self._use_intrinsics_in_verification and n < 6):  # opencv_verifier_base.py:70-79
+                out[i] = self._failure_result
+            else:
+                live.append(i)
+        if not live:
+            return out
+        import torch
+
+        eng = self._ensure_engine()
+        dev = torch.device("cuda", self._device)
+        uploaded = {}
+
+        def up(a: np.ndarray, dtype):  # one device copy per distinct host array
+            key = (id(a), dtype)
+            if key not in uploaded:
+                uploaded[key] = (a, torch.from_numpy(np.ascontiguousarray(a, dtype)).to(dev))
+            return uploaded[key][1]
+
+        mode = 0 if self._use_intrinsics_in_verification else 1
+        batch, problems = [], []
+        masks = torch.zeros(sum(items[i][2].shape[0] for i in live) + 1, dtype=torch.uint8, device=dev)
+        off = 0
+        for i in live:
+            kp1, kp2, rows, intr1, intr2 = items[i]
+            k = rows.shape[0]
+            c1, c2 = pinhole_cal(intr1), pinhole_cal(intr2)
+            xy1, xy2 = np.asarray(kp1.coordinates), np.asarray(kp2.coordinates)
+            pinhole = c1 is not None and c2 is not None
+            gather = xy1.dtype == np.float32 and xy2.dtype == np.float32 and pinhole
+            args = dict(mask=masks[off:off + k], cal1=c1 or (1.0, 0.0, 0.0), cal2=c2 or (1.0, 0.0, 0.0))
+            if gather:
+                args.update(kp1=up(xy1, np.float32), kp2=up(xy2, np.float32), matches=up(rows, np.int64))
+            else:
+                idx1, idx2 = rows[:, 0].astype(np.int64), rows[:, 1].astype(np.int64)
+                if mode == 0:
+                    p1, p2 = normalize_coordinates(xy1[idx1], intr1), normalize_coordinates(xy2[idx2], intr2)
+                else:
+                    p1, p2 = xy1.astype(np.float64)[idx1], xy2.astype(np.float64)[idx2]
+                args.update(x1=up(p1, np.float64), x2=up(p2, np.float64))
+            problems.append(ransac_problem(k, mode, 0.0, LMEDS_MAX_ITERS, **args))
+            batch.append((i, off, pinhole))
+            off += k
+        res = lmeds_verify_batched_dev(eng.ctx, problems, stream=torch.cuda.current_stream(dev).cuda_stream)
+        masks_h = masks.cpu().numpy()
+        for (i, o, pinhole), r in zip(batch, res):
+            if r.status != 0:
+                out[i] = self._failure_result
+                continue
+            kp1, kp2, rows, intr1, intr2 = items[i]
+            mask = masks_h[o:o + rows.shape[0]]
+            inl = np.where(mask == 1)[0]
+            R, t = np.array(r.R).reshape(3, 3), np.array(r.t)
+            if mode == 1 and not pinhole:  # utils/verification.py:99-112 with the full K, pose on the host-normalised inliers
+                E = intr2.K().T @ np.array(r.model).reshape(3, 3) @ intr1.K()
+                n1 = normalize_coordinates(np.asarray(kp1.coordinates, np.float64)[rows[inl, 0]], intr1)
+                n2 = normalize_coordinates(np.asarray(kp2.coordinates, np.float64)[rows[inl, 1]], intr2)
+                R, t, _ = eng.recover_pose(E, n1, n2)
+            out[i] = (Rot3(R), Unit3(t), rows[inl], float(np.mean(mask)))
+        return out

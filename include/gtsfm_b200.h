@@ -360,6 +360,42 @@ int b2_debug_ransac_trace_host(b2_context* ctx, int mode, const double* x1, cons
 int b2_debug_recover_pose_host(b2_context* ctx, const double* E, const double* x1, const double* x2, int k, double* out_cands,
                                int* out_votes, int* out_winner, double* out_R, double* out_t, int* out_num_good);
 
+/* ---- LMedS verifier (gtsfm/frontend/verifier/lmeds.py: cv2.findEssentialMat / findFundamentalMat with LMEDS) ----------
+ * A batched device restatement of cv2's LMeDS estimator: cv::RNG subsets (seed 2^64 - 1, F subsets with collinear points
+ * redrawn), max(3, RANSACUpdateNumIters(confidence, 0.45, m, max_iters)) subsets, every real root of the 5-point problem (E)
+ * or of the 7-point cubic (F, points rounded to float32 and F33 = 1), the median of the float errors, the lowest median in
+ * visiting order, and the inliers err <= (float)sigma^2 with sigma = max(0.001, 2.5 * 1.4826 * (1 + 5 / (k - m)) * sqrt(median)).
+ * Problems and results are b2_ransac_problem / b2_ransac_result: mode 0 = E (5-point, calibrated points), 1 = F (7-point,
+ * pixels); `threshold` is not read; `max_iters` is cv2's maxIters (<= 0: 1000, at most 65 536).  An E problem needs k >= 6,
+ * an F problem k >= 8 (the reference's guards; status 1 below that); status is 0 when a model was found (F: and at least 7
+ * inliers), and the pose is recovered as b2_ransac_verify_batched_dev does.  One synchronisation per sub-batch. */
+typedef struct b2_lmeds_params {
+  double confidence[2];  /* per mode: E 0.999 (cv2.findEssentialMat prob), F 0.99 (cv2.findFundamentalMat confidence) */
+} b2_lmeds_params;
+int b2_lmeds_verify_batched_dev(b2_context* ctx, const b2_ransac_problem* problems, int n, const b2_lmeds_params* params,
+                                b2_ransac_result* results, void* stream);
+/* Device workspace of one problem, and the cut into sub-batches under `budget_bytes` (b2_set_option "ransac_workspace_mb"
+ * is the budget of a call), as b2_ransac_workspace_bytes / b2_ransac_plan.  Pure host functions. */
+size_t b2_lmeds_workspace_bytes(const b2_ransac_problem* problem, const b2_lmeds_params* params);
+int b2_lmeds_plan(const b2_ransac_problem* problems, int n, const b2_lmeds_params* params, size_t budget_bytes, int* out_first);
+/* Test-only: one problem on host points (x1 / x2 [k][2] double), with the intermediate state. */
+typedef struct b2_lmeds_trace {
+  int cap;            /* in: subsets the arrays below hold (>= the problem's iteration count) */
+  int* idx;           /* [cap][m] subset table */
+  int* nsol;          /* [cap] solutions per subset */
+  double* models;     /* [cap][10][9] */
+  float* medians;     /* [cap * 10] median per slot (NaN: empty slot) */
+  int niters;         /* out: iteration count */
+  int drawn;          /* out: subsets drawn */
+  int slot;           /* out: chosen slot (subset * 10 + solution), -1 none */
+  float min_median;   /* out */
+  double sigma;       /* out */
+  float thr;          /* out: (float)sigma^2 */
+  int count;          /* out: inliers */
+} b2_lmeds_trace;
+int b2_debug_lmeds_trace_host(b2_context* ctx, int mode, const double* x1, const double* x2, int k, const b2_lmeds_params* params,
+                              int max_iters, b2_lmeds_trace* trace, b2_ransac_result* result, uint8_t* out_mask);
+
 /* ---- NetVLAD global descriptor (SURVEY.md section 8f rank 4; gtsfm/frontend/global_descriptor/netvlad_global_descriptor.py:53-71,
  * thirdparty/hloc/netvlad.py:52-75,163-193) ------------------------------------------------------------------------------------- */
 /* blob = 13 x (conv weight OIHW, bias) of VGG16 features[:-2], score_proj [64][512], centers [512][64], whitening weight
