@@ -54,6 +54,10 @@ class SiftImage(C.Structure):
                 ("out_desc", C.c_void_p), ("out_n", C.c_int), ("out_total", C.c_int)]
 
 
+class OrbImage(C.Structure):  # b2_orb_image: b2_sift_image's layout
+    _fields_ = SiftImage._fields_
+
+
 class D2NetImage(C.Structure):
     _fields_ = [("image", C.c_void_p), ("max_keypoints", C.c_int), ("out_xy", C.c_void_p), ("out_scores", C.c_void_p),
                 ("out_desc", C.c_void_p), ("out_n", C.c_int), ("out_total", C.c_int)]
@@ -64,7 +68,7 @@ class JpegImage(C.Structure):
                 ("out_rounds", C.c_int)]
 
 
-SIFT_CAPACITY = -5  # b2_sift_detect_host: more keypoints than the capacity; *out_n holds the count needed
+SIFT_CAPACITY = -5  # b2_sift_detect_host / b2_orb_detect_host: more keypoints than the capacity; *out_n holds the count needed
 
 
 class RansacParams(C.Structure):
@@ -172,6 +176,8 @@ SIGNATURES = {
     "b2_mnn_match_host": (_i, [_vp, _vp, _i, _vp, _i, _i, _i, C.c_double, _vp, _vp, _ip]),
     "b2_sift_detect_batched_dev": (_i, [_vp, C.POINTER(SiftImage), _i, _i, _i, _i, _sz, _vp]),
     "b2_sift_detect_host": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _ip]),
+    "b2_orb_detect_batched_dev": (_i, [_vp, C.POINTER(OrbImage), _i, _i, _i, _i, _sz, _vp]),
+    "b2_orb_detect_host": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _ip]),
     "b2_d2net_blob_floats": (_sz, []),
     "b2_d2net_norm_table": (_i, [_vp]),
     "b2_d2net_set_weights": (_i, [_vp, _vp, _sz]),

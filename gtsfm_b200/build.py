@@ -24,8 +24,9 @@ NVCC_FLAGS = [
     "-DB2_FIVEPT_QR",
 ]
 # per-source additions: the LMedS verifier replays cv2's double arithmetic, so its products and sums are not contracted
-# into FMAs (its solvers then round as the host build in tests/cpp/lmeds_shim.cpp does)
-NVCC_FLAGS_FOR = {"lmeds.cu": ["-fmad=false"]}
+# into FMAs (its solvers then round as the host build in tests/cpp/lmeds_shim.cpp does); the ORB detector likewise replays
+# cv2's float arithmetic (Harris, angles, pattern rotation, resize coordinates) and writes its one FMA chain out explicitly
+NVCC_FLAGS_FOR = {"lmeds.cu": ["-fmad=false"], "orb.cu": ["-fmad=false"]}
 
 
 def nvcc() -> str:
@@ -44,7 +45,7 @@ def _needs(src: Path, obj: Path, deps) -> bool:
 
 def build(force: bool = False, verbose: bool = False) -> Path:
     OBJ.mkdir(exist_ok=True)
-    headers = list(CSRC.glob("*.cuh")) + list((PKG.parent / "include").glob("*.h"))
+    headers = list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.inc")) + list((PKG.parent / "include").glob("*.h"))
     srcs = sorted(CSRC.glob("*.cu"))
     jobs = []
     for s in srcs:

@@ -41,6 +41,7 @@ extern "C" void b2_destroy(b2_context* ctx) {
   ml_destroy(ctx);
   d2_destroy(ctx);
   jp_destroy(ctx);
+  ob_destroy(ctx);
   for (cudaEvent_t e : ctx->prof.ev) cudaEventDestroy(e);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   delete ctx;

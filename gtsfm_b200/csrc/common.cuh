@@ -18,7 +18,7 @@
 #define B2_ERR_ARG -2
 #define B2_ERR_STATE -3
 #define B2_ERR_MNN_RATIO -4  // ratio test requested with fewer than 2 descriptors on one side (include/gtsfm_b200.h)
-#define B2_SIFT_CAPACITY -5  // b2_sift_detect_host: more keypoints than the caller's capacity, *out_n = the count needed
+#define B2_SIFT_CAPACITY -5  // b2_sift_detect_host / b2_orb_detect_host: more keypoints than the caller's capacity, *out_n = the count needed
 
 // DevBuf / HostBuf own their allocation: the destructor frees it, so a buffer in a model state is freed when the state is
 // deleted and a local one on every return path.  Not copyable (two owners would free twice).
@@ -102,6 +102,7 @@ struct SiftState;
 struct MegaLocState;
 struct D2NetState;
 struct JpegState;
+struct OrbState;
 
 // Device copies of host feature arrays handed to the *_host matcher entry points.  GTSfM matches one image's (keypoints,
 // descriptors) against ~20-40 partners, always passing the same host arrays, so re-uploading 5 MB per image per pair is
@@ -144,6 +145,7 @@ struct b2_context {
   MegaLocState* ml = nullptr;
   D2NetState* d2 = nullptr;
   JpegState* jp = nullptr;
+  OrbState* ob = nullptr;
   // staging shared by the *_host entry points
   DevBuf stage_d[8];
   HostBuf stage_h[4];
@@ -217,6 +219,7 @@ void sf_destroy(b2_context* ctx);
 void ml_destroy(b2_context* ctx);
 void d2_destroy(b2_context* ctx);
 void jp_destroy(b2_context* ctx);
+void ob_destroy(b2_context* ctx);
 
 // shared device helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

@@ -90,26 +90,6 @@ __device__ __forceinline__ int sf_reflect(int p, int len) {
   return p;
 }
 
-// cv2 hal::fastAtan2 (degrees, [0, 360))
-__device__ __forceinline__ float sf_atan(float y, float x) {
-  const float p1 = 0.9997878412794807f * (float)(180 / M_PI), p3 = -0.3258083974640975f * (float)(180 / M_PI);
-  const float p5 = 0.1555786518463281f * (float)(180 / M_PI), p7 = -0.04432655554792128f * (float)(180 / M_PI);
-  const float ax = fabsf(x), ay = fabsf(y);
-  float a, c, c2;
-  if (ax >= ay) {
-    c = ay / (ax + (float)DBL_EPSILON);
-    c2 = c * c;
-    a = (((p7 * c2 + p5) * c2 + p3) * c2 + p1) * c;
-  } else {
-    c = ax / (ay + (float)DBL_EPSILON);
-    c2 = c * c;
-    a = 90.f - (((p7 * c2 + p5) * c2 + p3) * c2 + p1) * c;
-  }
-  if (x < 0) a = 180.f - a;
-  if (y < 0) a = 360.f - a;
-  return a;
-}
-
 // cv2 KeyPoint order used by KeyPointsFilter::removeDuplicatedSorted
 __device__ __forceinline__ bool sf_less(const b2_sift_keypoint& a, const b2_sift_keypoint& b) {
   if (a.x != b.x) return a.x < b.x;
@@ -363,7 +343,7 @@ __global__ void __launch_bounds__(32 * SF_OR_WARPS) k_sift_orient(SfOctArgs a) {
       const float dx = G[(size_t)y * a.w + x + 1] - G[(size_t)y * a.w + x - 1];
       const float dy = G[(size_t)(y - 1) * a.w + x] - G[(size_t)(y + 1) * a.w + x];
       const float wgt = expf((float)(i * i + j * j) * expf_scale);
-      const float ori = sf_atan(dy, dx), mag = sqrtf(dx * dx + dy * dy);
+      const float ori = b2_fast_atan2(dy, dx), mag = sqrtf(dx * dx + dy * dy);
       int bin = __float2int_rn((SF_ORI_BINS / 360.f) * ori);
       if (bin >= SF_ORI_BINS) bin -= SF_ORI_BINS;
       if (bin < 0) bin += SF_ORI_BINS;
@@ -539,7 +519,7 @@ __global__ void __launch_bounds__(32) k_sift_describe(SfDescArgs a) {
       const float dx = img[(size_t)r * cols + c + 1] - img[(size_t)r * cols + c - 1];
       const float dy = img[(size_t)(r - 1) * cols + c] - img[(size_t)(r + 1) * cols + c];
       const float wgt = expf((c_rot * c_rot + r_rot * r_rot) * exp_scale);
-      float obin = (sf_atan(dy, dx) - ori) * bins_per_rad;
+      float obin = (b2_fast_atan2(dy, dx) - ori) * bins_per_rad;
       const float mag = sqrtf(dx * dx + dy * dy) * wgt;
       const int r0 = (int)floorf(rbin), c0 = (int)floorf(cbin);
       int o0 = (int)floorf(obin);

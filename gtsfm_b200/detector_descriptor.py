@@ -1,4 +1,4 @@
-"""SuperPoint, SIFT and D2-Net detector-descriptor plugins.
+"""SuperPoint, SIFT, ORB and D2-Net detector-descriptor plugins.
 
 Drop-in for gtsfm/frontend/detector_descriptor/superpoint.py:32-93 (`SuperPointDetectorDescriptor`): same constructor
 arguments, same `detect_and_describe(image) -> (Keypoints, (N, 256) float32)` contract, same post-processing order
@@ -13,6 +13,9 @@ survive the host-side mask / top-k selection, instead of for every detection (id
 `B200SIFTDetectorDescriptor` is the drop-in for gtsfm/frontend/detector_descriptor/sift.py:24-55 (`SIFTDetectorDescriptor`):
 cv2.SIFT_create() with its defaults, restated in csrc/sift.cu.  Its one deliberate difference: an image without keypoints
 gives (empty Keypoints, (0, 128) float32) where the reference raises a TypeError.
+
+`B200ORBDetectorDescriptor` is the drop-in for gtsfm/frontend/detector_descriptor/orb.py (`ORBDetectorDescriptor`):
+cv2.ORB_create() with its defaults, restated in csrc/orb.cu.
 
 `B200D2NetDetectorDescriptor` is the drop-in for gtsfm/frontend/detector_descriptor/d2net.py (`D2NetDetDesc`), single scale, restated
 in csrc/d2net.cu.
@@ -135,6 +138,10 @@ class SiftEngine:
     """cv2.SIFT_create() defaults on csrc/sift.cu: host calls (every keypoint, as cv2 returns them) and batched device calls
     (the max_keypoints largest responses, uint8 descriptors left on the GPU for TwoWayEngine.match_batched_dev)."""
 
+    DESC_DIM = SIFT_DESC_DIM
+    WORKSPACE_PER_PIXEL = 151  # device workspace bytes per image pixel of a batched call
+    HOST_CALL, BATCHED_CALL, IMAGE_T = "b2_sift_detect_host", "b2_sift_detect_batched_dev", _lib.SiftImage
+
     def __init__(self, device: int = 0, ctx: Optional[_lib.Context] = None, capacity: int = 8192):
         self.ctx = ctx or _lib.Context(device)
         self.capacity = capacity  # first guess of the host call's output size; grown to the count the library reports
@@ -159,24 +166,25 @@ class SiftEngine:
             while True:
                 cap = self.capacity
                 kp = np.empty(cap, _lib.SIFT_KEYPOINT_DTYPE)
-                desc = np.empty((cap, SIFT_DESC_DIM), np.uint8)
+                desc = np.empty((cap, self.DESC_DIM), np.uint8)
                 n = _lib.C.c_int(0)
-                rc = self.ctx.lib.b2_sift_detect_host(self.ctx.handle, _lib.ptr(img), h, w, ch, _lib.ptr(m), _lib.ptr(kp),
-                                                      _lib.ptr(desc), cap, _lib.C.byref(n))
+                rc = getattr(self.ctx.lib, self.HOST_CALL)(self.ctx.handle, _lib.ptr(img), h, w, ch, _lib.ptr(m), _lib.ptr(kp),
+                                                           _lib.ptr(desc), cap, _lib.C.byref(n))
                 if rc == _lib.SIFT_CAPACITY:
                     self.capacity = n.value
                     continue
-                self.ctx.check(rc, "sift_detect_host")
+                self.ctx.check(rc, self.HOST_CALL[3:])
                 return kp[: n.value].copy(), desc[: n.value].copy()
 
-    @staticmethod
-    def images_per_call(h: int, w: int) -> int:
-        return int(max(1, min(64, SIFT_WORKSPACE_BUDGET // (151 * h * w))))
+    @classmethod
+    def images_per_call(cls, h: int, w: int) -> int:
+        return int(max(1, min(64, SIFT_WORKSPACE_BUDGET // (cls.WORKSPACE_PER_PIXEL * h * w))))
 
     def extract_many(self, images, masks=None, max_keypoints: int = 5000):
         """images: sequence of same-shape CUDA uint8 tensors (H, W) / (H, W, C), rows may be pitched (stride(0) >= W C, unit
         inner strides); masks: None or a per-image sequence of CUDA (H, W) uint8 tensors / None.  -> list of (keypoint records
-        as a (n, 6) float32 view [x, y, size, angle, response, octave bits], (n, 128) uint8 descriptors, total before top-k)."""
+        as a (n, 6) float32 view [x, y, size, angle, response, octave bits], (n, DESC_DIM) uint8 descriptors, total before
+        top-k)."""
         import torch
 
         if len(images) == 0:
@@ -193,7 +201,7 @@ class SiftEngine:
         with self.lock:
             for c0 in range(0, len(images), per):
                 idx = range(c0, min(len(images), c0 + per))
-                st = (_lib.SiftImage * len(idx))()
+                st = (self.IMAGE_T * len(idx))()
                 keep = []
                 pitch = None
                 for s, i in enumerate(idx):
@@ -213,13 +221,14 @@ class SiftEngine:
                     if m is not None:
                         m = (m != 0).to(torch.uint8).contiguous()
                     kp = torch.empty((max_keypoints, 6), dtype=torch.float32, device=dev)
-                    desc = torch.empty((max_keypoints, SIFT_DESC_DIM), dtype=torch.uint8, device=dev)
+                    desc = torch.empty((max_keypoints, self.DESC_DIM), dtype=torch.uint8, device=dev)
                     keep.append((x, m, kp, desc))
-                    st[s] = _lib.SiftImage(x.data_ptr(), 0 if m is None else m.data_ptr(), int(max_keypoints), kp.data_ptr(),
-                                           desc.data_ptr(), 0, 0)
+                    st[s] = self.IMAGE_T(x.data_ptr(), 0 if m is None else m.data_ptr(), int(max_keypoints), kp.data_ptr(),
+                                         desc.data_ptr(), 0, 0)
                 stream = torch.cuda.current_stream(dev).cuda_stream
-                rc = self.ctx.lib.b2_sift_detect_batched_dev(self.ctx.handle, st, len(idx), h, w, ch, int(pitch), _lib.C.c_void_p(stream))
-                self.ctx.check(rc, "sift_detect_batched_dev")
+                rc = getattr(self.ctx.lib, self.BATCHED_CALL)(self.ctx.handle, st, len(idx), h, w, ch, int(pitch),
+                                                              _lib.C.c_void_p(stream))
+                self.ctx.check(rc, self.BATCHED_CALL[3:])
                 for s, (_, _, kp, desc) in enumerate(keep):
                     n = st[s].out_n
                     out.append((kp[:n], desc[:n], st[s].out_total))
@@ -255,6 +264,61 @@ class B200SIFTDetectorDescriptor(DetectorDescriptorBase):
                               responses=kp["response"].astype(np.float64))
         keypoints, sel = keypoints.get_top_k(self.max_keypoints)  # gtsfm/.../sift.py:53-54
         return keypoints, desc[sel].astype(np.float32)
+
+
+ORB_DESC_DIM = 32
+
+
+class OrbEngine(SiftEngine):
+    """cv2.ORB_create() defaults on csrc/orb.cu, with SiftEngine's calls: `detect_and_describe` returns every keypoint (level by
+    level, response descending, then y, x), `extract_many` leaves (n, 32) uint8 descriptors on the GPU, which
+    b2_mnn_match_batched_dev takes as they are (u8, dim 32)."""
+
+    DESC_DIM = ORB_DESC_DIM
+    WORKSPACE_PER_PIXEL = 40
+    HOST_CALL, BATCHED_CALL, IMAGE_T = "b2_orb_detect_host", "b2_orb_detect_batched_dev", _lib.OrbImage
+
+    def __init__(self, device: int = 0, ctx: Optional[_lib.Context] = None, capacity: int = 1024):
+        super().__init__(device, ctx, capacity)
+
+
+class B200ORBDetectorDescriptor(DetectorDescriptorBase):
+    """cv2 ORB (default parameters) on hand-written sm_90a kernels behind GTSfM's DetectorDescriptorBase; the drop-in for
+    gtsfm/frontend/detector_descriptor/orb.py (`ORBDetectorDescriptor`).  Its one deliberate difference: an image without
+    keypoints gives (empty Keypoints, (0, 32) uint8) where the reference raises a TypeError."""
+
+    def __init__(self, max_keypoints: int = 5000, device: int = 0) -> None:
+        super().__init__(max_keypoints=max_keypoints)
+        self._device = device
+        self._engine: Optional[OrbEngine] = None  # lazy, never pickled
+
+    def __getstate__(self):
+        st = dict(self.__dict__)
+        st["_engine"] = None
+        return st
+
+    def _ensure_engine(self) -> OrbEngine:
+        if self._engine is None:
+            self._engine = OrbEngine(self._device)
+        return self._engine
+
+    def detect_and_describe(self, image: Image) -> Tuple[Keypoints, np.ndarray]:
+        arr = image.value_array
+        if arr.ndim == 3 and arr.shape[2] not in (3, 4):
+            raise ValueError("Input image dimensions are wrong")  # gtsfm/utils/images.py:39-40
+        kp, desc = self._ensure_engine().detect_and_describe(arr, getattr(image, "mask", None))
+        return orb_keypoints(kp, desc, self.max_keypoints)
+
+
+def orb_keypoints(kp: np.ndarray, desc: np.ndarray, max_keypoints: int) -> Tuple[Keypoints, np.ndarray]:
+    """ORB keypoint records and descriptors -> the reference's (Keypoints(coordinates, scales=size, responses), uint8
+    descriptors) after get_top_k (gtsfm/.../orb.py:51-57)."""
+    if len(kp) == 0:
+        return Keypoints(np.zeros((0, 2))), np.zeros((0, ORB_DESC_DIM), np.uint8)
+    keypoints = Keypoints(np.stack([kp["x"], kp["y"]], 1).astype(np.float64), scales=kp["size"].astype(np.float64),
+                          responses=kp["response"].astype(np.float64))
+    keypoints, sel = keypoints.get_top_k(max_keypoints)
+    return keypoints, desc[sel]
 
 
 D2NET_DESC_DIM = 512

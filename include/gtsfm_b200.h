@@ -498,6 +498,32 @@ int b2_sift_detect_batched_dev(b2_context* ctx, b2_sift_image* images, int n_ima
 int b2_sift_detect_host(b2_context* ctx, const uint8_t* image, int height, int width, int channels, const uint8_t* mask,
                         b2_sift_keypoint* out_keypoints, uint8_t* out_desc, int capacity, int* out_n);
 
+/* ---- ORB detector-descriptor (gtsfm/frontend/detector_descriptor/orb.py) ------------------------------------------------------ */
+/* cv2.ORB_create() with its defaults restated bit for bit: 500 features, scale factor 1.2f, 8 levels, edge threshold 31, FAST
+ * threshold 20, Harris score, patch 31, WTA_K 2.  Images are uint8 H x W x {1, 3, 4} interleaved (RGB / RGBA go through cv2's
+ * fixed-point COLOR_RGB2GRAY); H x W <= 2^24 and each side <= 16384, larger input fails with -2.  A mask keeps a keypoint where
+ * it is non-zero, on every level as cv2 carries it down the pyramid.  Keypoints (b2_sift_keypoint: x, y, size = 31 s_l, angle,
+ * Harris response, octave = level) come level by level, each level by response descending, then y, then x (cv2's order within
+ * a level is std::nth_element's and is not reproduced); the set and every field equal cv2's.  Descriptors are 32 uint8 bytes per
+ * keypoint.  Results do not depend on the batch or the run.  Workspace: about 40 H W bytes per image of a batch. */
+typedef struct b2_orb_image {
+  const uint8_t* image;             /* DEVICE image, row pitch as passed to the call */
+  const uint8_t* mask;              /* DEVICE H x W uint8, dense, or NULL */
+  int max_keypoints;                /* >= 1: the max_keypoints largest responses (ties to the lower index), the order kept */
+  b2_sift_keypoint* out_keypoints;  /* DEVICE [max_keypoints] */
+  uint8_t* out_desc;                /* DEVICE [max_keypoints][32] */
+  int out_n;                        /* written on the HOST struct: keypoints written */
+  int out_total;                    /* written on the HOST struct: keypoints before the top-k */
+} b2_orb_image;
+/* Up to 64 same-shape images: every stage is one launch over the batch, counts stay on the device, and `stream` is synchronised
+ * once at the end. */
+int b2_orb_detect_batched_dev(b2_context* ctx, b2_orb_image* images, int n_images, int height, int width, int channels,
+                              size_t pitch, void* stream);
+/* HOST pointers, dense image, optional mask: every keypoint (no top-k).  When there are more than `capacity` keypoints nothing
+ * is written and the call returns -5 with *out_n = the number needed; otherwise *out_n = the number written. */
+int b2_orb_detect_host(b2_context* ctx, const uint8_t* image, int height, int width, int channels, const uint8_t* mask,
+                       b2_sift_keypoint* out_keypoints, uint8_t* out_desc, int capacity, int* out_n);
+
 /* ---- D2-Net detector-descriptor (gtsfm/frontend/detector_descriptor/d2net.py, thirdparty/d2net/lib/{model_test,pyramid,utils}.py)
  * Single scale, use_relu, 'torch' preprocessing: VGG16 conv1_1 .. conv3_3, AvgPool2d(2, stride=1), conv4_1 .. conv4_3 with
  * dilation 2 -> dense map (H/4 - 1) x (W/4 - 1) x 512; HardDetectionModule (edge threshold 5), HandcraftedLocalizationModule,
