@@ -81,6 +81,18 @@ class RansacProblem(C.Structure):  # b2_ransac_problem
                 ("threshold", C.c_double), ("mask", C.c_void_p)]
 
 
+class LinearProblem(C.Structure):  # b2_linear_problem (tests only)
+    _fields_ = [("a1", C.c_void_p), ("lda1", C.c_int), ("a2", C.c_void_p), ("lda2", C.c_int), ("b", C.c_void_p), ("ldb", C.c_int),
+                ("resid", C.c_void_p), ("ldr", C.c_int), ("c", C.c_void_p), ("ldc", C.c_int), ("c_hi", C.c_void_p), ("c_lo", C.c_void_p),
+                ("ldch", C.c_int), ("m", C.c_int), ("n", C.c_int)]
+
+
+class LinearLaunch(C.Structure):  # b2_linear_launch (tests only)
+    _fields_ = [("path", C.c_int), ("k1", C.c_int), ("k2", C.c_int), ("per_problem_b", C.c_int), ("bias", C.c_void_p),
+                ("scale", C.c_float), ("relu", C.c_int), ("gelu", C.c_int), ("head_major", C.c_int), ("lo_unscaled", C.c_int),
+                ("resid_in_place", C.c_int)]
+
+
 class RansacResult(C.Structure):  # b2_ransac_result
     _fields_ = [("status", C.c_int), ("num_inliers", C.c_int), ("model", C.c_double * 9), ("R", C.c_double * 9), ("t", C.c_double * 3)]
 
@@ -121,7 +133,7 @@ SIGNATURES = {
     "b2_profile_start": (_i, [_vp, C.c_char_p]),
     "b2_profile_stop": (_i, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.POINTER(C.c_double)]),
     "b2_debug_fetch": (C.c_int64, [_vp, C.c_char_p, _vp, C.c_int64]),
-    "b2_debug_gemm_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i]),
+    "b2_debug_linear_host": (_i, [_vp, C.POINTER(LinearLaunch), C.POINTER(LinearProblem), _i]),
     "b2_debug_gemm_segments_host": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "b2_debug_attention_host": (_i, [_vp, _i, _ip, _ip, _i, _f, _i, _vp, _vp, _vp, _vp]),
     "b2_debug_superglue_assign_host": (_i, [_vp, _i, _i, _vp, _i, _i, _f, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ip, _ip]),

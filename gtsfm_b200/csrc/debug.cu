@@ -1,5 +1,6 @@
-// Test-only entry points: run one GEMM through the SIMT fp32 kernel or the wgmma split-fp16 kernel (parity tests), the
-// wgmma kernel's column-segment / rotary epilogue, and one batched launch of the split-fp16 flash attention kernel.
+// Test-only entry points: one run_linear call on either GEMM path (the SIMT fp32 kernel or the wgmma split-fp16 kernel) in
+// any of its modes, the wgmma kernel's column-segment / rotary epilogue, and one batched launch of the split-fp16 flash
+// attention kernel.
 #include <stdlib.h>
 
 #include <vector>
@@ -13,46 +14,128 @@ static __global__ void k_split_unscaled_f32(const float* __restrict__ x, size_t 
   if (i < n) tc::split_h_unscaled(x[i], hi[i], lo[i]);
 }
 
-extern "C" int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, const float* B, const float* bias, float* C,
-                                  int M, int N, int K) {
-  if (!ctx || !A || !B || !C || M <= 0 || N <= 0 || K <= 0 || (K % 64)) return B2_ERR_ARG;
+// One fp32 operand on the device: the host values, and their hi / lo * 2^11 planes (the producing epilogues' format)
+struct DbgOperand {
+  DevBuf f, h, l;
+};
+static int dbg_upload_split(b2_context* ctx, cudaStream_t st, const float* host, size_t n, DbgOperand& o) {
+  if (n == 0) return B2_OK;
+  B2_CUDA(ctx, o.f.ensure(n * 4));
+  B2_CUDA(ctx, o.h.ensure(n * 2));
+  B2_CUDA(ctx, o.l.ensure(n * 2));
+  B2_CUDA(ctx, cudaMemcpyAsync(o.f.p, host, n * 4, cudaMemcpyHostToDevice, st));
+  B2_LAUNCH(ctx, k_split_f32, (unsigned)((n + 255) / 256), 256, 0, st, o.f.as<float>(), n, o.h.as<__half>(), o.l.as<__half>());
+  B2_CHECK_LAUNCH(ctx);
+  return B2_OK;
+}
+// A host buffer that the call copies to the device and back whole, so that values outside the written region return as
+// they went in, followed on the device by `guard` bytes of 0xFF (NaN in fp32 and fp16) that the kernel must leave alone.
+static int dbg_upload(b2_context* ctx, cudaStream_t st, const void* host, size_t bytes, size_t guard, DevBuf& d) {
+  if (bytes == 0) return B2_OK;
+  B2_CUDA(ctx, d.ensure(bytes + guard));
+  B2_CUDA(ctx, cudaMemcpyAsync(d.p, host, bytes, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemsetAsync(static_cast<unsigned char*>(d.p) + bytes, 0xFF, guard, st));
+  return B2_OK;
+}
+static int dbg_download(b2_context* ctx, cudaStream_t st, void* host, size_t bytes, size_t guard, const DevBuf& d, bool& guard_ok) {
+  std::vector<unsigned char> g(guard);
+  B2_CUDA(ctx, cudaMemcpyAsync(host, d.p, bytes, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(g.data(), static_cast<const unsigned char*>(d.p) + bytes, guard, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  for (unsigned char v : g) guard_ok = guard_ok && v == 0xFF;
+  return B2_OK;
+}
+
+extern "C" int b2_debug_linear_host(b2_context* ctx, const b2_linear_launch* L, const b2_linear_problem* P, int np) {
+  if (!ctx || !L || !P || np <= 0 || (L->path != 0 && L->path != 1) || L->k1 < 0 || L->k2 < 0) return B2_ERR_ARG;
+  const bool tc = L->path == 1, hm = L->head_major != 0;
+  if (!P[0].b || P[0].ldb < L->k1 + L->k2) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_linear_host: problem 0 needs a B operand");
+  // the kernel takes the residual's and the planes' leading dimensions once per launch: every problem must agree
+  int maxn = 0, ldr = -1, ldch = -1;
+  for (int i = 0; i < np; ++i) {
+    const b2_linear_problem& p = P[i];
+    if (p.m < 0 || p.n < 0) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_linear_host: negative m or n");
+    if (p.m == 0 || p.n == 0) continue;
+    maxn = p.n > maxn ? p.n : maxn;
+    if (!p.a1 || p.lda1 < L->k1 || (L->k2 && (!p.a2 || p.lda2 < L->k2)) || (L->per_problem_b && (!p.b || p.ldb < L->k1 + L->k2)))
+      return b2_fail(ctx, B2_ERR_ARG, "b2_debug_linear_host: a missing operand or a leading dimension below its K");
+    if (!p.c && !p.c_hi) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_linear_host: a problem without an output");
+    if (!p.c_hi != !p.c_lo) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_linear_host: planes come in pairs (c_hi and c_lo)");
+    if (!tc && (p.c_hi || !p.c)) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_linear_host: the SIMT path writes an fp32 output only");
+    if (p.c && !hm && p.ldc < p.n) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_linear_host: ldc below n");
+    if (L->resid_in_place && (!p.c || p.resid || hm))
+      return b2_fail(ctx, B2_ERR_ARG, "b2_debug_linear_host: an in-place residual needs a row-major fp32 output and no resid");
+    const int r = L->resid_in_place ? p.ldc : (p.resid ? p.ldr : -1);
+    if (r >= 0 && ((ldr >= 0 && r != ldr) || r < p.n)) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_linear_host: residual pitches differ or are below n");
+    if (r >= 0) ldr = r;
+    if (p.c_hi && !hm) {
+      if ((ldch >= 0 && p.ldch != ldch) || p.ldch < p.n) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_linear_host: plane pitches differ or are below n");
+      ldch = p.ldch;
+    }
+  }
   std::lock_guard<std::mutex> lk(ctx->mu);
   cudaSetDevice(ctx->device);
   cudaStream_t st = ctx->stream;
-  DevBuf dA, dB, dC, dBias, dErr;
-  B2_CUDA(ctx, dA.ensure((size_t)M * K * 4));
-  B2_CUDA(ctx, dB.ensure((size_t)N * K * 4));
-  B2_CUDA(ctx, dC.ensure((size_t)M * N * 4));
-  B2_CUDA(ctx, dBias.ensure((size_t)N * 4));
+  struct Bufs {
+    DbgOperand a1, a2, b;
+    DevBuf r, c, ch, cl;
+  };
+  std::vector<Bufs> d(np);
+  DevBuf dBias, dErr;
   B2_CUDA(ctx, dErr.ensure(16));
-  B2_CUDA(ctx, cudaMemcpyAsync(dA.p, A, (size_t)M * K * 4, cudaMemcpyHostToDevice, st));
-  B2_CUDA(ctx, cudaMemcpyAsync(dB.p, B, (size_t)N * K * 4, cudaMemcpyHostToDevice, st));
-  if (bias) B2_CUDA(ctx, cudaMemcpyAsync(dBias.p, bias, (size_t)N * 4, cudaMemcpyHostToDevice, st));
   B2_CUDA(ctx, cudaMemsetAsync(dErr.p, 0, 16, st));
-  if (mode == 0) {
-    const int rc = launch_gemm(ctx, st, gemm_linear(dA.as<float>(), K, K, dB.as<float>(), bias ? dBias.as<float>() : nullptr, dC.as<float>(), N, M, N));
-    if (rc != B2_OK) return rc;
-  } else {
-    // modes 1 and 2 both run the wgmma kernel on operands split here (A and B as fp16 hi / lo planes)
-    DevBuf dAh, dAl, dBh, dBl;
-    B2_CUDA(ctx, dAh.ensure((size_t)M * K * 2));
-    B2_CUDA(ctx, dAl.ensure((size_t)M * K * 2));
-    B2_CUDA(ctx, dBh.ensure((size_t)N * K * 2));
-    B2_CUDA(ctx, dBl.ensure((size_t)N * K * 2));
-    B2_LAUNCH(ctx, k_split_f32, (unsigned)(((size_t)M * K + 255) / 256), 256, 0, st, dA.as<float>(), (size_t)M * K, dAh.as<__half>(), dAl.as<__half>());
-    B2_LAUNCH(ctx, k_split_f32, (unsigned)(((size_t)N * K + 255) / 256), 256, 0, st, dB.as<float>(), (size_t)N * K, dBh.as<__half>(), dBl.as<__half>());
-    B2_CUDA(ctx, cudaFuncSetAttribute(k_gemm_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GW_SMEM));
-    TcWeights tw{nullptr, nullptr, nullptr, dErr.as<int>(), true};
-    tw.sm_count = ctx->sm_count;
-    LinArgs a;
-    a.a1p = {dAh.as<__half>(), dAl.as<__half>()}, a.lda1 = K, a.K1 = K, a.bp = {dBh.as<__half>(), dBl.as<__half>()}, a.ldb = K;
-    a.bias = bias ? dBias.as<float>() : nullptr, a.cf = dC.as<float>(), a.ldc = N, a.tc_want_f32 = true, a.M = M, a.N = N;
-    const int rc = run_linear(ctx, st, tw, &a, 1);
-    if (rc != B2_OK) return rc;
-    B2_CUDA(ctx, cudaStreamSynchronize(st));
+  if (L->bias && maxn) {
+    B2_CUDA(ctx, dBias.ensure((size_t)maxn * 4));
+    B2_CUDA(ctx, cudaMemcpyAsync(dBias.p, L->bias, (size_t)maxn * 4, cudaMemcpyHostToDevice, st));
   }
+  int rc;
+  if (!L->per_problem_b && (rc = dbg_upload_split(ctx, st, P[0].b, (size_t)maxn * P[0].ldb, d[0].b))) return rc;
+  std::vector<LinArgs> la(np);
+  for (int i = 0; i < np; ++i) {
+    const b2_linear_problem& p = P[i];
+    Bufs& q = d[i];
+    LinArgs& a = la[i];
+    // run_linear reads K and the epilogue of the launch from problem 0, which may be an empty one
+    a.K1 = L->k1, a.K2 = L->k2, a.bias = L->bias ? dBias.as<float>() : nullptr, a.scale = L->scale;
+    a.ldr = ldr > 0 ? ldr : 0, a.ldch = ldch > 0 ? ldch : 0;
+    a.head_major = L->head_major, a.relu = L->relu, a.gelu = L->gelu, a.lo_unscaled = L->lo_unscaled, a.M = p.m, a.N = p.n;
+    if (!L->per_problem_b) a.w = d[0].b.f.as<float>(), a.ldb = P[0].ldb;  // the weight of the launch, its planes through TcWeights
+    if (p.m == 0 || p.n == 0) continue;  // run_linear skips the problem
+    const size_t m = (size_t)p.m, hm_elems = (size_t)cdiv(p.n, 64) * m * 64;
+    if ((rc = dbg_upload_split(ctx, st, p.a1, m * p.lda1, q.a1))) return rc;
+    if (L->k2 && (rc = dbg_upload_split(ctx, st, p.a2, m * p.lda2, q.a2))) return rc;
+    if (L->per_problem_b && (rc = dbg_upload_split(ctx, st, p.b, (size_t)p.n * p.ldb, q.b))) return rc;
+    if (p.resid && (rc = dbg_upload(ctx, st, p.resid, m * p.ldr * 4, 0, q.r))) return rc;
+    if (p.c && (rc = dbg_upload(ctx, st, p.c, (hm ? hm_elems : m * p.ldc) * 4, (size_t)GW_M * (hm ? 64 : p.ldc) * 4, q.c))) return rc;
+    if (p.c_hi) {
+      const size_t e = hm ? hm_elems : m * p.ldch, g = (size_t)GW_M * (hm ? 64 : p.ldch) * 2;
+      if ((rc = dbg_upload(ctx, st, p.c_hi, e * 2, g, q.ch)) || (rc = dbg_upload(ctx, st, p.c_lo, e * 2, g, q.cl))) return rc;
+    }
+    a.a1f = q.a1.f.as<float>(), a.a1p = {q.a1.h.as<__half>(), q.a1.l.as<__half>()}, a.lda1 = p.lda1;
+    if (L->k2) a.a2f = q.a2.f.as<float>(), a.a2p = {q.a2.h.as<__half>(), q.a2.l.as<__half>()}, a.lda2 = p.lda2;
+    if (L->per_problem_b) a.bf = q.b.f.as<float>(), a.bp = {q.b.h.as<__half>(), q.b.l.as<__half>()}, a.ldb = p.ldb;
+    a.resid = L->resid_in_place ? q.c.as<float>() : (p.resid ? q.r.as<float>() : nullptr);
+    a.cf = p.c ? q.c.as<float>() : nullptr, a.ldc = p.ldc, a.tc_want_f32 = p.c != nullptr;
+    a.cp = {q.ch.as<__half>(), q.cl.as<__half>()};
+  }
+  if (tc) B2_CUDA(ctx, cudaFuncSetAttribute(k_gemm_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GW_SMEM));
+  TcWeights tw{d[0].b.f.as<float>(), d[0].b.h.as<__half>(), d[0].b.l.as<__half>(), dErr.as<int>(), tc};
+  tw.sm_count = ctx->sm_count;
+  if ((rc = run_linear(ctx, st, tw, la.data(), np))) return rc;
+  bool guard_ok = true;
+  for (int i = 0; i < np; ++i) {
+    const b2_linear_problem& p = P[i];
+    const Bufs& q = d[i];
+    if (p.m == 0 || p.n == 0) continue;
+    const size_t m = (size_t)p.m, e = hm ? (size_t)cdiv(p.n, 64) * m * 64 : 0;
+    if (p.c && (rc = dbg_download(ctx, st, p.c, (hm ? e : m * p.ldc) * 4, (size_t)GW_M * (hm ? 64 : p.ldc) * 4, q.c, guard_ok))) return rc;
+    if (p.c_hi) {
+      const size_t eh = hm ? e : m * p.ldch, g = (size_t)GW_M * (hm ? 64 : p.ldch) * 2;
+      if ((rc = dbg_download(ctx, st, p.c_hi, eh * 2, g, q.ch, guard_ok)) || (rc = dbg_download(ctx, st, p.c_lo, eh * 2, g, q.cl, guard_ok))) return rc;
+    }
+  }
+  if (!guard_ok) return b2_fail(ctx, B2_ERR_STATE, "b2_debug_linear_host: the kernel wrote past row m of an output");
   int err = 0;
-  B2_CUDA(ctx, cudaMemcpyAsync(C, dC.p, (size_t)M * N * 4, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaMemcpyAsync(&err, dErr.p, 4, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
   if (err) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");

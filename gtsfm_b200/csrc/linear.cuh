@@ -81,6 +81,13 @@ static int run_linear(b2_context* ctx, cudaStream_t st, const TcWeights& tw, con
       const LinArgs& x = a[i];
       if (x.M <= 0 || x.N <= 0) continue;
       if (x.gelu) return b2_fail(ctx, B2_ERR_ARG, "run_linear: the GELU epilogue exists on the wgmma path only");
+      // k_gemm_nt loads float4 operands in K steps of GB_K: a ragged K would read past the end of a row
+      if (x.K1 % GB_K || x.K2 % GB_K || x.lda1 % 4 || x.lda2 % 4 || x.ldb % 4)
+        return b2_fail(ctx, B2_ERR_ARG, "run_linear: the SIMT GEMM needs K1, K2 multiples of 16 and lda1, lda2, ldb multiples of 4");
+    }
+    for (int i = 0; i < np; ++i) {
+      const LinArgs& x = a[i];
+      if (x.M <= 0 || x.N <= 0) continue;
       for (int s = 0; s < nseg; ++s) {  // a segmented linear runs one launch per segment here
         const int c0 = s * x.seg_n;
         GemmArgs g{};
@@ -95,6 +102,8 @@ static int run_linear(b2_context* ctx, cudaStream_t st, const TcWeights& tw, con
     }
     return B2_OK;
   }
+  // k_gemm_ws walks (K1 + K2) / GW_K whole chunks and switches to A2 at a chunk boundary: a ragged K would be dropped
+  if (a0.K1 % GW_K || a0.K2 % GW_K) return b2_fail(ctx, B2_ERR_ARG, "run_linear: the wgmma GEMM needs K1 and K2 multiples of 64");
   if (!tma_encoder()) return b2_fail(ctx, B2_ERR_CUDA, "cuTensorMapEncodeTiled is not available (driver too old?)");
   const bool per_b = a0.w == nullptr;
   static thread_local GemmWsMaps maps;  // 12 KB: keep it off the stack of deep call chains

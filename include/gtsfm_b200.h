@@ -67,10 +67,33 @@ int b2_profile_stop(b2_context* ctx, double* total_ms, uint64_t* launches, doubl
 /* Copies a named intermediate device buffer of the last call to host (tests only). Returns #floats written or <0. */
 int64_t b2_debug_fetch(b2_context* ctx, const char* name, float* host_out, int64_t max_floats);
 
-/* Test-only: C[M,N] = A[M,K] * B[N,K]^T (+ bias) on HOST fp32 buffers.  mode 0 = SIMT fp32 kernel, 1 = wgmma split-fp16
- * kernel with fp32 B converted in-kernel, 2 = wgmma split-fp16 kernel with pre-split fp16 B.  K must be a multiple of 64. */
-int b2_debug_gemm_host(b2_context* ctx, int mode, const float* A, const float* B, const float* bias, float* C, int M, int N,
-                       int K);
+/* Test-only: one call of the library's shared linear (the GEMM every network runs on) over np <= 16 problems on HOST fp32
+ * buffers, C_z = ((([A1_z | A2_z] B_z^T) + bias) * scale, then ReLU or exact GELU) + resid_z.  path 1 runs the wgmma split-fp16
+ * kernel (K1, K2 multiples of 64), path 0 the exact-fp32 SIMT kernel (K1, K2 multiples of 16, lda1, lda2, ldb multiples of
+ * 4; fp32 output only, no GELU); other inputs return -2.  A, B are split into fp16 hi / lo * 2^11 planes on the device.  Device
+ * copies have the host pitches.  Each output buffer (c: m ldc floats, or ceil(n / 64) m 64 when head_major; planes: m ldch
+ * halves, or ceil(n / 64) m 64) is copied to the device before the launch and back whole after it, so values outside the
+ * written region return unchanged unless the kernel overwrote them; on the device each output is followed by 128 rows of
+ * 0xFF bytes, and the call returns -3 when the kernel wrote any of them (or its pipeline timed out).  Problems with m = 0 or
+ * n = 0 are skipped.  ldr and ldch are one per launch: problems that have them must agree. */
+typedef struct b2_linear_problem {
+  const float* a1; int lda1;                 /* [m][lda1], the first k1 columns used */
+  const float* a2; int lda2;                 /* [m][lda2], the first k2 columns used (k2 > 0) */
+  const float* b;  int ldb;                  /* [n][ldb]; problem 0's is shared unless per_problem_b */
+  const float* resid; int ldr;               /* [m][ldr] or NULL */
+  float* c; int ldc;                         /* fp32 output or NULL (wgmma path) */
+  uint16_t* c_hi; uint16_t* c_lo; int ldch;  /* fp16 plane outputs (bits) or NULL (wgmma path) */
+  int m, n;
+} b2_linear_problem;
+typedef struct b2_linear_launch {
+  int path;             /* 0 = SIMT k_gemm_nt, 1 = wgmma k_gemm_ws */
+  int k1, k2, per_problem_b;
+  const float* bias;    /* [max n] or NULL */
+  float scale;          /* 1 for none */
+  int relu, gelu, head_major, lo_unscaled;
+  int resid_in_place;   /* the device C is the residual (c's rows hold it on entry); resid must be NULL */
+} b2_linear_launch;
+int b2_debug_linear_host(b2_context* ctx, const b2_linear_launch* launch, const b2_linear_problem* problems, int np);
 /* Test-only: the wgmma GEMM's column-segment epilogue on HOST fp32 buffers.  A [M][K], B [256 nseg][K], bias [256 nseg]
  * (1 <= nseg <= 3, K a multiple of 64); output columns 256 s .. 256 s + 255 go to segment s of out_hi / out_lo, each
  * [nseg][4][M][64] fp16 bits (head-major, unscaled lo).  Segments with a rot_mask bit get rotary from cs / sn [M][32].

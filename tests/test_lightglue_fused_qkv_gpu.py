@@ -5,7 +5,11 @@
   and sums, then the split into fp16 hi and unscaled lo (hi = fp16(clamp(x)), lo = fp16(clamp(x) - hi)).
 - Cross attention: [to_qk; to_v] as one N = 512 launch must equal two separate N = 256 launches, bit for bit.
 
-M covers a single row, a ragged last row tile and the default workload's 5000 keypoints; cos / sin are random."""
+M covers a single row, half a row tile, one whole row tile, ragged last row tiles of 1 row (129, 257) and the default
+workload's 5000 keypoints; cos / sin are random.  The unfused GEMM runs through b2_debug_linear_host (one problem, fp32
+output)."""
+import ctypes
+
 import numpy as np
 import pytest
 
@@ -41,15 +45,17 @@ def _split_unscaled(x):
     return hi.view(np.uint16), lo.view(np.uint16)
 
 
-@pytest.mark.parametrize("M", [1, 129, 5000])
+@pytest.mark.parametrize("M", [1, 64, 128, 129, 257, 5000])
 def test_rotary_segments_equal_fp32_gemm_then_rotary_and_split(b200_ctx, M):
     A, B, bias = _operands(M, 3, 7 + M)
     rng = np.random.default_rng(100 + M)
     ang = rng.uniform(-np.pi, np.pi, (M, 32))
     cs, sn = np.cos(ang).astype(np.float32), np.sin(ang).astype(np.float32)
     C = np.full((M, 768), np.nan, np.float32)
-    rc = b200_ctx.lib.b2_debug_gemm_host(b200_ctx.handle, 1, _lib.ptr(A), _lib.ptr(B), _lib.ptr(bias), _lib.ptr(C), M, 768, K)
-    b200_ctx.check(rc, "b2_debug_gemm_host")
+    launch = _lib.LinearLaunch(path=1, k1=K, bias=_lib.ptr(bias).value, scale=1.0)
+    prob = _lib.LinearProblem(a1=_lib.ptr(A).value, lda1=K, b=_lib.ptr(B).value, ldb=K, c=_lib.ptr(C).value, ldc=768, m=M, n=768)
+    rc = b200_ctx.lib.b2_debug_linear_host(b200_ctx.handle, ctypes.byref(launch), ctypes.byref(prob), 1)
+    b200_ctx.check(rc, "b2_debug_linear_host")
     hi, lo = _segments(b200_ctx, A, B, bias, 3, rot_mask=3, cs=cs, sn=sn)
     for s in range(3):
         x = C[:, 256 * s:256 * (s + 1)].reshape(M, 4, 32, 2)
