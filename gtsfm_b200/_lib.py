@@ -93,6 +93,12 @@ class LinearLaunch(C.Structure):  # b2_linear_launch (tests only)
                 ("resid_in_place", C.c_int)]
 
 
+class ConvLayer(C.Structure):  # b2_conv_layer (tests only)
+    _fields_ = [("path", C.c_int), ("dilation", C.c_int), ("pool", C.c_int), ("relu", C.c_int), ("ctas", C.c_int), ("height", C.c_int),
+                ("width", C.c_int), ("cin", C.c_int), ("cout", C.c_int), ("in_", C.c_void_p), ("weight", C.c_void_p), ("bias", C.c_void_p),
+                ("out", C.c_void_p), ("out_hi", C.c_void_p), ("out_lo", C.c_void_p)]
+
+
 class RansacResult(C.Structure):  # b2_ransac_result
     _fields_ = [("status", C.c_int), ("num_inliers", C.c_int), ("model", C.c_double * 9), ("R", C.c_double * 9), ("t", C.c_double * 3)]
 
@@ -134,6 +140,7 @@ SIGNATURES = {
     "b2_profile_stop": (_i, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.POINTER(C.c_double)]),
     "b2_debug_fetch": (C.c_int64, [_vp, C.c_char_p, _vp, C.c_int64]),
     "b2_debug_linear_host": (_i, [_vp, C.POINTER(LinearLaunch), C.POINTER(LinearProblem), _i]),
+    "b2_debug_conv_host": (_i, [_vp, C.POINTER(ConvLayer)]),
     "b2_debug_gemm_segments_host": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp, _vp]),
     "b2_debug_attention_host": (_i, [_vp, _i, _ip, _ip, _i, _f, _i, _vp, _vp, _vp, _vp]),
     "b2_debug_superglue_assign_host": (_i, [_vp, _i, _i, _vp, _i, _i, _f, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ip, _ip]),
@@ -195,7 +202,6 @@ SIGNATURES = {
     "b2_d2net_set_weights": (_i, [_vp, _vp, _sz]),
     "b2_d2net_detect_batched_dev": (_i, [_vp, C.POINTER(D2NetImage), _i, _i, _i, _i, _sz, _vp]),
     "b2_d2net_detect_host": (_i, [_vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _ip, _ip]),
-    "b2_debug_conv_ps_host": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
     "b2_debug_d2net_avgpool_host": (_i, [_vp, _vp, _i, _i, _vp]),
     "b2_debug_d2net_rank_host": (_i, [_vp, _vp, _vp, _i, _i, _vp]),
     "b2_jpeg_status_string": (C.c_char_p, [_i]),

@@ -422,7 +422,7 @@ extern "C" int b2_d2net_detect_host(b2_context* ctx, const uint8_t* image, int h
   return B2_OK;
 }
 
-// ---- test-only entry points: the dilated convolution, the average pool and the ordering, each on its own ---------------------
+// ---- test-only entry points: the average pool and the ordering, each on its own ----------------------------------------------
 
 __global__ void k_d2_debug_keys(const float* __restrict__ score, const int* __restrict__ cij, int n, D2Cand* __restrict__ cand) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -431,44 +431,6 @@ __global__ void k_d2_debug_keys(const float* __restrict__ score, const int* __re
   d.key = d2_key(score[t], cij[3 * t], cij[3 * t + 1], cij[3 * t + 2]);
   d.fi = d.fj = 0.f, d.pad[0] = d.pad[1] = 0;
   cand[t] = d;
-}
-
-extern "C" int b2_debug_conv_ps_host(b2_context* ctx, int dilation, const float* in, int H, int W, int Cin, int Cout, const float* weight,
-                                     const float* bias, int relu, float* out) {
-  if (!ctx || !in || !weight || !bias || !out || H <= 0 || W <= 0 || Cin % 64 || Cout % 64 || Cin <= 0 || Cout <= 0) return B2_ERR_ARG;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  if (!tma_encoder()) return b2_fail(ctx, B2_ERR_CUDA, "cuTensorMapEncodeTiled is not available");
-  cudaSetDevice(ctx->device);
-  std::vector<float> wk((size_t)Cout * 9 * Cin);
-  for (int o = 0; o < Cout; ++o)  // OIHW -> [co][tap * Cin + ci], the order conv_ps_repack gives layers >= 1
-    for (int tp = 0; tp < 9; ++tp)
-      for (int i = 0; i < Cin; ++i) wk[(size_t)o * 9 * Cin + (size_t)tp * Cin + i] = weight[((size_t)o * Cin + i) * 9 + tp];
-  const size_t nin = (size_t)H * W * Cin, nout = (size_t)H * W * Cout;
-  DevBuf tmp, wh, wl, ip, il, b, o, err;
-  const size_t big = nin > wk.size() ? nin : wk.size();
-  // ip holds both planes (hi, then lo): allocated at full size first, so the upload below does not reallocate it
-  B2_CUDA(ctx, ip.ensure(2 * nin * sizeof(__half)));
-  B2_CUDA(ctx, tmp.ensure(big * sizeof(float)));
-  B2_CUDA(ctx, conv_ps_upload_planes(wk.data(), wk.size(), wh, wl, tmp, big));
-  B2_CUDA(ctx, conv_ps_upload_planes(in, nin, ip, il, tmp, big));
-  B2_CUDA(ctx, b.ensure(Cout * sizeof(float)));
-  B2_CUDA(ctx, o.ensure(nout * sizeof(float)));
-  B2_CUDA(ctx, err.ensure(16));
-  B2_CUDA(ctx, cudaMemcpy(b.p, bias, Cout * sizeof(float), cudaMemcpyHostToDevice));
-  B2_CUDA(ctx, cudaMemset(err.p, 0, 16));
-  // the kernel reads the lo plane right after the hi one
-  B2_CUDA(ctx, cudaMemcpy(ip.as<__half>() + nin, il.p, nin * sizeof(__half), cudaMemcpyDeviceToDevice));
-  B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CP_SMEM));
-  B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CpGeom<2>::SMEM));
-  const int rc = conv_ps_run(ctx, ctx->stream, ip.as<__half>(), H, W, Cin, Cout, 0, relu, dilation, wh.as<__half>(), wl.as<__half>(), b.as<float>(),
-                             nullptr, o.as<float>(), err.as<int>(), "debug");
-  if (rc) return rc;
-  int e = 0;
-  B2_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  B2_CUDA(ctx, cudaMemcpy(&e, err.p, sizeof(int), cudaMemcpyDeviceToHost));
-  B2_CUDA(ctx, cudaMemcpy(out, o.p, nout * sizeof(float), cudaMemcpyDeviceToHost));
-  if (e) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
-  return B2_OK;
 }
 
 extern "C" int b2_debug_d2net_avgpool_host(b2_context* ctx, const float* in, int H, int W, float* out) {

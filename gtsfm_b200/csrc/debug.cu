@@ -1,11 +1,12 @@
 // Test-only entry points: one run_linear call on either GEMM path (the SIMT fp32 kernel or the wgmma split-fp16 kernel) in
-// any of its modes, the wgmma kernel's column-segment / rotary epilogue, and one batched launch of the split-fp16 flash
-// attention kernel.
+// any of its modes, one 3x3 convolution layer on either path (k_conv3x3 or k_conv_ps), the wgmma kernel's column-segment /
+// rotary epilogue, and one batched launch of the split-fp16 flash attention kernel.
 #include <stdlib.h>
 
 #include <vector>
 
 #include "common.cuh"
+#include "conv_ps.cuh"
 #include "linear.cuh"
 
 // fp32 -> fp16 hi plane and UNSCALED lo plane (the operand format of the attention kernel)
@@ -139,6 +140,88 @@ extern "C" int b2_debug_linear_host(b2_context* ctx, const b2_linear_launch* L, 
   B2_CUDA(ctx, cudaMemcpyAsync(&err, dErr.p, 4, cudaMemcpyDeviceToHost, st));
   B2_CUDA(ctx, cudaStreamSynchronize(st));
   if (err) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
+  return B2_OK;
+}
+
+extern "C" int b2_debug_conv_host(b2_context* ctx, const b2_conv_layer* L) {
+  if (!ctx || !L) return B2_ERR_ARG;
+  const b2_conv_layer& c = *L;
+  const int H = c.height, W = c.width, Cin = c.cin, Cout = c.cout;
+  const bool tc = c.path == 1, pool = c.pool != 0;
+  if (c.path != 0 && c.path != 1) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_conv_host: path must be 0 (SIMT) or 1 (wgmma)");
+  if (!c.in || !c.weight || !c.bias) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_conv_host: missing input, weight or bias");
+  if (!c.out && !c.out_hi) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_conv_host: no output");
+  if (!c.out_hi != !c.out_lo) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_conv_host: planes come in pairs (out_hi and out_lo)");
+  if (H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_conv_host: a size below 1");
+  if (pool && (H < 2 || W < 2)) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_conv_host: the pooled output would be empty");
+  // k_conv3x3 has ReLU built in, pads by 1, loads Cin in steps of CK channels and writes 64-channel blocks of fp32
+  if (!tc && (!c.relu || c.dilation != 1 || Cin % CK || Cout % 64 || c.out_hi || c.ctas))
+    return b2_fail(ctx, B2_ERR_ARG, "b2_debug_conv_host: the SIMT path needs ReLU, dilation 1, Cin a multiple of 8, Cout of 64, an fp32 "
+                                    "output only and its own grid");
+  const int OH = pool ? H / 2 : H, OW = pool ? W / 2 : W;
+  const size_t nin = (size_t)H * W * Cin, nout = (size_t)OH * OW * Cout, nw = (size_t)Cout * 9 * Cin;
+  const size_t guard = ((size_t)CP_TH * OW + CP_TW) * Cout;  // elements: a tile's rows below the output and a tile's width past them
+  // weights OIHW -> [co][tap * Cin + ci] for the implicit GEMM (conv_ps_repack's order), [tap][ci][co] for the SIMT kernel
+  std::vector<float> wk(nw);
+  for (int o = 0; o < Cout; ++o)
+    for (int i = 0; i < Cin; ++i)
+      for (int tp = 0; tp < 9; ++tp) {
+        const float v = c.weight[((size_t)o * Cin + i) * 9 + tp];
+        if (tc) wk[(size_t)o * 9 * Cin + (size_t)tp * Cin + i] = v;
+        else wk[((size_t)tp * Cin + i) * Cout + o] = v;
+      }
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  cudaStream_t st = ctx->stream;
+  DbgOperand x, w;
+  DevBuf xp, b, of, op, err;
+  int rc;
+  B2_CUDA(ctx, err.ensure(16));
+  B2_CUDA(ctx, cudaMemsetAsync(err.p, 0, 16, st));
+  B2_CUDA(ctx, b.ensure((size_t)Cout * 4));
+  B2_CUDA(ctx, cudaMemcpyAsync(b.p, c.bias, (size_t)Cout * 4, cudaMemcpyHostToDevice, st));
+  if (tc) {
+    if ((rc = dbg_upload_split(ctx, st, wk.data(), nw, w))) return rc;
+    // the input's planes in one buffer, lo after hi, as conv_ps_run reads them
+    B2_CUDA(ctx, x.f.ensure(nin * 4));
+    B2_CUDA(ctx, xp.ensure(nin * 2 * 2));
+    B2_CUDA(ctx, cudaMemcpyAsync(x.f.p, c.in, nin * 4, cudaMemcpyHostToDevice, st));
+    B2_LAUNCH(ctx, k_split_f32, (unsigned)((nin + 255) / 256), 256, 0, st, x.f.as<float>(), nin, xp.as<__half>(), xp.as<__half>() + nin);
+    B2_CHECK_LAUNCH(ctx);
+  } else {
+    if ((rc = dbg_upload(ctx, st, c.in, nin * 4, 0, x.f)) || (rc = dbg_upload(ctx, st, wk.data(), nw * 4, 0, w.f))) return rc;
+  }
+  if (c.out && (rc = dbg_upload(ctx, st, c.out, nout * 4, guard * 4, of))) return rc;
+  if (c.out_hi) {  // one buffer, lo after hi (conv_ps_run's layout), then the guard
+    B2_CUDA(ctx, op.ensure((2 * nout + guard) * 2));
+    B2_CUDA(ctx, cudaMemcpyAsync(op.p, c.out_hi, nout * 2, cudaMemcpyHostToDevice, st));
+    B2_CUDA(ctx, cudaMemcpyAsync(op.as<__half>() + nout, c.out_lo, nout * 2, cudaMemcpyHostToDevice, st));
+    B2_CUDA(ctx, cudaMemsetAsync(op.as<__half>() + 2 * nout, 0xFF, guard * 2, st));
+  }
+  if (tc) {
+    B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CP_SMEM));
+    B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CpGeom<2>::SMEM));
+    rc = conv_ps_run(ctx, st, xp.as<__half>(), H, W, Cin, Cout, pool, c.relu != 0, c.dilation, w.h.as<__half>(), w.l.as<__half>(), b.as<float>(),
+                     c.out_hi ? op.as<__half>() : nullptr, c.out ? of.as<float>() : nullptr, err.as<int>(), "debug", c.ctas);
+  } else {
+    rc = conv3x3_simt_run(ctx, st, x.f.as<float>(), w.f.as<float>(), b.as<float>(), of.as<float>(), H, W, Cin, Cout, pool);
+  }
+  if (rc) return rc;
+  bool guard_ok = true;
+  if (c.out && (rc = dbg_download(ctx, st, c.out, nout * 4, guard * 4, of, guard_ok))) return rc;
+  if (c.out_hi) {
+    std::vector<unsigned char> g(guard * 2);
+    B2_CUDA(ctx, cudaMemcpyAsync(c.out_hi, op.p, nout * 2, cudaMemcpyDeviceToHost, st));
+    B2_CUDA(ctx, cudaMemcpyAsync(c.out_lo, op.as<__half>() + nout, nout * 2, cudaMemcpyDeviceToHost, st));
+    B2_CUDA(ctx, cudaMemcpyAsync(g.data(), op.as<__half>() + 2 * nout, guard * 2, cudaMemcpyDeviceToHost, st));
+    B2_CUDA(ctx, cudaStreamSynchronize(st));
+    for (unsigned char v : g) guard_ok = guard_ok && v == 0xFF;
+  }
+  if (!guard_ok) return b2_fail(ctx, B2_ERR_STATE, "b2_debug_conv_host: the kernel wrote past the end of an output");
+  int e = 0;
+  B2_CUDA(ctx, cudaMemcpyAsync(&e, err.p, 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  if (e) return b2_fail(ctx, B2_ERR_STATE, "wgmma pipeline timed out on an mbarrier (kernel bug)");
   return B2_OK;
 }
 

@@ -148,111 +148,6 @@ __global__ void __launch_bounds__(C1A_THREADS) k_conv1a(const uint8_t* __restric
   }
 }
 
-// Generic 3x3 conv, pad 1, bias + ReLU, optional fused 2x2/2 max-pool, NHWC fp32, SIMT fp32 FMA (exact-fp32 path).
-// Block tile: 8 rows x 16 cols of pixels x 64 output channels; thread micro-tile 2x4 pixels x 4 channels.
-constexpr int CT_H = 8, CT_W = 16, CK = 8, CKP = 12;  // CKP: padded per-pixel stride in smem (floats)
-template <int POOL>
-__global__ void __launch_bounds__(256) k_conv3x3(const float* __restrict__ in, const float* __restrict__ wt,
-                                                  const float* __restrict__ bias, float* __restrict__ out, int H, int W,
-                                                  int Cin, int Cout) {
-  __shared__ __align__(16) float in_s[(CT_H + 2) * (CT_W + 2) * CKP];
-  __shared__ __align__(16) float w_s[9 * CK * 64];
-  const int t = threadIdx.x;
-  const int cg = t & 15, pg = t >> 4;
-  const int prow = (pg >> 2) * 2, pcol = (pg & 3) * 4;
-  const int y0 = blockIdx.y * CT_H, x0 = blockIdx.x * CT_W;
-  const int co0 = blockIdx.z * 64;
-  float acc[2][4][4];
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-#pragma unroll
-      for (int c = 0; c < 4; ++c) acc[i][j][c] = 0.f;
-
-  for (int c0 = 0; c0 < Cin; c0 += CK) {
-    // input patch (10 x 18 pixels x CK channels), zero padded
-    for (int i = t; i < (CT_H + 2) * (CT_W + 2) * (CK / 4); i += 256) {
-      int q = i % (CK / 4);
-      int p = i / (CK / 4);
-      int py = p / (CT_W + 2), px = p % (CT_W + 2);
-      int yy = y0 + py - 1, xx = x0 + px - 1;
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (yy >= 0 && yy < H && xx >= 0 && xx < W)
-        v = *reinterpret_cast<const float4*>(in + ((size_t)yy * W + xx) * Cin + c0 + q * 4);
-      *reinterpret_cast<float4*>(&in_s[p * CKP + q * 4]) = v;
-    }
-    // weights [tap][c0..c0+CK)[co0..co0+64)
-    for (int i = t; i < 9 * CK * 16; i += 256) {
-      int q = i & 15;
-      int k = (i >> 4) % CK;
-      int tap = i / (16 * CK);
-      *reinterpret_cast<float4*>(&w_s[(tap * CK + k) * 64 + q * 4]) =
-          *reinterpret_cast<const float4*>(wt + ((size_t)tap * Cin + c0 + k) * Cout + co0 + q * 4);
-    }
-    __syncthreads();
-#pragma unroll
-    for (int tap = 0; tap < 9; ++tap) {
-      const int dy = tap / 3, dx = tap % 3;
-#pragma unroll
-      for (int k4 = 0; k4 < CK / 4; ++k4) {
-        float4 wv[4];
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          wv[kk] = *reinterpret_cast<const float4*>(&w_s[(tap * CK + k4 * 4 + kk) * 64 + cg * 4]);
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float4 a = *reinterpret_cast<const float4*>(
-                &in_s[((prow + i + dy) * (CT_W + 2) + (pcol + j + dx)) * CKP + k4 * 4]);
-            const float av[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              acc[i][j][0] = fmaf(av[kk], wv[kk].x, acc[i][j][0]);
-              acc[i][j][1] = fmaf(av[kk], wv[kk].y, acc[i][j][1]);
-              acc[i][j][2] = fmaf(av[kk], wv[kk].z, acc[i][j][2]);
-              acc[i][j][3] = fmaf(av[kk], wv[kk].w, acc[i][j][3]);
-            }
-          }
-        }
-      }
-    }
-    __syncthreads();
-  }
-  const float4 bv = *reinterpret_cast<const float4*>(bias + co0 + cg * 4);
-  const float bb[4] = {bv.x, bv.y, bv.z, bv.w};
-  if (POOL == 0) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        int yy = y0 + prow + i, xx = x0 + pcol + j;
-        if (yy < H && xx < W) {
-          float4 o = make_float4(fmaxf(acc[i][j][0] + bb[0], 0.f), fmaxf(acc[i][j][1] + bb[1], 0.f),
-                                 fmaxf(acc[i][j][2] + bb[2], 0.f), fmaxf(acc[i][j][3] + bb[3], 0.f));
-          *reinterpret_cast<float4*>(out + ((size_t)yy * W + xx) * Cout + co0 + cg * 4) = o;
-        }
-      }
-  } else {
-    const int Ho = H >> 1, Wo = W >> 1;
-    const int yo = (y0 + prow) >> 1;
-#pragma unroll
-    for (int jp = 0; jp < 2; ++jp) {
-      int xo = ((x0 + pcol) >> 1) + jp;
-      if (yo < Ho && xo < Wo) {
-        float o[4];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          float m = fmaxf(fmaxf(acc[0][2 * jp][c], acc[0][2 * jp + 1][c]), fmaxf(acc[1][2 * jp][c], acc[1][2 * jp + 1][c]));
-          o[c] = fmaxf(m + bb[c], 0.f);  // max commutes with the monotone bias-add + ReLU
-        }
-        *reinterpret_cast<float4*>(out + ((size_t)yo * Wo + xo) * Cout + co0 + cg * 4) = make_float4(o[0], o[1], o[2], o[3]);
-      }
-    }
-  }
-}
-
 // convPb (1x1, 256 -> 65) + softmax over 65 + drop dustbin + depth-to-space (superpoint.py:162-166).
 // block = 128 threads, 16 cells.
 constexpr int PB_CELLS = 16;
@@ -604,14 +499,7 @@ __global__ void __launch_bounds__(256) k_sample_desc(const float* __restrict__ d
 
 static int sp_conv3x3(b2_context* ctx, cudaStream_t st, const float* in, int li, float* out, int H, int W, bool pool) {
   SuperPointState* s = ctx->sp;
-  dim3 grid(cdiv(W, CT_W), cdiv(H, CT_H), SP_CO[li] / 64);
-  b2_prof_work(ctx, "k_conv3x3", 2.0 * 9.0 * H * W * SP_CI[li] * SP_CO[li]);
-  if (pool)
-    B2_LAUNCH(ctx, k_conv3x3<1>, grid, 256, 0, st, in, s->w[li], s->b[li], out, H, W, SP_CI[li], SP_CO[li]);
-  else
-    B2_LAUNCH(ctx, k_conv3x3<0>, grid, 256, 0, st, in, s->w[li], s->b[li], out, H, W, SP_CI[li], SP_CO[li]);
-  B2_CHECK_LAUNCH(ctx);
-  return B2_OK;
+  return conv3x3_simt_run(ctx, st, in, s->w[li], s->b[li], out, H, W, SP_CI[li], SP_CO[li], pool);
 }
 
 // wgmma implicit-GEMM convolution on split-fp16 NHWC planes (conv_ps.cuh: persistent, halo reuse, resident weights).
@@ -644,11 +532,8 @@ static int sp_conv3x3_tc(b2_context* ctx, cudaStream_t st, const DevBuf& in, int
       ctx->debug["conv_dbg"] = {s->conv_dbg.as<float>(), (int64_t)(12 * per_layer)};
     }
   }
-  const int nblk = Cout / 64, units = cdiv(W, CP_TW) * cdiv(H, CP_TH) * nblk;
-  int grid = ctx->sm_count < units ? ctx->sm_count : units;
-  grid -= grid % nblk;  // a CTA keeps one 64-channel block of the weights resident: CTA c serves block c % nblk
   b2_prof_work(ctx, "k_conv_ps", 2.0 * 9.0 * H * W * Cin * Cout);
-  B2_LAUNCH(ctx, k_conv_ps<1>, grid, CP_THREADS, CP_SMEM, st, maps, a);
+  B2_LAUNCH(ctx, k_conv_ps<1>, conv_ps_grid(ctx->sm_count, H, W, Cout), CP_THREADS, CP_SMEM, st, maps, a);
   B2_CHECK_LAUNCH(ctx);
   return B2_OK;
 }

@@ -94,6 +94,30 @@ typedef struct b2_linear_launch {
   int resid_in_place;   /* the device C is the residual (c's rows hold it on entry); resid must be NULL */
 } b2_linear_launch;
 int b2_debug_linear_host(b2_context* ctx, const b2_linear_launch* launch, const b2_linear_problem* problems, int np);
+/* Test-only: one 3x3 convolution layer (padding = dilation) on HOST buffers, out = act(maxpool(conv(in, weight) + bias)) with the
+ * 2x2/2 max-pool (floor) optional and act = ReLU or identity.  NHWC input [height][width][cin], OIHW weight [cout][cin][3][3],
+ * bias [cout]; outputs [oh][ow][cout], (oh, ow) = (height / 2, width / 2) with pool, else (height, width).
+ *   path 1: k_conv_ps<dilation> through the launch helper SuperPoint's, NetVLAD's and D2-Net's layers share, on input and
+ *     weights split into fp16 hi / lo * 2^11 planes on the device; fp32 and / or plane outputs.  Cin or cout not a multiple of
+ *     64, or a dilation other than 1 or 2, returns -2 from that helper.  ctas = 0 launches the grid the networks launch,
+ *     otherwise exactly ctas CTAs, a multiple of cout / 64 (else -2).
+ *   path 0: the exact-fp32 SIMT k_conv3x3<pool> (SuperPoint under force_simt): relu = 1, dilation 1, cin a multiple of 8, cout
+ *     of 64, an fp32 output only and ctas = 0, otherwise -2.
+ * No output, a pool with height or width below 2, or a size below 1 return -2.  Each output is copied to the device and back
+ * whole, so a value the kernel does not write returns as it went in; on the device it is followed by 0xFF guard bytes (the
+ * planes: one buffer, lo after hi, then the guard), and the call returns -3 when the kernel wrote any of them (or its pipeline
+ * timed out). */
+typedef struct b2_conv_layer {
+  int path;                             /* 1 = wgmma k_conv_ps, 0 = SIMT k_conv3x3 */
+  int dilation, pool, relu, ctas;
+  int height, width, cin, cout;
+  const float* in;                      /* [height][width][cin] */
+  const float* weight;                  /* [cout][cin][3][3] */
+  const float* bias;                    /* [cout] */
+  float* out;                           /* [oh][ow][cout] or NULL */
+  uint16_t* out_hi; uint16_t* out_lo;   /* fp16 bits [oh][ow][cout] each, or NULL (path 1) */
+} b2_conv_layer;
+int b2_debug_conv_host(b2_context* ctx, const b2_conv_layer* layer);
 /* Test-only: the wgmma GEMM's column-segment epilogue on HOST fp32 buffers.  A [M][K], B [256 nseg][K], bias [256 nseg]
  * (1 <= nseg <= 3, K a multiple of 64); output columns 256 s .. 256 s + 255 go to segment s of out_hi / out_lo, each
  * [nseg][4][M][64] fp16 bits (head-major, unscaled lo).  Segments with a rot_mask bit get rotary from cs / sn [M][32].
@@ -577,12 +601,8 @@ int b2_d2net_detect_batched_dev(b2_context* ctx, b2_d2net_image* images, int n_i
 int b2_d2net_detect_host(b2_context* ctx, const uint8_t* image, int height, int width, int channels, int max_keypoints,
                          float* out_xy, float* out_scores, float* out_desc, int* out_n, int* out_total);
 /* Test-only entry points (tests/test_d2net_kernels_gpu.py), HOST pointers:
- *  b2_debug_conv_ps_host: one k_conv_ps<dilation> layer (dilation 1 or 2, padding = dilation, Cin and Cout multiples of 64) on fp32 NHWC
- *    [H][W][Cin] with OIHW weights [Cout][Cin][3][3] and bias, optional ReLU -> fp32 NHWC [H][W][Cout];
  *  b2_debug_d2net_avgpool_host: the AvgPool2d(2, stride=1) kernel on fp32 NHWC [H][W][256] -> [H - 1][W - 1][256] (hi + lo planes);
  *  b2_debug_d2net_rank_host: the keypoint ordering on n candidates (score, c, i, j) -> order[r] = candidate of rank r < min(n, max_k). */
-int b2_debug_conv_ps_host(b2_context* ctx, int dilation, const float* in, int height, int width, int cin, int cout, const float* weight,
-                          const float* bias, int relu, float* out);
 int b2_debug_d2net_avgpool_host(b2_context* ctx, const float* in, int height, int width, float* out);
 int b2_debug_d2net_rank_host(b2_context* ctx, const float* scores, const int* cij, int n, int max_k, int* order);
 

@@ -161,6 +161,8 @@ def _dense_gpu(x, sd_gpu):
 
 def buffer_cost(ctx, reps):
     """One 512 -> 512 layer at the lund feature-map size (282 x 189) on both instances: device ms and TFLOP/s."""
+    import ctypes
+
     from gtsfm_b200 import _lib
 
     H, W, C = 282, 189, 512
@@ -171,11 +173,12 @@ def buffer_cost(ctx, reps):
     out = np.empty((H, W, C), np.float32)
     row = {}
     for dil in (1, 2):
-        args = (ctx.handle, dil, _lib.ptr(x), H, W, C, C, _lib.ptr(wt), _lib.ptr(b), 1, _lib.ptr(out))
-        ctx.check(ctx.lib.b2_debug_conv_ps_host(*args), "debug conv")
+        layer = _lib.ConvLayer(1, dil, 0, 1, 0, H, W, C, C, _lib.ptr(x).value, _lib.ptr(wt).value, _lib.ptr(b).value, _lib.ptr(out).value, None,
+                               None)
+        ctx.check(ctx.lib.b2_debug_conv_host(ctx.handle, ctypes.byref(layer)), "debug conv")
         ctx.profile_start(f"k_conv_ps<{dil}>")
         for _ in range(reps):
-            ctx.check(ctx.lib.b2_debug_conv_ps_host(*args), "debug conv")
+            ctx.check(ctx.lib.b2_debug_conv_host(ctx.handle, ctypes.byref(layer)), "debug conv")
         ms, _, work = ctx.profile_stop()
         row[f"dilation_{dil}"] = {"ms": round(ms / reps, 4), "tflops": round(work / reps / (ms / reps * 1e-3) / 1e12, 1),
                                   "activation_buffers": 3 if dil == 1 else 2}

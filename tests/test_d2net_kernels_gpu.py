@@ -1,8 +1,7 @@
 """GPU: the pieces of the D2-Net path on their own, through the test-only entry points, plus the device-to-device handoff to
-the two-way matcher.
+the two-way matcher.  Its convolutions (k_conv_ps<1> and the dilated k_conv_ps<2>) are tested with the other networks' in
+tests/test_conv_ps_gpu.py.
 
-* k_conv_ps<2> (3x3, dilation 2, padding 2) and k_conv_ps<1> against torch's float64 conv2d on random NHWC planes, at shapes that
-  are not multiples of the 16 x 8 tile;
 * the AvgPool2d(2, stride=1) kernel against torch's avg_pool2d;
 * the keypoint order (score descending, ties by (channel, row, column)) on candidates with many exactly equal scores;
 * extract_many's device descriptors fed to TwoWayEngine.match_batched_dev against the host matcher, and the golden descriptors
@@ -14,41 +13,6 @@ from gtsfm_b200 import _lib
 from gtsfm_b200 import synthetic as syn
 
 pytestmark = pytest.mark.gpu
-
-
-def _conv(ctx, x, w, b, dil, relu):
-    H, W, cin = x.shape
-    cout = w.shape[0]
-    out = np.empty((H, W, cout), np.float32)
-    rc = ctx.lib.b2_debug_conv_ps_host(ctx.handle, dil, _lib.ptr(np.ascontiguousarray(x)), H, W, cin, cout, _lib.ptr(np.ascontiguousarray(w)),
-                                       _lib.ptr(np.ascontiguousarray(b)), relu, _lib.ptr(out))
-    ctx.check(rc, "debug_conv_ps_host")
-    return out
-
-
-@pytest.mark.parametrize("dil,H,W,cin,cout,relu", [(2, 37, 29, 256, 512, 1), (2, 13, 21, 512, 512, 1), (2, 5, 3, 64, 128, 0),
-                                                   (2, 70, 45, 128, 64, 0), (1, 37, 29, 256, 128, 1)])
-def test_conv_ps_against_conv2d(b200_ctx, dil, H, W, cin, cout, relu):
-    import torch
-    import torch.nn.functional as F
-
-    rng = np.random.default_rng(H * 1000 + W + dil)
-    x = np.maximum(rng.standard_normal((H, W, cin)), 0).astype(np.float32)  # post-ReLU activations, as in the network
-    w = (rng.standard_normal((cout, cin, 3, 3)) * np.sqrt(2.0 / (9 * cin))).astype(np.float32)
-    b = (0.05 * rng.standard_normal(cout)).astype(np.float32)
-    got = _conv(b200_ctx, x, w, b, dil, relu)
-    t = lambda a: torch.from_numpy(a).double()  # noqa: E731
-    want = F.conv2d(t(x).permute(2, 0, 1)[None], t(w), t(b), padding=dil, dilation=dil)[0].permute(1, 2, 0)
-    if relu:
-        want = F.relu(want)
-    want = want.numpy()
-    # fp32 torch on the same operands: the rounding a plain float32 convolution has
-    f32 = F.conv2d(torch.from_numpy(x).permute(2, 0, 1)[None], torch.from_numpy(w), torch.from_numpy(b), padding=dil, dilation=dil)[0]
-    f32 = (F.relu(f32) if relu else f32).permute(1, 2, 0).numpy()
-    scale = np.abs(want).max()
-    err, err32 = np.abs(got - want).max() / scale, np.abs(f32 - want).max() / scale
-    print(f"dil {dil} {H}x{W} {cin}->{cout}: max err {err:.2e} of max |y| (fp32 torch {err32:.2e})")
-    assert err < 1e-5, err
 
 
 def test_avgpool_against_torch(b200_ctx):
