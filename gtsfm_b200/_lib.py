@@ -152,7 +152,6 @@ SIGNATURES = {
     "b2_superpoint_extract_dev": (_i, [_vp, _vp, _i, _i, _i, _sz, _f, _i, _i, _i, _vp, _vp, _vp, _ip, _vp]),
     "b2_superpoint_extract_async_dev": (_i, [_vp, _vp, _i, _i, _i, _sz, _f, _i, _i, _i, _vp, _vp, _vp, _vp, _vp]),
     "b2_superpoint_finish_dev": (_i, [_vp, _vp]),
-    "b2_topk_indices_dev": (_i, [_vp, _vp, _i, _i, _vp, _ip, _vp]),
     "b2_superpoint_detect_host": (_i, [_vp, _vp, _i, _i, _i, _f, _i, _i, _vp, _vp, _i, _ip, C.POINTER(C.c_uint64)]),
     "b2_superpoint_describe_host": (_i, [_vp, C.c_uint64, _vp, _i, _vp]),
     "b2_image_resize_dev": (_i, [_vp, _vp, _i, _i, _i, _sz, _vp, _i, _i, _vp]),

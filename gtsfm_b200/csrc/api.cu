@@ -68,10 +68,6 @@ extern "C" int b2_set_option(b2_context* ctx, const char* name, int64_t value) {
     ctx->rs_workspace_mb = (int)value;
     return B2_OK;
   }
-  if (!strcmp(name, "superpoint_graph")) {  // 1 (default): replay the SuperPoint network as one CUDA graph; 0: direct launches
-    ctx->sp_graph = value ? 1 : 0;
-    return B2_OK;
-  }
   if (!strcmp(name, "force_simt")) {  // takes effect for models whose weights are set AFTER this call
     ctx->force_simt = value ? 1 : 0;
     return B2_OK;

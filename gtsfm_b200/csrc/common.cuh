@@ -123,7 +123,6 @@ struct b2_context {
   int sm_count = 132;
   int reserve_sms = 0;  // SMs the persistent kernels of this context leave free (b2_set_option "reserve_sms")
   int lg_batch = 0;     // pairs per LightGlue batch (0 = the library maximum, 8); b2_set_option "lightglue_batch"
-  int sp_graph = -1;    // SuperPoint network as a CUDA graph: 1 / 0, -1 = B2_SP_GRAPH env (default off)
   int rs_workspace_mb = 1024;  // RANSAC workspace budget per sub-batch of a batched call; b2_set_option "ransac_workspace_mb"
   int force_simt = -1;  // 1: models loaded afterwards run the exact-fp32 SIMT kernels (no tensor cores); -1 = B2_FORCE_SIMT env
   std::string err;

@@ -63,7 +63,6 @@ struct ConvPsArgs {
   __half *Oh, *Ol;    // optional output planes NHWC
   float* Of;          // optional fp32 output NHWC
   int* err_flag;
-  float* dbg;  // optional [gridDim.x][8] timestamps (globaltimer ns & 0xFFFFFF), profiling runs only
 };
 
 namespace tc {
@@ -74,13 +73,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst_smem, const CUtensorMap
       : "memory");
 }
 }  // namespace tc
-
-__device__ __forceinline__ void cp_stamp(float* dbg, int slot) {
-  if (!dbg) return;
-  unsigned long long tns;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(tns));
-  dbg[blockIdx.x * 8 + slot] = (float)(tns & 0xFFFFFFull);
-}
 
 template <int D = 1>
 static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_constant__ ConvPsMaps maps, ConvPsArgs g) {
@@ -104,7 +96,6 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
   const int nt = lane_id < ntiles ? (ntiles - lane_id + stride - 1) / stride : 0;  // this CTA's tiles: lane_id + k * stride
 
   if (t == 0) {
-    cp_stamp(g.dbg, 0);
     for (int i = 0; i < NA; ++i) tc::mbar_init(&fullA[i], 1), tc::mbar_init(&emptyA[i], 8);
     for (int i = 0; i < 9; ++i) tc::mbar_init(&fullB[i], 1), tc::mbar_init(&emptyB[i], 8);
     tc::fence_mbar_init();
@@ -115,7 +106,6 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
   }
   __syncthreads();
   bool ok = true;
-  if (t == 0) cp_stamp(g.dbg, 1), g.dbg ? (void)(g.dbg[blockIdx.x * 8 + 7] = (float)nt) : (void)0;
 
   if (warp == 8) {
     if (lane == 0) {
@@ -159,7 +149,6 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
           const uint32_t buf = a_cnt % NA;
           ok = tc::mbar_wait(&fullA[buf], (a_cnt / NA) & 1) && ok;
           const uint32_t base = sA + buf * A_BYTES;
-          if (a_cnt == 0 && t == 0) cp_stamp(g.dbg, 2);
 #pragma unroll 1
           for (int tap = 0; tap < 9; ++tap) {
             if (new_b) ok = tc::mbar_wait(&fullB[tap], (bver - 1) & 1) && ok;
@@ -200,7 +189,6 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
           ++a_cnt;
         }
       }
-      if (k == 0 && t == 0) cp_stamp(g.dbg, 3);
       // ---- epilogue: v[4j + 2i + e] = pixel (h0 + i, wc), channel 8j + c2 + e ----
       float v[32];
 #pragma unroll
@@ -255,12 +243,10 @@ static __global__ void __launch_bounds__(CP_THREADS, 1) k_conv_ps(const __grid_c
           }
         }
       }
-      if (k == nt - 1 && t == 0) cp_stamp(g.dbg, 5);
     }
   }
   if (!ok && g.err_flag) *g.err_flag = 1;
   __syncthreads();
-  if (t == 0) cp_stamp(g.dbg, 6);
 }
 
 // NHWC fp16 activation plane [H][W][C] -> 3-D map {C, W, H}, box {64, 8 + 2 dil, 16 + 2 dil}, 128-byte swizzle, zero OOB fill
@@ -275,7 +261,7 @@ static inline bool tma_map_nhwc_halo(CUtensorMap* out, const __half* base, int H
              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// ---- host helpers shared by the VGG-style networks on this kernel (NetVLAD, D2-Net) ----------------------------------------
+// ---- host helpers shared by the networks on this kernel (SuperPoint, NetVLAD, D2-Net) --------------------------------------
 
 // Walks n layers of (OIHW 3x3 weight, bias) from `blob`: layer 0 (3 input channels, run by a SIMT kernel) -> w0 fp32
 // [tap][ci][co]; layers >= 1 -> `stage` at woff[l] as [co][tap * Cin + ci] (the implicit GEMM's K order); biases concatenated
@@ -331,24 +317,39 @@ static inline int conv_ps_grid(int sm_count, int H, int W, int Cout) {
   return grid - grid % nblk;
 }
 
+// One layer's tensor maps, kept by a caller that runs the same layer on the same buffers call after call (SuperPoint: four
+// host-side encodes per layer and image otherwise).  The key is everything the maps depend on.
+struct ConvPsMapCache {
+  ConvPsMaps maps;
+  const __half *ih = nullptr, *wh = nullptr, *wl = nullptr;
+  int H = 0, W = 0, Cin = 0, Cout = 0, dil = 0;
+};
+
 // One layer on k_conv_ps<dil> (dil = padding, 1 or 2): input planes `ih` [H][W][Cin] with the lo plane right after the hi one,
 // weight planes wh / wl [Cout][9 Cin] -> output planes `oh` (lo after hi) and / or fp32 `of`, NHWC.  ctas = 0 launches
-// conv_ps_grid's grid, otherwise exactly `ctas` CTAs (a multiple of Cout / 64).  The caller has set the kernel's dynamic
-// shared-memory attribute (CP_SMEM / CpGeom<2>::SMEM).
+// conv_ps_grid's grid, otherwise exactly `ctas` CTAs (a multiple of Cout / 64).  `cache` = NULL encodes the maps on every
+// call, otherwise only when its key differs.  The caller has set the kernel's dynamic shared-memory attribute (CP_SMEM /
+// CpGeom<2>::SMEM).
 static int conv_ps_run(b2_context* ctx, cudaStream_t st, const __half* ih, int H, int W, int Cin, int Cout, int pool, int relu, int dil,
                        const __half* wh, const __half* wl, const float* bias, __half* oh, float* of, int* err_flag, const char* model,
-                       int ctas = 0) {
+                       int ctas = 0, ConvPsMapCache* cache = nullptr) {
   if (dil != 1 && dil != 2) return b2_fail(ctx, B2_ERR_ARG, "conv_ps: dilation must be 1 or 2");
   // the kernel walks Cin / 64 whole chunks and Cout / 64 channel blocks: a remainder would be dropped
   if (Cin <= 0 || Cout <= 0 || Cin % 64 || Cout % 64 || H <= 0 || W <= 0)
     return b2_fail(ctx, B2_ERR_ARG, "conv_ps: Cin and Cout must be positive multiples of 64, H and W positive");
   if (ctas < 0 || ctas % (Cout / 64)) return b2_fail(ctx, B2_ERR_ARG, "conv_ps: the grid must be a multiple of Cout / 64");
   const int OH = pool ? H / 2 : H, OW = pool ? W / 2 : W;
-  ConvPsMaps maps;
-  const __half* il = ih + (size_t)H * W * Cin;
-  bool ok = tma_map_nhwc_halo(&maps.ah, ih, H, W, Cin, dil) && tma_map_nhwc_halo(&maps.al, il, H, W, Cin, dil) &&
-            tma_map_2d(&maps.wh, wh, Cout, 9 * Cin, 9 * Cin, 64) && tma_map_2d(&maps.wl, wl, Cout, 9 * Cin, 9 * Cin, 64);
-  if (!ok) return b2_fail(ctx, B2_ERR_CUDA, std::string("cuTensorMapEncodeTiled failed (") + model + " conv)");
+  ConvPsMapCache local;
+  ConvPsMapCache& mc = cache ? *cache : local;
+  if (mc.ih != ih || mc.wh != wh || mc.wl != wl || mc.H != H || mc.W != W || mc.Cin != Cin || mc.Cout != Cout || mc.dil != dil) {
+    mc = ConvPsMapCache{};  // a failed encode leaves no key behind
+    const __half* il = ih + (size_t)H * W * Cin;
+    bool ok = tma_map_nhwc_halo(&mc.maps.ah, ih, H, W, Cin, dil) && tma_map_nhwc_halo(&mc.maps.al, il, H, W, Cin, dil) &&
+              tma_map_2d(&mc.maps.wh, wh, Cout, 9 * Cin, 9 * Cin, 64) && tma_map_2d(&mc.maps.wl, wl, Cout, 9 * Cin, 9 * Cin, 64);
+    if (!ok) return b2_fail(ctx, B2_ERR_CUDA, std::string("cuTensorMapEncodeTiled failed (") + model + " conv)");
+    mc.ih = ih, mc.wh = wh, mc.wl = wl, mc.H = H, mc.W = W, mc.Cin = Cin, mc.Cout = Cout, mc.dil = dil;
+  }
+  const ConvPsMaps& maps = mc.maps;
   ConvPsArgs a{};
   a.H = H, a.W = W, a.Cin = Cin, a.Cout = Cout, a.pool = pool, a.relu = relu, a.bias = bias;
   if (oh) a.Oh = oh, a.Ol = oh + (size_t)OH * OW * Cout;

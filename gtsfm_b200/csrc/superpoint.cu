@@ -9,8 +9,6 @@
 // segment, which is what both the implicit-GEMM K loop and the bilinear descriptor gather want); conv weights repacked
 // at load to [tap][cin][cout]; 1x1 weights to [cin][cout]; score / NMS maps (H8, W8) fp32; dense descriptors
 // (Hc, Wc, 256) fp32; keypoints as (x, y) float pairs in torch.nonzero (row-major) order.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "conv_ps.cuh"
 #include "image.cuh"
@@ -34,12 +32,8 @@ struct SuperPointState {
   float* w[SP_NCONV] = {};
   float* b[SP_NCONV] = {};
   // wgmma path: 3x3 weights as [cout][tap * cin] split-fp16 planes (B operand of the implicit GEMM)
-  DevBuf wsplit_h, wsplit_l, errflag, conv_dbg, logits;
-  struct ConvMapCache {
-    ConvPsMaps maps;
-    const void *ih = nullptr, *wh = nullptr;
-    int H = 0, W = 0;
-  } conv_maps[12];
+  DevBuf wsplit_h, wsplit_l, errflag, logits;
+  ConvPsMapCache conv_maps[SP_NCONV];  // the maps only change with the image size / a reallocation
   size_t wsoff[SP_NCONV] = {};
   bool use_tc = true;
   // workspace
@@ -49,30 +43,10 @@ struct SuperPointState {
   bool have_dense = false;
   uint64_t map_token = 0;  // identifies the dense descriptor map a detect call left behind (checked by describe)
   DevBuf sel_idx, sel_cnt; // device top-k selection of b2_superpoint_extract_dev
-  // CUDA graph of the network (sp_detect_impl)
-  static constexpr int GKEY = 20, GSLOTS = 4;
-  struct GraphSlot {
-    uint64_t key[GKEY] = {};
-    cudaGraphExec_t exec = nullptr;
-    uint64_t launches = 0;
-  } gslot[GSLOTS];
-  cudaStream_t cap_stream = nullptr;
-  int gnext = 0, gcaptures = 0;
 };
 
-static inline uint32_t __float_as_uint_host(float f) {
-  uint32_t u;
-  memcpy(&u, &f, 4);
-  return u;
-}
-
 void sp_destroy(b2_context* ctx) {
-  if (!ctx->sp) return;
-  SuperPointState* s = ctx->sp;
-  for (auto& g : s->gslot)
-    if (g.exec) cudaGraphExecDestroy(g.exec);
-  if (s->cap_stream) cudaStreamDestroy(s->cap_stream);
-  delete s;
+  delete ctx->sp;
   ctx->sp = nullptr;
 }
 
@@ -502,40 +476,14 @@ static int sp_conv3x3(b2_context* ctx, cudaStream_t st, const float* in, int li,
   return conv3x3_simt_run(ctx, st, in, s->w[li], s->b[li], out, H, W, SP_CI[li], SP_CO[li], pool);
 }
 
-// wgmma implicit-GEMM convolution on split-fp16 NHWC planes (conv_ps.cuh: persistent, halo reuse, resident weights).
+// wgmma implicit-GEMM convolution + ReLU on split-fp16 NHWC planes (conv_ps.cuh: persistent, halo reuse, resident weights).
 // `in` / `out` buffers hold the hi plane followed by the lo plane (+ pixels * channels halves).
 static int sp_conv3x3_tc(b2_context* ctx, cudaStream_t st, const DevBuf& in, int li, int H, int W, bool pool, DevBuf* out_planes,
                          float* out_f32) {
   SuperPointState* s = ctx->sp;
-  const int Cin = SP_CI[li], Cout = SP_CO[li];
-  const int OH = pool ? H / 2 : H, OW = pool ? W / 2 : W;
-  const __half* ih = in.as<__half>();
-  const __half* il = ih + (size_t)H * W * Cin;
-  const __half* wh = s->wsplit_h.as<__half>() + s->wsoff[li];
-  const __half* wl = s->wsplit_l.as<__half>() + s->wsoff[li];
-  SuperPointState::ConvMapCache& mc = s->conv_maps[li];  // the maps only change with the image size / a reallocation
-  if (mc.ih != ih || mc.wh != wh || mc.H != H || mc.W != W) {
-    bool ok = tma_map_nhwc_halo(&mc.maps.ah, ih, H, W, Cin) && tma_map_nhwc_halo(&mc.maps.al, il, H, W, Cin) &&
-              tma_map_2d(&mc.maps.wh, wh, Cout, 9 * Cin, 9 * Cin, 64) && tma_map_2d(&mc.maps.wl, wl, Cout, 9 * Cin, 9 * Cin, 64);
-    if (!ok) return b2_fail(ctx, B2_ERR_CUDA, "cuTensorMapEncodeTiled failed (conv)");
-    mc.ih = ih, mc.wh = wh, mc.H = H, mc.W = W;
-  }
-  const ConvPsMaps& maps = mc.maps;
-  ConvPsArgs a{};
-  a.H = H, a.W = W, a.Cin = Cin, a.Cout = Cout, a.pool = pool ? 1 : 0, a.relu = 1, a.bias = s->b[li];
-  if (out_planes) a.Oh = out_planes->as<__half>(), a.Ol = a.Oh + (size_t)OH * OW * Cout;
-  a.Of = out_f32, a.err_flag = s->errflag.as<int>();
-  if (getenv("B2_CONV_DBG")) {  // profiling runs: per-CTA timestamps of layer li, read back through b2_debug_fetch("conv_dbg")
-    const size_t per_layer = (size_t)ctx->sm_count * 8;
-    if (s->conv_dbg.ensure(12 * per_layer * sizeof(float)) == cudaSuccess) {
-      a.dbg = s->conv_dbg.as<float>() + li * per_layer;
-      ctx->debug["conv_dbg"] = {s->conv_dbg.as<float>(), (int64_t)(12 * per_layer)};
-    }
-  }
-  b2_prof_work(ctx, "k_conv_ps", 2.0 * 9.0 * H * W * Cin * Cout);
-  B2_LAUNCH(ctx, k_conv_ps<1>, conv_ps_grid(ctx->sm_count, H, W, Cout), CP_THREADS, CP_SMEM, st, maps, a);
-  B2_CHECK_LAUNCH(ctx);
-  return B2_OK;
+  return conv_ps_run(ctx, st, in.as<__half>(), H, W, SP_CI[li], SP_CO[li], pool, 1, 1, s->wsplit_h.as<__half>() + s->wsoff[li],
+                     s->wsplit_l.as<__half>() + s->wsoff[li], s->b[li], out_planes ? out_planes->as<__half>() : nullptr, out_f32,
+                     s->errflag.as<int>(), "superpoint", 0, &s->conv_maps[li]);
 }
 
 // 1x1 head (convPb / convDb) on the shared wgmma GEMM: out[cell][n] = sum_k in[cell][k] * W[n][k] + bias[n]  (fp32-equivalent)
@@ -623,15 +571,9 @@ extern "C" int b2_superpoint_set_weights(b2_context* ctx, const float* blob, siz
     }
     DevBuf tmp;
     B2_CUDA(ctx, tmp.ensure(tot * sizeof(float)));
-    B2_CUDA(ctx, s->wsplit_h.ensure(tot * sizeof(__half)));
-    B2_CUDA(ctx, s->wsplit_l.ensure(tot * sizeof(__half)));
+    B2_CUDA(ctx, conv_ps_upload_planes(stage.data(), tot, s->wsplit_h, s->wsplit_l, tmp, tot));
     B2_CUDA(ctx, s->errflag.ensure(16));
     B2_CUDA(ctx, cudaMemset(s->errflag.p, 0, 16));
-    B2_CUDA(ctx, cudaMemcpy(tmp.p, stage.data(), tot * sizeof(float), cudaMemcpyHostToDevice));
-    B2_LAUNCH(ctx, k_split_f32, (unsigned)((tot + 255) / 256), 256, 0, (cudaStream_t)0, tmp.as<float>(), tot, s->wsplit_h.as<__half>(),
-              s->wsplit_l.as<__half>());
-    B2_CHECK_LAUNCH(ctx);
-    B2_CUDA(ctx, cudaDeviceSynchronize());
     B2_CUDA(ctx, cudaFuncSetAttribute(k_conv_ps<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CP_SMEM));
     B2_CUDA(ctx, cudaFuncSetAttribute(k_gemm_ws, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)GW_SMEM));
     s->use_tc = !b2_force_simt(ctx) && tma_encoder() != nullptr;
@@ -642,8 +584,7 @@ extern "C" int b2_superpoint_set_weights(b2_context* ctx, const float* blob, siz
 }
 
 // Everything between the grey image and the compacted keypoint list + dense descriptor map, enqueued on `st`.  Buffers are
-// sized by the caller; the sequence is a pure function of (H, W, thr, border, cap, output pointers), which is what lets
-// sp_detect_impl replay it as a CUDA graph.
+// sized by the caller.
 static int sp_enqueue_network(b2_context* ctx, cudaStream_t st, int H, int W, float thr, int border, float* out_xy, float* out_score, int cap) {
   SuperPointState* s = ctx->sp;
   const int H2 = H / 2, W2 = W / 2, H4 = H2 / 2, W4 = W2 / 2, Hc = H4 / 2, Wc = W4 / 2;
@@ -713,16 +654,6 @@ static int sp_enqueue_network(b2_context* ctx, cudaStream_t st, int H, int W, fl
   return B2_OK;
 }
 
-// true when bench.py is timing (CUDA events per launch) a kernel that sp_enqueue_network launches: events cannot be placed
-// inside a replayed graph, so those runs launch directly
-static bool sp_prof_in_network(const ProfState& p) {
-  if (!p.on) return false;
-  static const char* const names[] = {"k_conv1a", "k_conv_ps", "k_gemm_ws", "k_head_softmax", "k_head_l2norm", "k_nms", "k_scan_rows", "k_compact"};
-  for (const char* n : names)
-    if (strncmp(n, p.name.c_str(), p.name.size()) == 0) return true;
-  return false;
-}
-
 static int sp_detect_impl(b2_context* ctx, const uint8_t* image, int H, int W, int channels, size_t pitch, float thr,
                           int nms_radius, int border, float* out_xy, float* out_score, int cap, int* out_n,
                           cudaStream_t st, uint64_t* out_token = nullptr, bool defer_sync = false) {
@@ -748,11 +679,6 @@ static int sp_detect_impl(b2_context* ctx, const uint8_t* image, int H, int W, i
   B2_CUDA(ctx, s->rowcnt.ensure((size_t)(H8 + 1) * sizeof(int)));
   B2_CUDA(ctx, s->rowoff.ensure((size_t)(H8 + 2) * sizeof(int)));
   B2_CUDA(ctx, s->dense.ensure((size_t)Hc * Wc * 256 * sizeof(float)));
-  float* a0 = s->a0.as<float>();
-  float* a1 = s->a1.as<float>();
-  float* feat = s->feat.as<float>();
-  float* head = s->head.as<float>();
-
   const bool tcp = s->use_tc;
   if (tcp) {
     B2_CUDA(ctx, s->kpxy.ensure((size_t)Hc * Wc * 128 * sizeof(float)));
@@ -760,65 +686,7 @@ static int sp_detect_impl(b2_context* ctx, const uint8_t* image, int H, int W, i
   }
   B2_LAUNCH(ctx, k_to_gray, dim3(cdiv(W, 256), H), 256, 0, st, image, pitch, channels, H, W, s->gray.as<uint8_t>());
   B2_CHECK_LAUNCH(ctx);
-  // OPT-IN (b2_set_option "superpoint_graph" / B2_SP_GRAPH=1): the network's ~21 launches replayed as ONE CUDA graph per (shape,
-  // parameters, buffers) key, captured on a private stream the first time the key is seen.  The host
-  // enqueues faster than the GPU drains, so there is no launch gap for a graph to remove.  Direct launches when one of its kernels is being profiled, on the SIMT path, with
-  // B2_SP_GRAPH=0, or when the key keeps changing (caller-owned output pointers that move on every call).
-  int rc;
-  SuperPointState::GraphSlot* hit = nullptr;
-  bool use_graph = tcp && !sp_prof_in_network(ctx->prof) && !getenv("B2_CONV_DBG");
-  if (use_graph) {
-    if (ctx->sp_graph >= 0) {
-      use_graph = ctx->sp_graph != 0;
-    } else {
-      const char* e = getenv("B2_SP_GRAPH");
-      use_graph = e && e[0] == '1';  // default OFF: measured slower than direct launches (the path is GPU-bound, see below)
-    }
-  }
-  if (use_graph) {
-    const uint64_t key[SuperPointState::GKEY] = {(uint64_t)H, (uint64_t)W, (uint64_t)__float_as_uint_host(thr), (uint64_t)border, (uint64_t)cap,
-        (uint64_t)(uintptr_t)out_xy, (uint64_t)(uintptr_t)out_score, (uint64_t)(uintptr_t)s->gray.p, (uint64_t)(uintptr_t)s->a0.p,
-        (uint64_t)(uintptr_t)s->a1.p, (uint64_t)(uintptr_t)s->feat.p, (uint64_t)(uintptr_t)s->head.p, (uint64_t)(uintptr_t)s->heat.p,
-        (uint64_t)(uintptr_t)s->nms.p, (uint64_t)(uintptr_t)s->rowcnt.p, (uint64_t)(uintptr_t)s->rowoff.p, (uint64_t)(uintptr_t)s->dense.p,
-        (uint64_t)(uintptr_t)s->kpxy.p, (uint64_t)(uintptr_t)s->logits.p, (uint64_t)ctx->sm_count};
-    for (auto& g : s->gslot)
-      if (g.exec && memcmp(key, g.key, sizeof(key)) == 0) hit = &g;
-    if (!hit) {
-      if (s->gcaptures >= 256) {  // keys that never repeat (caller buffers moving every call): stop paying for captures
-        use_graph = false;
-      } else {
-        if (!s->cap_stream) B2_CUDA(ctx, cudaStreamCreateWithFlags(&s->cap_stream, cudaStreamNonBlocking));
-        const uint64_t l0 = ctx->launches;
-        B2_CUDA(ctx, cudaStreamBeginCapture(s->cap_stream, cudaStreamCaptureModeThreadLocal));
-        rc = sp_enqueue_network(ctx, s->cap_stream, H, W, thr, border, out_xy, out_score, cap);
-        cudaGraph_t graph = nullptr;
-        const cudaError_t ce = cudaStreamEndCapture(s->cap_stream, &graph);
-        const uint64_t nl = ctx->launches - l0;
-        ctx->launches = l0;
-        if (rc || ce != cudaSuccess || !graph) {
-          if (graph) cudaGraphDestroy(graph);
-          cudaGetLastError();
-          return rc ? rc : b2_fail(ctx, B2_ERR_CUDA, std::string("CUDA graph capture of the SuperPoint network failed: ") + cudaGetErrorString(ce));
-        }
-        SuperPointState::GraphSlot& g = s->gslot[s->gnext];
-        s->gnext = (s->gnext + 1) % SuperPointState::GSLOTS;
-        if (g.exec) cudaGraphExecDestroy(g.exec), g.exec = nullptr;
-        const cudaError_t ie = cudaGraphInstantiate(&g.exec, graph, 0);
-        cudaGraphDestroy(graph);
-        if (ie != cudaSuccess) return b2_fail(ctx, B2_ERR_CUDA, std::string("cudaGraphInstantiate: ") + cudaGetErrorString(ie));
-        memcpy(g.key, key, sizeof(key));
-        g.launches = nl;
-        s->gcaptures++;
-        hit = &g;
-      }
-    }
-  }
-  if (use_graph) {
-    B2_CUDA(ctx, cudaGraphLaunch(hit->exec, st));
-    ctx->launches += hit->launches;
-  } else if ((rc = sp_enqueue_network(ctx, st, H, W, thr, border, out_xy, out_score, cap))) {
-    return rc;
-  }
+  if (int rc = sp_enqueue_network(ctx, st, H, W, thr, border, out_xy, out_score, cap)) return rc;
   int n = 0, err = 0;
   if (!defer_sync) {
     B2_CUDA(ctx, cudaMemcpyAsync(&n, s->rowoff.as<int>() + H8, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -916,23 +784,6 @@ __global__ void __launch_bounds__(1024) k_topk_select(const float* __restrict__ 
   if (n_dev) n = min(n, *n_dev);  // candidate count still on the device (single-sync extract): n is then the capacity bound
   b2_topk_select_cta(score, n, k, out_idx, out_count);
 }
-
-extern "C" int b2_topk_indices_dev(b2_context* ctx, const float* scores, int n, int k, int32_t* out_idx, int* out_k,
-                                   void* stream) {
-  if (!ctx || !out_k || n < 0 || k < 0 || (n > 0 && (!scores || !out_idx))) return B2_ERR_ARG;
-  *out_k = 0;
-  if (n == 0 || k == 0) return B2_OK;
-  std::lock_guard<std::mutex> lk(ctx->mu);
-  cudaSetDevice(ctx->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  B2_CUDA(ctx, ctx->stage_d[7].ensure(16));
-  B2_LAUNCH(ctx, k_topk_select, 1, 1024, 0, st, scores, n, (const int*)nullptr, k, (int*)out_idx, ctx->stage_d[7].as<int>());
-  B2_CHECK_LAUNCH(ctx);
-  B2_CUDA(ctx, cudaMemcpyAsync(out_k, ctx->stage_d[7].p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  B2_CUDA(ctx, cudaStreamSynchronize(st));
-  return B2_OK;
-}
-
 
 // ------------------------------------------------------------------------------------------------------------------
 // fused device-resident extraction for the batched path: detect -> top-k (device radix select, row-major order kept) ->

@@ -52,8 +52,6 @@ uint64_t b2_h2d_bytes(const b2_context* ctx);
  * split-fp16 ones (the on-device cross-check of the tensor-core path; tests only).
  * "ransac_workspace_mb" = 1..: device workspace one sub-batch of b2_ransac_verify_batched_dev may use (default 1024); a call with
  * more problems than fit is cut into consecutive sub-batches, which changes no result.
- * "superpoint_graph" = 0 (default) | 1: launch every kernel of the SuperPoint network directly / replay the ~21 launches as one
- * CUDA graph per (image shape, parameters, buffers) key (the path is GPU-bound, not launch-bound).
  * "feature_cache" = 0 | 1: drop every cached device copy of host feature arrays and (0, default) copy on every call like the
  * reference / (1) keep device copies keyed by (host pointer, size) and validated by a hash of the FULL contents, so arrays
  * edited in place are re-sent.  Only pays off for callers that pass the same numpy buffers repeatedly (it does nothing for
@@ -180,10 +178,6 @@ int b2_superpoint_extract_async_dev(b2_context* ctx, const uint8_t* image, int h
                                     float threshold, int nms_radius, int border, int max_keypoints, float* out_xy,
                                     float* out_score, float* out_desc, int* out_n_pinned, void* stream);
 int b2_superpoint_finish_dev(b2_context* ctx, void* stream);
-/* Device top-k by score (k largest, ties broken by lower index), result kept in row-major order; writes the selected
- * indices (int32, ascending) and returns count in *out_k (HOST).  For the batched path; the per-call plugin uses the
- * reference's host argpartition to keep its index order. */
-int b2_topk_indices_dev(b2_context* ctx, const float* scores, int n, int k, int32_t* out_idx, int* out_k, void* stream);
 
 /* Host-pointer variants (H2D / D2H inside). */
 int b2_superpoint_detect_host(b2_context* ctx, const uint8_t* image, int height, int width, int channels,

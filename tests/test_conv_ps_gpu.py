@@ -31,7 +31,7 @@ B2_ERR_ARG = -2
 
 # name: (H, W, Cin, Cout, dilation, pool, relu, outputs: "planes" | "fp32" | "both")
 CASES = {
-    # SuperPoint (sp_conv3x3_tc): every layer writes planes, conv4b planes and fp32
+    # SuperPoint (sp_conv3x3_tc, which launches through conv_ps_run): every layer writes planes, conv4b planes and fp32
     "sp_conv1b": (61, 45, 64, 64, 1, 1, 1, "planes"),
     "sp_conv2a": (300, 200, 64, 64, 1, 0, 1, "planes"),  # 475 tiles on at most 132 CTAs
     "sp_conv3a": (33, 17, 64, 128, 1, 0, 1, "planes"),

@@ -3,7 +3,7 @@ import numpy as np
 import pytest
 import torch
 
-from gtsfm_b200 import synthetic as syn
+from gtsfm_b200 import _lib, synthetic as syn
 from gtsfm_b200.correspondence_generator import B200CorrespondenceGenerator
 from gtsfm_b200.detector_descriptor import SuperPointEngine
 from gtsfm_b200.gtsfm_api import Image
@@ -81,9 +81,9 @@ def test_batched_match_equals_per_pair_and_golden(b200_ctx, golden_dir):
         assert len(stops) >= 2 or profile == "prune", "the batch should mix stopping layers"
 
 
-def test_detect_many_and_graph_replay_equal_detect(b200_ctx):
-    """The no-sync multi-image path (b2_superpoint_extract_async_dev) and the opt-in CUDA-graph replay of the network give the
-    same features as one synchronous detect per image, on mixed image sizes (graph keys) and a flat image."""
+def test_detect_many_equals_detect(b200_ctx):
+    """The no-sync multi-image path (b2_superpoint_extract_async_dev) gives the same features as one synchronous detect per
+    image, on mixed image sizes and a flat image.  The SuperPoint network has one launch path: there is no graph option."""
     sp_sd = syn.superpoint_state_dict(0)
     frames, _ = syn.synthetic_sequence(4, 240, 320)
     big, _ = syn.synthetic_sequence(2, 480, 640)
@@ -93,14 +93,11 @@ def test_detect_many_and_graph_replay_equal_detect(b200_ctx):
     ref = [fe.detect(im) for im in imgs]
     assert len(ref[1]) == 700 and 0 < len(ref[0]) <= 700
     many = fe.detect_many(imgs)
-    b200_ctx.set_option("superpoint_graph", 1)
-    try:
-        graph = [fe.detect(im) for im in imgs] + fe.detect_many(imgs)
-    finally:
-        b200_ctx.set_option("superpoint_graph", 0)
-    for r, got in zip(ref * 3, many + graph):
+    for r, got in zip(ref, many):
         assert len(got) == len(r) and got.shape == r.shape
         assert torch.equal(got.kp, r.kp) and torch.equal(got.score, r.score) and torch.equal(got.desc, r.desc)
+    with pytest.raises(_lib.B200Error, match="unknown option"):
+        b200_ctx.set_option("superpoint_graph", 1)
 
 
 def test_superglue_lanes_and_lightglue_batches_equal_sequential(b200_ctx, monkeypatch):
