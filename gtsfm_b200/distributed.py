@@ -29,15 +29,15 @@ def image_owner(position: int, world: int) -> int:
     return position % world
 
 
-def all_gather_features(kp: torch.Tensor, score: torch.Tensor, desc: torch.Tensor, counts: torch.Tensor):
-    """Each rank passes the features of the images it detected, padded to the same shapes on every rank: kp (n, k, 2), score
-    (n, k), desc (n, k, 256), counts (n,) int32 (0 for padding slots).  Returns the rank-major concatenations (world * n, ...):
-    slot r * n + j = rank r's j-th image."""
+def all_gather_features(*tensors: torch.Tensor):
+    """Each rank passes the features of the images it detected, padded to the same shapes on every rank, one slot per image:
+    e.g. kp (n, k, 2), score (n, k), desc (n, k, D) in the detector's dtype, counts (n,) int32 (0 for padding slots).  Returns
+    the rank-major concatenations (world * n, ...) in the same order: slot r * n + j = rank r's j-th image."""
     if not dist.is_initialized() or dist.get_world_size() == 1:
-        return kp, score, desc, counts
+        return tensors
     world = dist.get_world_size()
     out = []
-    for t in (kp, score, desc, counts):
+    for t in tensors:
         t = t.contiguous()
         full = torch.empty((world * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
         dist.all_gather_into_tensor(full, t)

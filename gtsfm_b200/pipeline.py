@@ -31,9 +31,10 @@ from .verifier import DEFAULT_SEED, E_MAX_ITERS, LMEDS_MAX_ITERS, RANSAC_SUCCESS
 @dataclass
 class DeviceFeatures:
     kp: torch.Tensor  # (k, 2) float32 (x, y), device
-    score: torch.Tensor  # (k,)
-    desc: torch.Tensor  # (k, 256)
+    score: torch.Tensor  # (k,) float32 response
+    desc: torch.Tensor  # (k, D) in the detector's dtype: SuperPoint f32 x 256, SIFT u8 x 128, ORB u8 x 32, D2-Net f32 x 512
     shape: Tuple[int, int]
+    scale: Optional[torch.Tensor] = None  # (k,) float32 keypoint size, for the detectors whose Keypoints carry scales (SIFT, ORB)
     # LightGlue's pair-independent layer-0 state of this image (b2_lightglue_encode_batched_dev), made on first use by
     # DeviceFrontEnd.match_batch / match_many and keyed by DeviceFrontEnd._enc_key(); freed with the features
     enc: Dict[tuple, torch.Tensor] = field(default_factory=dict, repr=False, compare=False)
@@ -284,7 +285,7 @@ class DeviceFrontEnd:
         """`match_superglue` over a list of pairs, dealt round-robin to SG_LANES lanes (library contexts configured like the front
         end's, with their own SuperGlue instance, stream and host thread each): SuperGlue runs pair by pair with many narrow
         kernels (2000-keypoint GNN layers, one-block filters), which concurrent pairs fill.  `on_pair(index, matches)` is called
-        from the lane's thread as a pair completes.  Results in input order."""
+        from the lane's thread as a pair completes, with `matches` complete on the device.  Results in input order."""
         if len(pairs) == 0:
             return []
         lanes = self._role_lanes("superglue", max(1, min(SG_LANES, len(pairs))), threaded=True)
@@ -298,6 +299,9 @@ class DeviceFrontEnd:
                     if lane.stream is not None:
                         m.record_stream(main)
                     if on_pair:
+                        # match_superglue's int64 conversion is still queued on this lane's stream: complete it before
+                        # `on_pair` can hand `m` to work on another stream (the verification lane)
+                        torch.cuda.current_stream(self.device).synchronize()
                         on_pair(i, m)
                     res.append(m)
             return res
