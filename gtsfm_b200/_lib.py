@@ -124,6 +124,24 @@ class LmedsTrace(C.Structure):  # b2_lmeds_trace (tests only)
                 ("thr", C.c_float), ("count", C.c_int)]
 
 
+class TwoViewProblem(C.Structure):  # b2_twoview_problem
+    _fields_ = [("kp1", C.c_void_p), ("kp2", C.c_void_p), ("matches", C.c_void_p), ("mask", C.c_void_p), ("k", C.c_int),
+                ("cal1", C.c_double * 3), ("cal2", C.c_double * 3), ("R", C.c_double * 9), ("t", C.c_double * 3),
+                ("out_mask", C.c_void_p), ("out_rows", C.c_void_p)]
+
+
+class TwoViewParams(C.Structure):  # b2_twoview_params
+    _fields_ = [("max_iters", C.c_int), ("min_num_inliers", C.c_int), ("min_inlier_ratio", C.c_double),
+                ("ba_reproj_error_threshold", C.c_double), ("tri_reproj_error_threshold", C.c_double),
+                ("min_triangulation_angle", C.c_double)]
+
+
+class TwoViewResult(C.Structure):  # b2_twoview_result
+    _fields_ = [("status", C.c_int), ("num_rows", C.c_int), ("num_verified", C.c_int), ("num_tracks", C.c_int),
+                ("iterations", C.c_int), ("bundle_adjusted", C.c_int), ("indeterminate", C.c_int), ("trace_len", C.c_int),
+                ("R", C.c_double * 9), ("t", C.c_double * 3), ("final_error", C.c_double)]
+
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 
@@ -186,6 +204,11 @@ SIGNATURES = {
     "b2_lmeds_workspace_bytes": (_sz, [C.POINTER(RansacProblem), C.POINTER(LmedsParams)]),
     "b2_lmeds_plan": (_i, [C.POINTER(RansacProblem), _i, C.POINTER(LmedsParams), _sz, _ip]),
     "b2_debug_lmeds_trace_host": (_i, [_vp, _i, _vp, _vp, _i, C.POINTER(LmedsParams), _i, C.POINTER(LmedsTrace), C.POINTER(RansacResult), _vp]),
+    "b2_twoview_ba_batched_dev": (_i, [_vp, C.POINTER(TwoViewProblem), _i, C.POINTER(TwoViewParams), C.POINTER(TwoViewResult), _vp]),
+    "b2_twoview_ba_workspace_bytes": (_sz, [C.POINTER(TwoViewProblem), C.POINTER(TwoViewParams)]),
+    "b2_twoview_ba_plan": (_i, [C.POINTER(TwoViewProblem), _i, C.POINTER(TwoViewParams), _sz, _ip]),
+    "b2_debug_twoview_ba_trace_host": (_i, [_vp, C.POINTER(TwoViewProblem), _i, C.POINTER(TwoViewParams), C.POINTER(TwoViewResult), _vp,
+                                            _vp]),
     "b2_ransac_sync_count": (C.c_uint64, [_vp]),
     "b2_recover_pose_host": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _ip]),
     "b2_debug_ransac_trace_host": (_i, [_vp, _i, _vp, _vp, _i, C.POINTER(RansacParams), C.POINTER(RansacTrace), _vp, _vp, _ip, _vp, _vp]),

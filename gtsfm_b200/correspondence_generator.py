@@ -219,7 +219,9 @@ class B200CorrespondenceGenerator(_Base):
 
         `verify_with = (intrinsics {image: (f, u0, v0)}, threshold_px)` additionally runs the two-view verification of this
         rank's pairs (gtsfm/two_view_estimator.py:350-481) UNDER the matching - a chunk's RANSAC is queued on the verification
-        stream the moment its matches exist - and leaves {pair: TwoViewResult} in `self.last_two_view`."""
+        stream the moment its matches exist - and leaves {pair: TwoViewResult} in `self.last_two_view`.  An optional third
+        element, a dict of B200TwoViewBatch's refinement arguments (`bundle_adjust_2view=True`, thresholds), also runs the
+        triangulation, two-view bundle adjustment and inlier support right behind each chunk's verification."""
         import time
 
         t_start = time.perf_counter()
@@ -280,14 +282,21 @@ class B200CorrespondenceGenerator(_Base):
         t_detect = time.perf_counter()
         local: Dict[Tuple[int, int], np.ndarray] = {}
         pending = []
+        refine = None
+        if verify_with is not None:
+            from .two_view import B200TwoViewBatch, submit_chunk
+            from .verifier import DEFAULT_SEED
+
+            if len(verify_with) > 2:
+                refine = B200TwoViewBatch(fe, **verify_with[2]).refine
 
         def on_chunk(idx, ms):  # a chunk of this rank's pairs whose matches are complete on the device
             if verify_with is None:
                 return
-            intr, thr = verify_with  # the chunk is verified by one batched call (pairs under 6 matches fail inside it)
+            intr, thr = verify_with[:2]  # the chunk is verified by one batched call (pairs under 6 matches fail inside it)
             prs = [mine[j] for j in idx]
             items = [(feats[i1], feats[i2], m, intr[i1], intr[i2]) for (i1, i2), m in zip(prs, ms)]
-            pending.append((prs, list(ms), fe.verify_many_async(items, thr)))
+            pending.append(submit_chunk(fe, prs, items, thr, DEFAULT_SEED, "ransac", refine))
 
         matched = self._match(fe, [(feats[i1], feats[i2]) for i1, i2 in mine], on_chunk)
         for f in feats.values():  # the matcher's per-image encodings (11.5 MB at 5000 keypoints) are not needed past matching
@@ -296,8 +305,6 @@ class B200CorrespondenceGenerator(_Base):
         for pair, m in zip(mine, matched):
             local[pair] = self._host_matches(m)
         if verify_with is not None:
-            from .two_view import B200TwoViewBatch
-
             self.last_two_view = {}
             for chunk in pending:
                 B200TwoViewBatch._collect_chunk(chunk, self.last_two_view)

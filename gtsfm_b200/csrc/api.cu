@@ -34,6 +34,7 @@ extern "C" void b2_destroy(b2_context* ctx) {
   sg_destroy(ctx);
   rs_destroy(ctx);
   lm_destroy(ctx);
+  tv_destroy(ctx);
   rt_destroy(ctx);
   nv_destroy(ctx);
   mn_destroy(ctx);

@@ -103,6 +103,7 @@ struct MegaLocState;
 struct D2NetState;
 struct JpegState;
 struct OrbState;
+struct TwoViewState;
 
 // Device copies of host feature arrays handed to the *_host matcher entry points.  GTSfM matches one image's (keypoints,
 // descriptors) against ~20-40 partners, always passing the same host arrays, so re-uploading 5 MB per image per pair is
@@ -145,6 +146,7 @@ struct b2_context {
   D2NetState* d2 = nullptr;
   JpegState* jp = nullptr;
   OrbState* ob = nullptr;
+  TwoViewState* tv = nullptr;
   // staging shared by the *_host entry points
   DevBuf stage_d[8];
   HostBuf stage_h[4];
@@ -219,6 +221,7 @@ void ml_destroy(b2_context* ctx);
 void d2_destroy(b2_context* ctx);
 void jp_destroy(b2_context* ctx);
 void ob_destroy(b2_context* ctx);
+void tv_destroy(b2_context* ctx);
 
 // shared device helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

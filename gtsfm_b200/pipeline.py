@@ -467,6 +467,74 @@ class DeviceFrontEnd:
         return out
 
 
+    def refine_many_async(self, items: Sequence[tuple], verified, options: "RefineOptions"):
+        """refine_many() queued on the verification lane behind the verification whose Future is `verified` (the lane's one
+        host thread runs them in order, on the lane's stream): -> ONE Future for the whole list."""
+        lane = self._verify_lane()
+        return lane.pool.submit(lambda: self.refine_many(items, verified.result(), options, lane.ctx, lane.stream))
+
+    def refine_many(self, items: Sequence[tuple], verified: Sequence[tuple], options: "RefineOptions",
+                    ctx: Optional[_lib.Context] = None, stream: Optional[torch.cuda.Stream] = None, trace: bool = False) -> list:
+        """The reference's triangulation, two-view bundle adjustment and inlier support (two_view_estimator.py:350-481
+        with bundle_adjust_2view) for a list of (a, b, matches, cal1, cal2) and verify_many()'s results for them, in one
+        b2_twoview_ba_batched_dev call.  -> per item (R (3, 3) | None, unit t | None, kept rows as a DEVICE (n, 2) int64
+        tensor | None, the b2_twoview_result | None); None, None, None, None for a pair whose verification failed.
+        `trace`: also the LM cost traces, [n][max_iters + 2] (the test-only entry point)."""
+        ctx = ctx or self.ctx
+        sptr = _lib.C.c_void_p(stream.cuda_stream) if stream is not None else self._stream()
+        out: list = [(None, None, None, None)] * len(items)
+        live, problems, keep = [], [], []
+        with torch.cuda.stream(stream) if stream is not None else contextlib.nullcontext():
+            for i, ((a, b, m, cal1, cal2), (E, R, t, _, mask)) in enumerate(zip(items, verified)):
+                if E is None:
+                    continue
+                m = m.contiguous()
+                rows = torch.empty((max(int(m.shape[0]), 1), 2), dtype=torch.int64, device=self.device)
+                keep.append((m, rows))
+                live.append(i)
+                p = _lib.TwoViewProblem()
+                p.kp1, p.kp2, p.matches, p.mask, p.out_rows = (_lib.ptr(x) for x in (a.kp, b.kp, m, mask, rows))
+                p.k = int(m.shape[0])
+                p.cal1[:], p.cal2[:] = [float(c) for c in cal1], [float(c) for c in cal2]
+                p.R[:], p.t[:] = [float(v) for v in np.asarray(R).ravel()], [float(v) for v in np.asarray(t).ravel()]
+                problems.append(p)
+        if not problems:
+            return (out, None) if trace else out
+        n = len(problems)
+        arr = (_lib.TwoViewProblem * n)(*problems)
+        res = (_lib.TwoViewResult * n)()
+        prm = options.params()
+        if trace:
+            tr = np.zeros((n, prm.max_iters + 2))
+            ctx.check(self.lib.b2_debug_twoview_ba_trace_host(ctx.handle, arr, n, _lib.C.byref(prm), res, _lib.ptr(tr), sptr),
+                      "debug_twoview_ba_trace_host")
+        else:
+            ctx.check(self.lib.b2_twoview_ba_batched_dev(ctx.handle, arr, n, _lib.C.byref(prm), res, sptr), "twoview_ba_batched_dev")
+        for j, (i, r) in enumerate(zip(live, res)):
+            if r.status == 0:
+                out[i] = (np.array(r.R).reshape(3, 3), np.array(r.t), keep[j][1][:r.num_rows], r)
+            else:
+                out[i] = (None, None, None, r)
+        return (out, tr) if trace else out
+
+
+@dataclass
+class RefineOptions:
+    """The two-view refinement's settings (gtsfm/two_view_estimator.py:86-99, inlier_support_processor.py, and the
+    front-end configs' triangulation options)."""
+    ba_reproj_error_threshold: float = 0.5
+    min_num_inliers_est_model: int = 15
+    min_inlier_ratio_est_model: float = 0.1
+    triangulation_reproj_error_threshold: float = float("inf")
+    min_triangulation_angle: float = 0.0
+    max_iters: int = 100
+
+    def params(self) -> "_lib.TwoViewParams":
+        return _lib.TwoViewParams(int(self.max_iters), int(self.min_num_inliers_est_model), float(self.min_inlier_ratio_est_model),
+                                  float(self.ba_reproj_error_threshold), float(self.triangulation_reproj_error_threshold),
+                                  float(self.min_triangulation_angle))
+
+
 def _check_method(method: str) -> None:
     if method not in ("ransac", "lmeds"):
         raise ValueError(f"verification method must be 'ransac' or 'lmeds', not {method!r}")

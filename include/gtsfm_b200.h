@@ -401,6 +401,62 @@ int b2_debug_ransac_trace_host(b2_context* ctx, int mode, const double* x1, cons
 int b2_debug_recover_pose_host(b2_context* ctx, const double* E, const double* x1, const double* x2, int k, double* out_cands,
                                int* out_votes, int* out_winner, double* out_R, double* out_t, int* out_num_good);
 
+/* ---- Two-view refinement (gtsfm/two_view_estimator.py:350-481 with bundle_adjust_2view) -------------------------------
+ * For each verified pair: triangulate every verified row in the cameras Pose3() / Pose3(R, t)^-1 (DLT + gtsam's point
+ * refinement, cheirality, reprojection and angle checks), bundle-adjust the two cameras (pose + Cal3Bundler f, k1, k2)
+ * and the points with gtsam's robust (Huber 1.345) two-view graph and Levenberg-Marquardt schedule, reject the pair when
+ * the Hessian at the optimum is indeterminate, keep the tracks whose reprojection errors are below the threshold in both
+ * images, and apply the inlier-support thresholds.  fp64 throughout; oracle/twoview_ba_ref.py is the NumPy statement.
+ * Cameras are distortion-free on input (k1 = k2 = 0): cal = {f, u0, v0}.  Pairs with fewer than min_num_inliers verified
+ * rows are not adjusted; their verified rows go through the inlier-support decision as they are. */
+typedef struct b2_twoview_problem {
+  const float* kp1;        /* DEVICE [n1][2] pixel coordinates of image 1 */
+  const float* kp2;        /* DEVICE [n2][2] */
+  const int64_t* matches;  /* DEVICE [k][2] putative match rows */
+  const uint8_t* mask;     /* DEVICE [k] verification's inlier mask: the verified rows */
+  int k;
+  double cal1[3];          /* f, u0, v0 */
+  double cal2[3];
+  double R[9];             /* verification's i2Ri1 (row-major) and unit i2ti1 */
+  double t[3];
+  uint8_t* out_mask;       /* DEVICE [k] or NULL: 1 for the rows of the refined v_corr_idxs */
+  int64_t* out_rows;       /* DEVICE [k][2] or NULL: those rows of `matches`, compacted in row order */
+} b2_twoview_problem;
+typedef struct b2_twoview_params {
+  int max_iters;                        /* LM iterations (the reference: 100) */
+  int min_num_inliers;                  /* 15 (InlierSupportProcessor, and the condition of two_view_estimator.py:412) */
+  double min_inlier_ratio;              /* 0.1; the ratio is the verified rows over k (the pre-BA ratio, :426) */
+  double ba_reproj_error_threshold;     /* 0.5 px */
+  double tri_reproj_error_threshold;    /* triangulation's reproj_error_threshold: inf by default, 100 in sift_front_end */
+  double min_triangulation_angle;       /* degrees, 0 by default */
+} b2_twoview_params;
+typedef struct b2_twoview_result {
+  int status;          /* 0: R, t valid and num_rows rows kept; 1: the pair fails (None, None, empty) */
+  int num_rows;        /* rows set in out_mask / written to out_rows (0 on failure) */
+  int num_verified;    /* verified rows (mask) */
+  int num_tracks;      /* verified rows that triangulated */
+  int iterations;      /* successful LM iterations */
+  int bundle_adjusted; /* num_verified >= min_num_inliers: the refinement ran */
+  int indeterminate;   /* the Hessian at the optimum had a pivot at or below 1e-10 of its diagonal entry */
+  int trace_len;       /* costs recorded by the LM (initial + one per outer iteration) */
+  double R[9];         /* refined i2Ri1 (the input pose when no track survived) */
+  double t[3];         /* refined unit i2ti1 */
+  double final_error;  /* graph error at the optimum */
+} b2_twoview_result;
+/* n pairs, each stage launched once per sub-batch (3 kernels), one synchronisation per sub-batch; results HOST [n].  A
+ * pair's result does not depend on what it is batched with.  Bad arguments return B2_ERR_ARG before any launch. */
+int b2_twoview_ba_batched_dev(b2_context* ctx, const b2_twoview_problem* problems, int n, const b2_twoview_params* params,
+                              b2_twoview_result* results, void* stream);
+/* Device workspace of one problem and the cut into sub-batches under `budget_bytes` (b2_set_option "ransac_workspace_mb"
+ * is the budget of a call), as b2_ransac_workspace_bytes / b2_ransac_plan.  Pure host functions. */
+size_t b2_twoview_ba_workspace_bytes(const b2_twoview_problem* problem, const b2_twoview_params* params);
+int b2_twoview_ba_plan(const b2_twoview_problem* problems, int n, const b2_twoview_params* params, size_t budget_bytes,
+                       int* out_first);
+/* Test-only: b2_twoview_ba_batched_dev that also returns each pair's LM cost trace: out_trace HOST [n][max_iters + 2],
+ * entries [0, trace_len) valid (the cost before the first iteration, then after each). */
+int b2_debug_twoview_ba_trace_host(b2_context* ctx, const b2_twoview_problem* problems, int n, const b2_twoview_params* params,
+                                   b2_twoview_result* results, double* out_trace, void* stream);
+
 /* ---- LMedS verifier (gtsfm/frontend/verifier/lmeds.py: cv2.findEssentialMat / findFundamentalMat with LMEDS) ----------
  * A batched device restatement of cv2's LMeDS estimator: cv::RNG subsets (seed 2^64 - 1, F subsets with collinear points
  * redrawn), max(3, RANSACUpdateNumIters(confidence, 0.45, m, max_iters)) subsets, every real root of the 5-point problem (E)
