@@ -142,6 +142,23 @@ class TwoViewResult(C.Structure):  # b2_twoview_result
                 ("R", C.c_double * 9), ("t", C.c_double * 3), ("final_error", C.c_double)]
 
 
+class TwoViewEvalProblem(C.Structure):  # b2_twoview_eval_problem
+    _fields_ = [("kp1", C.c_void_p), ("kp2", C.c_void_p), ("matches", C.c_void_p), ("mask", C.c_void_p), ("k", C.c_int),
+                ("has_pose", C.c_int), ("has_gt", C.c_int), ("pad_", C.c_int), ("R", C.c_double * 9), ("t", C.c_double * 3),
+                ("wRi1", C.c_double * 9), ("wti1", C.c_double * 3), ("wRi2", C.c_double * 9), ("wti2", C.c_double * 3),
+                ("cal1", C.c_double * 3), ("cal2", C.c_double * 3), ("out_d2", C.c_void_p), ("out_inlier", C.c_void_p)]
+
+
+class TwoViewEvalParams(C.Structure):  # b2_twoview_eval_params
+    _fields_ = [("eval_threshold_px", C.c_double)]
+
+
+class TwoViewEvalResult(C.Structure):  # b2_twoview_eval_result
+    _fields_ = [("num_rows", C.c_int), ("num_inliers_gt", C.c_int), ("no_gt", C.c_int), ("no_rows", C.c_int),
+                ("inlier_avg_reproj_error_gt", C.c_double), ("outlier_avg_reproj_error_gt", C.c_double),
+                ("R_error_deg", C.c_double), ("U_error_deg", C.c_double)]
+
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 
@@ -204,6 +221,8 @@ SIGNATURES = {
     "b2_lmeds_workspace_bytes": (_sz, [C.POINTER(RansacProblem), C.POINTER(LmedsParams)]),
     "b2_lmeds_plan": (_i, [C.POINTER(RansacProblem), _i, C.POINTER(LmedsParams), _sz, _ip]),
     "b2_debug_lmeds_trace_host": (_i, [_vp, _i, _vp, _vp, _i, C.POINTER(LmedsParams), _i, C.POINTER(LmedsTrace), C.POINTER(RansacResult), _vp]),
+    "b2_twoview_eval_batched_dev": (_i, [_vp, C.POINTER(TwoViewEvalProblem), _i, C.POINTER(TwoViewEvalParams),
+                                        C.POINTER(TwoViewEvalResult), _vp]),
     "b2_twoview_ba_batched_dev": (_i, [_vp, C.POINTER(TwoViewProblem), _i, C.POINTER(TwoViewParams), C.POINTER(TwoViewResult), _vp]),
     "b2_twoview_ba_workspace_bytes": (_sz, [C.POINTER(TwoViewProblem), C.POINTER(TwoViewParams)]),
     "b2_twoview_ba_plan": (_i, [C.POINTER(TwoViewProblem), _i, C.POINTER(TwoViewParams), _sz, _ip]),

@@ -221,7 +221,9 @@ class B200CorrespondenceGenerator(_Base):
         rank's pairs (gtsfm/two_view_estimator.py:350-481) UNDER the matching - a chunk's RANSAC is queued on the verification
         stream the moment its matches exist - and leaves {pair: TwoViewResult} in `self.last_two_view`.  An optional third
         element, a dict of B200TwoViewBatch's refinement arguments (`bundle_adjust_2view=True`, thresholds), also runs the
-        triangulation, two-view bundle adjustment and inlier support right behind each chunk's verification."""
+        triangulation, two-view bundle adjustment and inlier support right behind each chunk's verification; in it,
+        `gt_cameras` ({image: (R_wTi, t_wTi, f, u0, v0)}) and `eval_threshold_px` give the results' reports their
+        ground-truth metrics, as B200TwoViewBatch.run does."""
         import time
 
         t_start = time.perf_counter()
@@ -282,13 +284,15 @@ class B200CorrespondenceGenerator(_Base):
         t_detect = time.perf_counter()
         local: Dict[Tuple[int, int], np.ndarray] = {}
         pending = []
-        refine = None
+        refine, rep = None, None
         if verify_with is not None:
             from .two_view import B200TwoViewBatch, submit_chunk
             from .verifier import DEFAULT_SEED
 
-            if len(verify_with) > 2:
-                refine = B200TwoViewBatch(fe, **verify_with[2]).refine
+            kw = dict(verify_with[2]) if len(verify_with) > 2 else {}
+            gt_cameras, gt_scene_mesh = kw.pop("gt_cameras", None), kw.pop("gt_scene_mesh", None)
+            tvb = B200TwoViewBatch(fe, **kw)
+            refine, rep = tvb.refine, tvb.report_options(gt_cameras, gt_scene_mesh)
 
         def on_chunk(idx, ms):  # a chunk of this rank's pairs whose matches are complete on the device
             if verify_with is None:
@@ -296,7 +300,7 @@ class B200CorrespondenceGenerator(_Base):
             intr, thr = verify_with[:2]  # the chunk is verified by one batched call (pairs under 6 matches fail inside it)
             prs = [mine[j] for j in idx]
             items = [(feats[i1], feats[i2], m, intr[i1], intr[i2]) for (i1, i2), m in zip(prs, ms)]
-            pending.append(submit_chunk(fe, prs, items, thr, DEFAULT_SEED, "ransac", refine))
+            pending.append(submit_chunk(fe, prs, items, thr, DEFAULT_SEED, "ransac", refine, rep))
 
         matched = self._match(fe, [(feats[i1], feats[i2]) for i1, i2 in mine], on_chunk)
         for f in feats.values():  # the matcher's per-image encodings (11.5 MB at 5000 keypoints) are not needed past matching

@@ -35,6 +35,7 @@ extern "C" void b2_destroy(b2_context* ctx) {
   rs_destroy(ctx);
   lm_destroy(ctx);
   tv_destroy(ctx);
+  te_destroy(ctx);
   rt_destroy(ctx);
   nv_destroy(ctx);
   mn_destroy(ctx);

@@ -104,6 +104,7 @@ struct D2NetState;
 struct JpegState;
 struct OrbState;
 struct TwoViewState;
+struct TwoViewEvalState;
 
 // Device copies of host feature arrays handed to the *_host matcher entry points.  GTSfM matches one image's (keypoints,
 // descriptors) against ~20-40 partners, always passing the same host arrays, so re-uploading 5 MB per image per pair is
@@ -147,6 +148,7 @@ struct b2_context {
   JpegState* jp = nullptr;
   OrbState* ob = nullptr;
   TwoViewState* tv = nullptr;
+  TwoViewEvalState* te = nullptr;
   // staging shared by the *_host entry points
   DevBuf stage_d[8];
   HostBuf stage_h[4];
@@ -222,6 +224,7 @@ void d2_destroy(b2_context* ctx);
 void jp_destroy(b2_context* ctx);
 void ob_destroy(b2_context* ctx);
 void tv_destroy(b2_context* ctx);
+void te_destroy(b2_context* ctx);
 
 // shared device helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

@@ -224,3 +224,25 @@ if GlobalDescriptorBase is None:
         @abc.abstractmethod
         def get_preprocessing_transforms(self):
             ...
+
+
+try:  # pragma: no cover - exercised only inside a full GTSfM environment
+    from gtsfm.common.two_view_estimation_report import TwoViewEstimationReport
+except Exception:  # noqa: BLE001
+    from dataclasses import dataclass
+
+    @dataclass(frozen=False)
+    class TwoViewEstimationReport:  # mirrors gtsfm/common/two_view_estimation_report.py:13-56 (fields and defaults)
+        v_corr_idxs: np.ndarray
+        num_inliers_est_model: float
+        inlier_ratio_est_model: Optional[float] = None
+        num_inliers_gt_model: Optional[float] = None
+        inlier_ratio_gt_model: Optional[float] = None
+        v_corr_idxs_inlier_mask_gt: Optional[np.ndarray] = None
+        R_error_deg: Optional[float] = None
+        U_error_deg: Optional[float] = None
+        i2Ri1: Optional[Rot3] = None
+        i2Ui1: Optional[Unit3] = None
+        reproj_error_gt_model: Optional[np.ndarray] = None
+        inlier_avg_reproj_error_gt_model: Optional[float] = None
+        outlier_avg_reproj_error_gt_model: Optional[float] = None

@@ -474,12 +474,14 @@ class DeviceFrontEnd:
         return lane.pool.submit(lambda: self.refine_many(items, verified.result(), options, lane.ctx, lane.stream))
 
     def refine_many(self, items: Sequence[tuple], verified: Sequence[tuple], options: "RefineOptions",
-                    ctx: Optional[_lib.Context] = None, stream: Optional[torch.cuda.Stream] = None, trace: bool = False) -> list:
+                    ctx: Optional[_lib.Context] = None, stream: Optional[torch.cuda.Stream] = None, trace: bool = False,
+                    out_masks: Optional[Sequence[Optional[torch.Tensor]]] = None) -> list:
         """The reference's triangulation, two-view bundle adjustment and inlier support (two_view_estimator.py:350-481
         with bundle_adjust_2view) for a list of (a, b, matches, cal1, cal2) and verify_many()'s results for them, in one
         b2_twoview_ba_batched_dev call.  -> per item (R (3, 3) | None, unit t | None, kept rows as a DEVICE (n, 2) int64
         tensor | None, the b2_twoview_result | None); None, None, None, None for a pair whose verification failed.
-        `trace`: also the LM cost traces, [n][max_iters + 2] (the test-only entry point)."""
+        `trace`: also the LM cost traces, [n][max_iters + 2] (the test-only entry point).  `out_masks[i]`: a DEVICE (k,)
+        uint8 tensor that receives the rows bundle adjustment kept, before inlier support (the post-BA rows)."""
         ctx = ctx or self.ctx
         sptr = _lib.C.c_void_p(stream.cuda_stream) if stream is not None else self._stream()
         out: list = [(None, None, None, None)] * len(items)
@@ -494,6 +496,8 @@ class DeviceFrontEnd:
                 live.append(i)
                 p = _lib.TwoViewProblem()
                 p.kp1, p.kp2, p.matches, p.mask, p.out_rows = (_lib.ptr(x) for x in (a.kp, b.kp, m, mask, rows))
+                if out_masks is not None and out_masks[i] is not None:
+                    p.out_mask = _lib.ptr(out_masks[i])
                 p.k = int(m.shape[0])
                 p.cal1[:], p.cal2[:] = [float(c) for c in cal1], [float(c) for c in cal2]
                 p.R[:], p.t[:] = [float(v) for v in np.asarray(R).ravel()], [float(v) for v in np.asarray(t).ravel()]
@@ -516,6 +520,68 @@ class DeviceFrontEnd:
             else:
                 out[i] = (None, None, None, r)
         return (out, tr) if trace else out
+
+    def evaluate_many_async(self, units_fn, threshold_px: float = 4.0):
+        """evaluate_many() queued on the verification lane behind the work already queued there: `units_fn()` is called on
+        the lane's thread (after the verification / refinement Futures it reads are done) and returns the units.  -> ONE
+        Future for the whole list."""
+        lane = self._verify_lane()
+        return lane.pool.submit(lambda: self.evaluate_many(units_fn(), threshold_px, lane.ctx, lane.stream))
+
+    def evaluate_many(self, units: Sequence["EvalUnit"], threshold_px: float = 4.0, ctx: Optional[_lib.Context] = None,
+                      stream: Optional[torch.cuda.Stream] = None) -> list:
+        """The ground-truth metrics of the two-view reports (two_view_estimator.py:290-344) for a list of (pair, stage)
+        units in one b2_twoview_eval_batched_dev call (one launch).  -> per unit (b2_twoview_eval_result, squared Sampson
+        distances (n,) float64 HOST tensor, inlier mask (n,) uint8 HOST tensor), n the unit's rows; the tensors are empty
+        without ground truth.  The kernel writes the per-row results straight into page-locked host memory, so they are
+        on the host when the call's one synchronisation returns: no copy of their own."""
+        ctx = ctx or self.ctx
+        sptr = _lib.C.c_void_p(stream.cuda_stream) if stream is not None else self._stream()
+        if not units:
+            return []
+        ks = [int(u.matches.shape[0]) for u in units]
+        d2 = torch.empty(sum(ks) + 1, dtype=torch.float64, pin_memory=True)
+        inl = torch.empty(sum(ks) + 1, dtype=torch.uint8, pin_memory=True)
+        arr = (_lib.TwoViewEvalProblem * len(units))()
+        keep, off = [], 0
+        for p, u, k in zip(arr, units, ks):
+            m = u.matches.contiguous()
+            keep.append(m)  # alive until the C call has returned
+            p.kp1, p.kp2, p.matches, p.k = _lib.ptr(u.kp1), _lib.ptr(u.kp2), _lib.ptr(m), k
+            p.mask = _lib.ptr(u.mask) if u.mask is not None else None
+            if u.pose is not None:
+                p.has_pose = 1
+                p.R[:], p.t[:] = [float(v) for v in np.asarray(u.pose[0]).ravel()], [float(v) for v in np.asarray(u.pose[1]).ravel()]
+            if u.cam1 is not None and u.cam2 is not None:
+                p.has_gt = 1
+                for (R, t, f, u0, v0), pr, pt, pc in ((u.cam1, p.wRi1, p.wti1, p.cal1), (u.cam2, p.wRi2, p.wti2, p.cal2)):
+                    pr[:], pt[:] = [float(v) for v in np.asarray(R).ravel()], [float(v) for v in np.asarray(t).ravel()]
+                    pc[:] = [float(f), float(u0), float(v0)]
+            p.out_d2, p.out_inlier = d2.data_ptr() + 8 * off, inl.data_ptr() + off
+            off += k
+        res = (_lib.TwoViewEvalResult * len(units))()
+        prm = _lib.TwoViewEvalParams(float(threshold_px))
+        ctx.check(self.lib.b2_twoview_eval_batched_dev(ctx.handle, arr, len(units), _lib.C.byref(prm), res, sptr),
+                  "twoview_eval_batched_dev")
+        out, off = [], 0
+        for r, k in zip(res, ks):
+            n = r.num_rows if not r.no_gt else 0
+            out.append((r, d2[off:off + n], inl[off:off + n]))
+            off += k
+        return out
+
+
+@dataclass
+class EvalUnit:
+    """One (pair, stage) of the two-view reports' evaluation: the stage's rows are the rows of `matches` where `mask` is
+    set (None: every row).  `pose` = (i2Ri1, i2ti1) of the stage or None; cam = (R_wTi, t_wTi, f, u0, v0) or None."""
+    kp1: torch.Tensor
+    kp2: torch.Tensor
+    matches: torch.Tensor
+    mask: Optional[torch.Tensor]
+    pose: Optional[Tuple[np.ndarray, np.ndarray]]
+    cam1: Optional[tuple]
+    cam2: Optional[tuple]
 
 
 @dataclass

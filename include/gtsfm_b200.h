@@ -457,6 +457,52 @@ int b2_twoview_ba_plan(const b2_twoview_problem* problems, int n, const b2_twovi
 int b2_debug_twoview_ba_trace_host(b2_context* ctx, const b2_twoview_problem* problems, int n, const b2_twoview_params* params,
                                    b2_twoview_result* results, double* out_trace, void* stream);
 
+/* ---- Two-view reports: ground-truth metrics (gtsfm/two_view_estimator.py:290-344, 663-731; utils/metrics.py:38-129) ----
+ * One unit per (pair, stage): the stage's rows are the rows of `matches` where `mask` is set (NULL: every row), in row
+ * order.  With ground truth for both images (has_gt), each row gets its squared Sampson distance under the ground-truth
+ * F = K2^-T [t]x R K1^-1 of i2Ti1 = wTi2.between(wTi1) and the inlier byte d2 < eval_threshold_px^2; the inlier count,
+ * the np.nanmean of the inliers' and of the outliers' distances, and the rotation / unit-translation angles between the
+ * stage's estimate (has_pose) and the ground truth.  fp64; oracle/twoview_report_ref.py is the NumPy statement.
+ * Ground-truth cameras are distortion-free: cal = {f, u0, v0}; wRi row-major, wti the camera centre. */
+typedef struct b2_twoview_eval_problem {
+  const float* kp1;        /* DEVICE [n1][2] pixel coordinates of image 1 */
+  const float* kp2;        /* DEVICE [n2][2] */
+  const int64_t* matches;  /* DEVICE [k][2] match rows */
+  const uint8_t* mask;     /* DEVICE [k] or NULL: the rows of the stage (NULL: all k) */
+  int k;
+  int has_pose;            /* the stage has an estimate R, t */
+  int has_gt;              /* ground-truth cameras for both images */
+  int pad_;
+  double R[9];             /* the stage's i2Ri1 (row-major) and i2ti1 (normalised here) */
+  double t[3];
+  double wRi1[9];          /* ground truth wTi1, wTi2 */
+  double wti1[3];
+  double wRi2[9];
+  double wti2[3];
+  double cal1[3];          /* ground-truth f, u0, v0 */
+  double cal2[3];
+  double* out_d2;          /* device-accessible [k] or NULL (device or page-locked host memory): squared Sampson
+                              distance of the stage's j-th row */
+  uint8_t* out_inlier;     /* device-accessible [k] or NULL: its inlier byte */
+} b2_twoview_eval_problem;
+typedef struct b2_twoview_eval_params {
+  double eval_threshold_px; /* 4 in the reference's configs */
+} b2_twoview_eval_params;
+typedef struct b2_twoview_eval_result {
+  int num_rows;        /* the stage's rows */
+  int num_inliers_gt;  /* rows with d2 < thr^2 (0 without ground truth or rows) */
+  int no_gt;           /* no ground truth: the reference's mask and distances are None */
+  int no_rows;         /* no rows: likewise None */
+  double inlier_avg_reproj_error_gt;   /* NaN for an empty selection, as _masked_nanmean */
+  double outlier_avg_reproj_error_gt;
+  double R_error_deg;  /* NaN where the reference has None (no estimate or no ground truth) */
+  double U_error_deg;
+} b2_twoview_eval_result;
+/* n units, one launch and one synchronisation; results HOST [n].  A unit's result does not depend on what it is batched
+ * with.  Bad arguments return B2_ERR_ARG before any launch. */
+int b2_twoview_eval_batched_dev(b2_context* ctx, const b2_twoview_eval_problem* problems, int n, const b2_twoview_eval_params* params,
+                                b2_twoview_eval_result* results, void* stream);
+
 /* ---- LMedS verifier (gtsfm/frontend/verifier/lmeds.py: cv2.findEssentialMat / findFundamentalMat with LMEDS) ----------
  * A batched device restatement of cv2's LMeDS estimator: cv::RNG subsets (seed 2^64 - 1, F subsets with collinear points
  * redrawn), max(3, RANSACUpdateNumIters(confidence, 0.45, m, max_iters)) subsets, every real root of the 5-point problem (E)
