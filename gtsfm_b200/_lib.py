@@ -159,6 +159,12 @@ class TwoViewEvalResult(C.Structure):  # b2_twoview_eval_result
                 ("R_error_deg", C.c_double), ("U_error_deg", C.c_double)]
 
 
+class ViewGraphParams(C.Structure):  # b2_viewgraph_params
+    _fields_ = [("criterion", C.c_int), ("pad_", C.c_int), ("error_threshold_deg", C.c_double)]
+
+
+VG_MEDIAN, VG_MIN = 0, 1  # B2_VG_MEDIAN, B2_VG_MIN
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 
@@ -223,6 +229,8 @@ SIGNATURES = {
     "b2_debug_lmeds_trace_host": (_i, [_vp, _i, _vp, _vp, _i, C.POINTER(LmedsParams), _i, C.POINTER(LmedsTrace), C.POINTER(RansacResult), _vp]),
     "b2_twoview_eval_batched_dev": (_i, [_vp, C.POINTER(TwoViewEvalProblem), _i, C.POINTER(TwoViewEvalParams),
                                         C.POINTER(TwoViewEvalResult), _vp]),
+    "b2_viewgraph_cycle_filter_host": (_i, [_vp, _vp, _vp, _i, C.POINTER(ViewGraphParams), _vp, _vp, _vp, _vp]),
+    "b2_debug_viewgraph_triplets_host": (_i, [_vp, _vp, _vp, _i, C.c_int64, _vp, _vp, C.POINTER(C.c_int64), _vp]),
     "b2_twoview_ba_batched_dev": (_i, [_vp, C.POINTER(TwoViewProblem), _i, C.POINTER(TwoViewParams), C.POINTER(TwoViewResult), _vp]),
     "b2_twoview_ba_workspace_bytes": (_sz, [C.POINTER(TwoViewProblem), C.POINTER(TwoViewParams)]),
     "b2_twoview_ba_plan": (_i, [C.POINTER(TwoViewProblem), _i, C.POINTER(TwoViewParams), _sz, _ip]),

@@ -105,6 +105,7 @@ struct JpegState;
 struct OrbState;
 struct TwoViewState;
 struct TwoViewEvalState;
+struct ViewGraphState;
 
 // Device copies of host feature arrays handed to the *_host matcher entry points.  GTSfM matches one image's (keypoints,
 // descriptors) against ~20-40 partners, always passing the same host arrays, so re-uploading 5 MB per image per pair is
@@ -126,6 +127,7 @@ struct b2_context {
   int reserve_sms = 0;  // SMs the persistent kernels of this context leave free (b2_set_option "reserve_sms")
   int lg_batch = 0;     // pairs per LightGlue batch (0 = the library maximum, 8); b2_set_option "lightglue_batch"
   int rs_workspace_mb = 1024;  // RANSAC workspace budget per sub-batch of a batched call; b2_set_option "ransac_workspace_mb"
+  int vg_workspace_mb = 1024;  // view-graph filter: segment window of one chunk; b2_set_option "viewgraph_workspace_mb"
   int force_simt = -1;  // 1: models loaded afterwards run the exact-fp32 SIMT kernels (no tensor cores); -1 = B2_FORCE_SIMT env
   std::string err;
   std::mutex mu;
@@ -149,6 +151,7 @@ struct b2_context {
   OrbState* ob = nullptr;
   TwoViewState* tv = nullptr;
   TwoViewEvalState* te = nullptr;
+  ViewGraphState* vg = nullptr;
   // staging shared by the *_host entry points
   DevBuf stage_d[8];
   HostBuf stage_h[4];
@@ -225,6 +228,7 @@ void jp_destroy(b2_context* ctx);
 void ob_destroy(b2_context* ctx);
 void tv_destroy(b2_context* ctx);
 void te_destroy(b2_context* ctx);
+void vg_destroy(b2_context* ctx);
 
 // shared device helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

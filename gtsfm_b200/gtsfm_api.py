@@ -246,3 +246,19 @@ except Exception:  # noqa: BLE001
         reproj_error_gt_model: Optional[np.ndarray] = None
         inlier_avg_reproj_error_gt_model: Optional[float] = None
         outlier_avg_reproj_error_gt_model: Optional[float] = None
+
+
+try:  # pragma: no cover - exercised only inside a full GTSfM environment
+    from gtsfm.view_graph_estimator.cycle_consistent_rotation_estimator import EdgeErrorAggregationCriterion
+    from gtsfm.view_graph_estimator.view_graph_estimator_base import ViewGraphEstimatorBase
+except Exception:  # noqa: BLE001
+    from enum import Enum
+
+    class EdgeErrorAggregationCriterion(str, Enum):  # mirrors cycle_consistent_rotation_estimator.py:33-48
+        MIN_EDGE_ERROR = "MIN_EDGE_ERROR"
+        MEDIAN_EDGE_ERROR = "MEDIAN_EDGE_ERROR"
+
+    class ViewGraphEstimatorBase(abc.ABC):  # the part of view_graph_estimator_base.py:38-92 that `run` needs
+        @abc.abstractmethod
+        def run(self, i2Ri1_dict, i2Ui1_dict, calibrations, corr_idxs_i1i2, keypoints, two_view_reports, output_dir=None):
+            ...

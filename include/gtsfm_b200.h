@@ -52,6 +52,8 @@ uint64_t b2_h2d_bytes(const b2_context* ctx);
  * split-fp16 ones (the on-device cross-check of the tensor-core path; tests only).
  * "ransac_workspace_mb" = 1..: device workspace one sub-batch of b2_ransac_verify_batched_dev may use (default 1024); a call with
  * more problems than fit is cut into consecutive sub-batches, which changes no result.
+ * "viewgraph_workspace_mb" = 1..: the segment window of one chunk of b2_viewgraph_cycle_filter_host's MEDIAN (default 1024);
+ * a graph with more segment entries than fit is processed in several chunks, which changes no result.
  * "feature_cache" = 0 | 1: drop every cached device copy of host feature arrays and (0, default) copy on every call like the
  * reference / (1) keep device copies keyed by (host pointer, size) and validated by a hash of the FULL contents, so arrays
  * edited in place are re-sent.  Only pays off for callers that pass the same numpy buffers repeatedly (it does nothing for
@@ -502,6 +504,31 @@ typedef struct b2_twoview_eval_result {
  * with.  Bad arguments return B2_ERR_ARG before any launch. */
 int b2_twoview_eval_batched_dev(b2_context* ctx, const b2_twoview_eval_problem* problems, int n, const b2_twoview_eval_params* params,
                                 b2_twoview_eval_result* results, void* stream);
+
+/* ---- View-graph filter: cycle-consistent rotations (gtsfm/view_graph_estimator/cycle_consistent_rotation_estimator.py) --
+ * Edge e = (edges[e][0], edges[e][1]) with 0 <= i1 < i2, each at most once, and R[e] its i2Ri1 (row-major).  Every node
+ * set i0 < i1 < i2 whose three edges are inputs is a triplet with cycle error |rotvec((R(i0,i2)^T R(i1,i2)) R(i0,i1))| in
+ * degrees; an edge's aggregate is the median (the mean of the two middle values for an even count) or the minimum of the
+ * errors of its triplets, NaN when one of them is NaN.  An edge is kept when its aggregate < error_threshold_deg, or when it
+ * is in no triplet (aggregate NaN, num_cycles 0).  fp64; oracle/view_graph_ref.py is the NumPy statement.  Image indices may
+ * be sparse and large: memory is O(edges) plus the segment window of "viewgraph_workspace_mb" (b2_set_option) and 8 bytes
+ * per edge (MEDIAN only); a run cut into several windows returns what one window returns, bit for bit. */
+#define B2_VG_MEDIAN 0 /* EdgeErrorAggregationCriterion.MEDIAN_EDGE_ERROR */
+#define B2_VG_MIN 1    /* EdgeErrorAggregationCriterion.MIN_EDGE_ERROR */
+typedef struct b2_viewgraph_params {
+  int criterion;               /* B2_VG_MEDIAN or B2_VG_MIN */
+  int pad_;
+  double error_threshold_deg;  /* 7 in the reference */
+} b2_viewgraph_params;
+/* HOST inputs and outputs, all in input order: keep [n], aggregate [n], num_cycles [n] (the triplets of each edge).  Bad
+ * arguments (n < 0, a negative index, i1 >= i2) return B2_ERR_ARG before any launch; a repeated edge returns B2_ERR_ARG
+ * after the run, with the outputs untouched.  One synchronisation; the result does not depend on the input order. */
+int b2_viewgraph_cycle_filter_host(b2_context* ctx, const int32_t* edges, const double* R, int n, const b2_viewgraph_params* params,
+                                   uint8_t* keep, double* aggregate, int32_t* num_cycles, void* stream);
+/* Test-only: every triplet once, HOST out_nodes [capacity][3] (sorted node ids) and out_error [capacity] (degrees), in no
+ * particular order; *out_count = the number of triplets (entries past `capacity` are not written). */
+int b2_debug_viewgraph_triplets_host(b2_context* ctx, const int32_t* edges, const double* R, int n, int64_t capacity,
+                                     int32_t* out_nodes, double* out_error, int64_t* out_count, void* stream);
 
 /* ---- LMedS verifier (gtsfm/frontend/verifier/lmeds.py: cv2.findEssentialMat / findFundamentalMat with LMEDS) ----------
  * A batched device restatement of cv2's LMeDS estimator: cv::RNG subsets (seed 2^64 - 1, F subsets with collinear points
