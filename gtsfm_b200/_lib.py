@@ -187,6 +187,13 @@ SIGNATURES = {
     "b2_debug_superglue_assign_host": (_i, [_vp, _i, _i, _vp, _i, _i, _f, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ip, _ip]),
     "b2_debug_lightglue_assign_host": (_i, [_vp, _i, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ip,
                                             _ip]),
+    "b2_debug_lightglue_argmax_host": (_i, [_vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _vp, _ip]),
+    "b2_debug_lightglue_posenc_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b2_debug_lightglue_ln_gelu_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b2_debug_lightglue_rowheads_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b2_debug_lightglue_prune_host": (_i, [_vp, _i, _vp, _vp, _vp, _f, _f, _vp, _vp]),
+    "b2_debug_lightglue_gather_host": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "b2_debug_lightglue_filter_host": (_i, [_vp, _i, _i, _vp, _vp, _vp, _f, _vp, _vp, _vp, _vp, _ip]),
     "b2_superpoint_set_weights": (_i, [_vp, _vp, _sz]),
     "b2_superpoint_detect_dev": (_i, [_vp, _vp, _i, _i, _i, _sz, _f, _i, _i, _vp, _vp, _i, _ip, C.POINTER(C.c_uint64), _vp]),
     "b2_superpoint_describe_dev": (_i, [_vp, C.c_uint64, _vp, _i, _vp, _vp]),
@@ -201,6 +208,8 @@ SIGNATURES = {
     "b2_lightglue_match_dev": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, C.POINTER(LightGlueParams), _vp, _vp, _ip, _ip, _vp]),
     "b2_lightglue_match_host": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _i, C.POINTER(LightGlueParams), _vp, _vp, _ip, _ip]),
     "b2_lightglue_match_batched_dev": (_i, [_vp, C.POINTER(LightGluePair), _i, C.POINTER(LightGlueParams), _vp]),
+    "b2_lightglue_trace_count": (_i, [_vp]),
+    "b2_lightglue_trace_get": (_i, [_vp, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "b2_lightglue_encoded_bytes": (_sz, [_i]),
     "b2_lightglue_encode_batched_dev": (_i, [_vp, C.POINTER(LightGlueImage), _i, C.POINTER(LightGlueParams), _vp]),
     "b2_superglue_set_weights": (_i, [_vp, _vp, _sz]),

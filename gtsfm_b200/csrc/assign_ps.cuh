@@ -198,7 +198,7 @@ __global__ void __launch_bounds__(SK_T, 1) k_assign_ps(const SinkArgs a) {
             }
           } else if (i < M) {
             a.best0[i] = m;
-            a.arg0[i] = bi;
+            a.arg0[i] = bi == 0x7fffffff ? 0 : bi;  // no score beat -inf (a NaN row): best -inf, as the column merge does
           }
         }
       }

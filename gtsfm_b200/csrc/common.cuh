@@ -7,6 +7,7 @@
 #include <string.h>
 
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -129,6 +130,7 @@ struct b2_context {
   int rs_workspace_mb = 1024;  // RANSAC workspace budget per sub-batch of a batched call; b2_set_option "ransac_workspace_mb"
   int vg_workspace_mb = 1024;  // view-graph filter: segment window of one chunk; b2_set_option "viewgraph_workspace_mb"
   int force_simt = -1;  // 1: models loaded afterwards run the exact-fp32 SIMT kernels (no tensor cores); -1 = B2_FORCE_SIMT env
+  int lg_trace = 0;     // 1: b2_lightglue_match_* record each side's state after every layer (b2_lightglue_trace_get)
   std::string err;
   std::mutex mu;
   uint64_t launches = 0;
@@ -211,6 +213,24 @@ inline void b2_prof_work(b2_context* ctx, const char* kernel, double work) {
 #define B2_CHECK_LAUNCH(ctx) B2_CUDA(ctx, cudaGetLastError())
 
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
+
+// Test-only entry points (debug.cu, lightglue.cu): a host buffer that the call copies to the device and back whole, so that values outside the written region return as
+// they went in, followed on the device by `guard` bytes of 0xFF (NaN in fp32 and fp16) that the kernel must leave alone.
+inline int dbg_upload(b2_context* ctx, cudaStream_t st, const void* host, size_t bytes, size_t guard, DevBuf& d) {
+  if (bytes == 0 && guard == 0) return B2_OK;
+  B2_CUDA(ctx, d.ensure(bytes + guard));
+  B2_CUDA(ctx, cudaMemcpyAsync(d.p, host, bytes, cudaMemcpyHostToDevice, st));
+  B2_CUDA(ctx, cudaMemsetAsync(static_cast<unsigned char*>(d.p) + bytes, 0xFF, guard, st));
+  return B2_OK;
+}
+inline int dbg_download(b2_context* ctx, cudaStream_t st, void* host, size_t bytes, size_t guard, const DevBuf& d, bool& guard_ok) {
+  std::vector<unsigned char> g(guard);
+  B2_CUDA(ctx, cudaMemcpyAsync(host, d.p, bytes, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaMemcpyAsync(g.data(), static_cast<const unsigned char*>(d.p) + bytes, guard, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  for (unsigned char v : g) guard_ok = guard_ok && v == 0xFF;
+  return B2_OK;
+}
 
 // model state lifecycle (defined in the respective .cu files)
 void sp_destroy(b2_context* ctx);

@@ -29,24 +29,6 @@ static int dbg_upload_split(b2_context* ctx, cudaStream_t st, const float* host,
   B2_CHECK_LAUNCH(ctx);
   return B2_OK;
 }
-// A host buffer that the call copies to the device and back whole, so that values outside the written region return as
-// they went in, followed on the device by `guard` bytes of 0xFF (NaN in fp32 and fp16) that the kernel must leave alone.
-static int dbg_upload(b2_context* ctx, cudaStream_t st, const void* host, size_t bytes, size_t guard, DevBuf& d) {
-  if (bytes == 0) return B2_OK;
-  B2_CUDA(ctx, d.ensure(bytes + guard));
-  B2_CUDA(ctx, cudaMemcpyAsync(d.p, host, bytes, cudaMemcpyHostToDevice, st));
-  B2_CUDA(ctx, cudaMemsetAsync(static_cast<unsigned char*>(d.p) + bytes, 0xFF, guard, st));
-  return B2_OK;
-}
-static int dbg_download(b2_context* ctx, cudaStream_t st, void* host, size_t bytes, size_t guard, const DevBuf& d, bool& guard_ok) {
-  std::vector<unsigned char> g(guard);
-  B2_CUDA(ctx, cudaMemcpyAsync(host, d.p, bytes, cudaMemcpyDeviceToHost, st));
-  B2_CUDA(ctx, cudaMemcpyAsync(g.data(), static_cast<const unsigned char*>(d.p) + bytes, guard, cudaMemcpyDeviceToHost, st));
-  B2_CUDA(ctx, cudaStreamSynchronize(st));
-  for (unsigned char v : g) guard_ok = guard_ok && v == 0xFF;
-  return B2_OK;
-}
-
 extern "C" int b2_debug_linear_host(b2_context* ctx, const b2_linear_launch* L, const b2_linear_problem* P, int np) {
   if (!ctx || !L || !P || np <= 0 || (L->path != 0 && L->path != 1) || L->k1 < 0 || L->k2 < 0) return B2_ERR_ARG;
   const bool tc = L->path == 1, hm = L->head_major != 0;

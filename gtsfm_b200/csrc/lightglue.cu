@@ -52,6 +52,15 @@ struct LgPair {  // one pair of the running batch: sides 2 * slot, 2 * slot + 1
   float* out_scores = nullptr;
 };
 
+// One side's state after one layer, recorded when b2_set_option("lightglue_trace", 1) is set (b2_lightglue_trace_get).
+struct LgTraceRec {
+  int pair = 0, side = 0, layer = 0, n = 0;  // pair = index in the b2_lightglue_match_* call; n = rows going into the heads
+  int heads = 0;                             // conf / mat / unconf / kept / keep are filled (pruning or early exit on, not the last layer)
+  int unconf = 0, kept = 0, stop = 0;        // stop: the pair's early exit fired after this layer
+  std::vector<float> x, conf, mat;
+  std::vector<int> ind, keep;  // ind: original index of each row; keep: rows that survive pruning (src map, `kept` entries)
+};
+
 struct LightGlueState {
   bool loaded = false;
   int persist_ctas = 132;  // CTAs of the persistent kernels = SMs of the device minus the context's reserve_sms
@@ -67,6 +76,7 @@ struct LightGlueState {
   LgPair pair[LG_MAX_PAIRS];
   DevBuf sim[LG_MAX_PAIRS], counters, attn_part, attn_ml, attn_cnt, as_part, as_bar;
   HostBuf hread;
+  std::vector<LgTraceRec> trace;
 };
 
 template <typename J>
@@ -480,7 +490,7 @@ __global__ void __launch_bounds__(256) k_lg_row_argmax(const float* __restrict__
     int oi = __shfl_xor_sync(0xffffffffu, bi, o);
     if (ov > bv || (ov == bv && oi < bi)) bv = ov, bi = oi;
   }
-  if (lane == 0) best[r] = bv, arg[r] = bi;
+  if (lane == 0) best[r] = bv, arg[r] = bi == 0x7fffffff ? 0 : bi;  // no score beat -inf (a NaN row): best -inf, never a match
 }
 __global__ void __launch_bounds__(1024) k_lg_col_argmax(const float* __restrict__ sim, int m, int n,
                                                          const float* __restrict__ rmax, const float* __restrict__ rlog,
@@ -545,7 +555,7 @@ __global__ void __launch_bounds__(1024) k_lg_filter(const float* __restrict__ be
       j = a0[i];
       bool mutual = a1[j] == i;
       ms = mutual ? expf(best0[i]) : 0.f;
-      valid = mutual && ms > th;
+      valid = mutual && best0[i] > -INFINITY && ms > th;  // a row without an arg-max (best -inf) never matches, whatever th is
     }
     unsigned vm = __ballot_sync(0xffffffffu, valid);
     if (lane == 0) wtot[warp] = __popc(vm);
@@ -599,9 +609,10 @@ struct LgAssign {
   int* count;
 };
 
-// path 0 runs the persistent kernel when it fits (what the matcher does), 1 forces it, 2 forces the multi-launch passes; G
-// is the persistent kernel's CTA count.  *ran (when given) receives the path that ran, 1 or 2.
-static int lg_assign(b2_context* ctx, cudaStream_t st, const LgAssign& p, int path, int G, int* ran) {
+// The statistics and the mutual arg-max (everything before the filter).  path 0 runs the persistent kernel when it fits
+// (what the matcher does), 1 forces it, 2 forces the multi-launch passes; G is the persistent kernel's CTA count.  *ran
+// (when given) receives the path that ran, 1 or 2.
+static int lg_assign_argmax(b2_context* ctx, cudaStream_t st, const LgAssign& p, int path, int G, int* ran) {
   const float* sim = p.sim;
   const int M = p.M, N = p.N;
   const bool persistent = path == 0 ? assign_ps_fits(1, N) : path == 1;
@@ -631,6 +642,13 @@ static int lg_assign(b2_context* ctx, cudaStream_t st, const LgAssign& p, int pa
     B2_LAUNCH(ctx, k_lg_col_argmax, cdiv(N, 32), 1024, 0, st, sim, M, N, p.r.max, p.r.log, p.c.max, p.c.log, p.r.lsg, p.c.lsg, p.arg1);
     B2_CHECK_LAUNCH(ctx);
   }
+  return B2_OK;
+}
+
+static int lg_assign(b2_context* ctx, cudaStream_t st, const LgAssign& p, int path, int G, int* ran) {
+  const int M = p.M;
+  int rc;
+  if ((rc = lg_assign_argmax(ctx, st, p, path, G, ran))) return rc;
   B2_LAUNCH(ctx, k_lg_filter, 1, 1024, 0, st, p.best0, p.arg0, p.arg1, M, p.thr, p.ind0, p.ind1, p.out_matches, p.out_scores, p.count);
   B2_CHECK_LAUNCH(ctx);
   return B2_OK;
@@ -937,8 +955,34 @@ static int lg_enc_copy(b2_context* ctx, cudaStream_t st, LightGlueState* s, cons
   return B2_OK;
 }
 
-// One batch of up to LG_MAX_PAIRS pairs walked in lock-step (lightglue.py:474-629 for each of them).
-static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, const b2_lightglue_params* prm, cudaStream_t st) {
+// Appends the state of the sides in `act` after `layer` to the trace (synchronises the stream); with `heads` also their
+// confidence, matchability, counters and keep maps.  p0: index of the batch's first pair in the call.
+static int lg_trace_layer(b2_context* ctx, cudaStream_t st, LightGlueState* s, const LgActive& act, int layer, int p0, bool heads) {
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  const int* hc = s->hread.as<int>();
+  for (int i = 0; i < act.n; ++i) {
+    const int sdi = act.side[i];
+    const LgSide& sd = s->side[sdi];
+    LgTraceRec r;
+    r.pair = p0 + (sdi >> 1), r.side = sdi & 1, r.layer = layer, r.n = sd.n, r.heads = heads ? 1 : 0;
+    r.x.resize((size_t)sd.n * 256), r.ind.resize(sd.n);
+    B2_CUDA(ctx, cudaMemcpy(r.x.data(), sd.x[sd.cur].p, r.x.size() * 4, cudaMemcpyDeviceToHost));
+    B2_CUDA(ctx, cudaMemcpy(r.ind.data(), sd.ind[sd.cur].p, r.ind.size() * 4, cudaMemcpyDeviceToHost));
+    if (heads) {
+      r.unconf = hc[4 * (sdi >> 1) + r.side], r.kept = hc[4 * (sdi >> 1) + 2 + r.side];
+      r.conf.resize(sd.n), r.mat.resize(sd.n), r.keep.resize(r.kept);
+      B2_CUDA(ctx, cudaMemcpy(r.conf.data(), sd.conf.p, (size_t)sd.n * 4, cudaMemcpyDeviceToHost));
+      B2_CUDA(ctx, cudaMemcpy(r.mat.data(), sd.mat.p, (size_t)sd.n * 4, cudaMemcpyDeviceToHost));
+      B2_CUDA(ctx, cudaMemcpy(r.keep.data(), sd.src.p, (size_t)r.kept * 4, cudaMemcpyDeviceToHost));
+    }
+    s->trace.push_back(std::move(r));
+  }
+  return B2_OK;
+}
+
+// One batch of up to LG_MAX_PAIRS pairs walked in lock-step (lightglue.py:474-629 for each of them).  p0: index of its first
+// pair in the call (trace records only).
+static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, const b2_lightglue_params* prm, cudaStream_t st, int p0) {
   LightGlueState* s = ctx->lg;
   int rc;
   for (int p = 0; p < np; ++p) {
@@ -983,8 +1027,11 @@ static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, con
     if ((rc = lg_cross_block(ctx, st, s, act, layer, fp16_attn))) return rc;
     for (int p = 0; p < np; ++p)
       if (s->pair[p].active) s->pair[p].stop = layer;
-    if (layer == LG_LAYERS - 1) break;
-    if (!do_stop && !do_prune) continue;
+    if (layer == LG_LAYERS - 1 || (!do_stop && !do_prune)) {
+      if (ctx->lg_trace && (rc = lg_trace_layer(ctx, st, s, act, layer, p0, false))) return rc;
+      if (layer == LG_LAYERS - 1) break;
+      continue;
+    }
     bool prune_side[LG_MAX_SIDES];
     JobList<HeadJob> hj{};
     JobList<PruneJob> pj{};
@@ -1009,6 +1056,8 @@ static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, con
     B2_CHECK_LAUNCH(ctx);
     B2_CUDA(ctx, cudaMemcpyAsync(hread, counters, 4 * LG_MAX_PAIRS * sizeof(int), cudaMemcpyDeviceToHost, st));
     B2_CUDA(ctx, cudaStreamSynchronize(st));
+    const size_t trace0 = s->trace.size();
+    if (ctx->lg_trace && (rc = lg_trace_layer(ctx, st, s, act, layer, p0, true))) return rc;
     JobList<GatherJob> gj{};
     int ng = 0, gmax = 0;
     for (int p = 0; p < np; ++p) {
@@ -1020,6 +1069,7 @@ static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, con
         const float ratio = 1.0f - (float)(hc[0] + hc[1]) / (float)(lp.n0 + lp.n1);
         if (ratio > (float)prm->depth_confidence) {
           lp.active = false;
+          for (size_t t = trace0; t < s->trace.size(); ++t) s->trace[t].stop |= s->trace[t].pair == p0 + p;
           continue;
         }
       }
@@ -1036,7 +1086,10 @@ static int lg_match_batch(b2_context* ctx, b2_lightglue_pair* pairs, int np, con
         sd.cur = nxt;
         sd.n = hc[2 + side];
       }
-      if (s->side[2 * p].n == 0 || s->side[2 * p + 1].n == 0) lp.active = false;  // everything pruned away: no matches
+      if (s->side[2 * p].n == 0 || s->side[2 * p + 1].n == 0) {  // everything pruned away: no matches
+        lp.active = false;
+        lp.stop = layer + 1;  // the reference's loop stops at the top of the next layer (lightglue.py:580-592: stop = i + 1)
+      }
     }
     if (ng > 0) {
       B2_LAUNCH(ctx, k_lg_gather, dim3(cdiv(gmax, 8), ng), 256, 0, st, gj);
@@ -1112,10 +1165,11 @@ static int lg_match_pairs(b2_context* ctx, b2_lightglue_pair* pairs, int n_pairs
   LightGlueState* s = ctx->lg;
   if (!s || !s->loaded) return b2_fail(ctx, B2_ERR_STATE, "lightglue weights not set");
   s->persist_ctas = ctx->sm_count - ctx->reserve_sms > 0 ? ctx->sm_count - ctx->reserve_sms : 1;
+  s->trace.clear();
   const int bmax = ctx->lg_batch > 0 && ctx->lg_batch < LG_MAX_PAIRS ? ctx->lg_batch : LG_MAX_PAIRS;
   for (int p0 = 0; p0 < n_pairs; p0 += bmax) {
     const int np = n_pairs - p0 < bmax ? n_pairs - p0 : bmax;
-    int rc = lg_match_batch(ctx, pairs + p0, np, prm, st);
+    int rc = lg_match_batch(ctx, pairs + p0, np, prm, st, p0);
     if (rc) return rc;
   }
   return B2_OK;
@@ -1340,6 +1394,273 @@ extern "C" int b2_debug_lightglue_assign_host(b2_context* ctx, int path, int cta
     B2_CUDA(ctx, cudaMemcpy(out_scores, outs.p, (size_t)k * 4, cudaMemcpyDeviceToHost));
   }
   *out_k = k;
+  if (e) return b2_fail(ctx, B2_ERR_STATE, "the persistent assignment kernel timed out in its grid barrier (kernel bug)");
+  return B2_OK;
+}
+
+// ---- the per-layer trace (b2_set_option "lightglue_trace") ------------------------------------------------------------------
+
+extern "C" int b2_lightglue_trace_count(b2_context* ctx) {
+  if (!ctx) return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  return ctx->lg ? (int)ctx->lg->trace.size() : 0;
+}
+
+extern "C" int b2_lightglue_trace_get(b2_context* ctx, int i, int* meta, float* x, int* ind, float* conf, float* mat, int* keep) {
+  if (!ctx || !meta) return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (!ctx->lg || i < 0 || i >= (int)ctx->lg->trace.size()) return b2_fail(ctx, B2_ERR_ARG, "no such lightglue trace record");
+  const LgTraceRec& r = ctx->lg->trace[i];
+  const int m[8] = {r.pair, r.side, r.layer, r.n, r.heads, r.unconf, r.kept, r.stop};
+  memcpy(meta, m, sizeof(m));
+  if (x) memcpy(x, r.x.data(), r.x.size() * 4);
+  if (ind) memcpy(ind, r.ind.data(), r.ind.size() * 4);
+  if (conf) memcpy(conf, r.conf.data(), r.conf.size() * 4);
+  if (mat) memcpy(mat, r.mat.data(), r.mat.size() * 4);
+  if (keep) memcpy(keep, r.keep.data(), r.keep.size() * 4);
+  return B2_OK;
+}
+
+// ---- test-only entry points: one LightGlue kernel on host arrays, launched as lg_match_batch launches it ------------------
+// Entry i of a batched launch has n[i] rows (0 allowed); its arrays are concatenated over i on the host and live in buffers
+// of their own on the device, each output followed by a 0xFF guard that the kernel must leave alone.
+
+constexpr size_t LG_DBG_GUARD = 4096;
+
+struct LgDbg {
+  b2_context* ctx;
+  cudaStream_t st;
+  std::vector<std::unique_ptr<DevBuf>> bufs;
+  struct Out {
+    void* host;
+    size_t bytes;
+    const DevBuf* d;
+  };
+  std::vector<Out> outs;
+  // host -> device; an output (out = true) is copied in too, so what the kernel does not write comes back as it went in
+  template <typename T>
+  int put(const T* host, size_t n, bool out, T** dev) {
+    *dev = nullptr;
+    if (!host) return B2_OK;
+    bufs.emplace_back(new DevBuf());
+    DevBuf& d = *bufs.back();
+    int rc;
+    if ((rc = dbg_upload(ctx, st, host, n * sizeof(T), out ? LG_DBG_GUARD : 0, d))) return rc;
+    if (out) outs.push_back({const_cast<T*>(host), n * sizeof(T), &d});
+    *dev = d.as<T>();
+    return B2_OK;
+  }
+  int finish(const char* what) {
+    bool guard_ok = true;
+    int rc;
+    for (const Out& o : outs)
+      if ((rc = dbg_download(ctx, st, o.host, o.bytes, LG_DBG_GUARD, *o.d, guard_ok))) return rc;
+    if (!guard_ok) return b2_fail(ctx, B2_ERR_STATE, std::string(what) + ": the kernel wrote past the end of an output");
+    return B2_OK;
+  }
+};
+
+static int lg_dbg_sizes(const int* n, int np, int* mx) {
+  if (!n || np <= 0 || np > LG_MAX_SIDES) return B2_ERR_ARG;
+  *mx = 0;
+  for (int i = 0; i < np; ++i) {
+    if (n[i] < 0) return B2_ERR_ARG;
+    *mx = n[i] > *mx ? n[i] : *mx;
+  }
+  return B2_OK;
+}
+
+extern "C" int b2_debug_lightglue_posenc_host(b2_context* ctx, int np, const int* n, const float* kp, const float* wr, float* cs,
+                                              float* sn, int* ind) {
+  int mx, rc;
+  if (!ctx || !kp || !wr || !cs || !sn || !ind || lg_dbg_sizes(n, np, &mx)) return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  LgDbg d{ctx, ctx->stream};
+  JobList<PosJob> pj{};
+  float* dwr;
+  if ((rc = d.put(wr, 64, false, &dwr))) return rc;
+  for (int i = 0, o = 0; i < np; o += n[i++]) {
+    PosJob& j = pj.j[i];
+    j.n = n[i];
+    float* k;
+    if ((rc = d.put(kp + 2 * o, 2 * (size_t)n[i], false, &k)) || (rc = d.put(cs + 32 * (size_t)o, 32 * (size_t)n[i], true, &j.cs)) ||
+        (rc = d.put(sn + 32 * (size_t)o, 32 * (size_t)n[i], true, &j.sn)) || (rc = d.put(ind + o, (size_t)n[i], true, &j.ind)))
+      return rc;
+    j.kp = k;
+  }
+  if (mx > 0) {
+    const int pb = cdiv(mx * 32, 1024);
+    B2_LAUNCH(ctx, k_lg_posenc, dim3(pb < 16 ? pb : 16, np), 1024, 0, d.st, pj, dwr);
+    B2_CHECK_LAUNCH(ctx);
+  }
+  return d.finish("b2_debug_lightglue_posenc_host");
+}
+
+extern "C" int b2_debug_lightglue_ln_gelu_host(b2_context* ctx, int np, const int* n, const float* g, const float* b, float* h,
+                                               uint16_t* hi, uint16_t* lo) {
+  int mx, rc;
+  if (!ctx || !g || !b || !h || !hi != !lo || lg_dbg_sizes(n, np, &mx)) return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  LgDbg d{ctx, ctx->stream};
+  JobList<LnJob> lj{};
+  float *dg, *db;
+  if ((rc = d.put(g, 512, false, &dg)) || (rc = d.put(b, 512, false, &db))) return rc;
+  for (int i = 0, o = 0; i < np; o += n[i++]) {
+    LnJob& j = lj.j[i];
+    const size_t e = 512 * (size_t)o, ne = 512 * (size_t)n[i];
+    j.n = n[i];
+    uint16_t *dh = nullptr, *dl = nullptr;
+    if ((rc = d.put(h + e, ne, true, &j.h)) || (hi && ((rc = d.put(hi + e, ne, true, &dh)) || (rc = d.put(lo + e, ne, true, &dl)))))
+      return rc;
+    j.hi = reinterpret_cast<__half*>(dh), j.lo = reinterpret_cast<__half*>(dl);
+  }
+  if (mx > 0) {
+    B2_LAUNCH(ctx, k_lg_ln_gelu, dim3(cdiv(mx, 8), np), 256, 0, d.st, lj, dg, db);
+    B2_CHECK_LAUNCH(ctx);
+  }
+  return d.finish("b2_debug_lightglue_ln_gelu_host");
+}
+
+extern "C" int b2_debug_lightglue_rowheads_host(b2_context* ctx, int np, const int* n, const int* mode, const float* x, const float* w1,
+                                                const float* b1, const float* w2, const float* b2, float* o1, float* o2, float* zraw) {
+  int mx, rc;
+  if (!ctx || !mode || !x || !o1 || !o2 || !zraw || !w1 != !b1 || !w2 != !b2 || lg_dbg_sizes(n, np, &mx)) return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  LgDbg d{ctx, ctx->stream};
+  JobList<HeadJob> hj{};
+  float *dw1, *db1, *dw2, *db2;
+  if ((rc = d.put(w1, 256, false, &dw1)) || (rc = d.put(b1, 1, false, &db1)) || (rc = d.put(w2, 256, false, &dw2)) ||
+      (rc = d.put(b2, 1, false, &db2)))
+    return rc;
+  for (int i = 0, o = 0; i < np; o += n[i++]) {
+    HeadJob& j = hj.j[i];
+    float *dx, *d1, *d2, *dz;
+    if ((rc = d.put(x + 256 * (size_t)o, 256 * (size_t)n[i], false, &dx)) || (rc = d.put(o1 + o, (size_t)n[i], true, &d1)) ||
+        (rc = d.put(o2 + o, (size_t)n[i], true, &d2)) || (rc = d.put(zraw + o, (size_t)n[i], true, &dz)))
+      return rc;
+    // mode bit 0: head 2 on for this entry; bit 1: its sigmoid is written (o2); bit 2: its raw logit is written (zraw)
+    const bool h2 = (mode[i] & 1) && dw2;
+    j = {dx, n[i], h2 ? dw2 : nullptr, h2 ? db2 : nullptr, d1, (mode[i] & 2) ? d2 : nullptr, (mode[i] & 4) ? dz : nullptr};
+  }
+  if (mx > 0) {
+    B2_LAUNCH(ctx, k_lg_rowheads, dim3(cdiv(mx, 8), np), 256, 0, d.st, hj, dw1, db1);
+    B2_CHECK_LAUNCH(ctx);
+  }
+  return d.finish("b2_debug_lightglue_rowheads_host");
+}
+
+extern "C" int b2_debug_lightglue_prune_host(b2_context* ctx, int np, const int* n, const float* conf, const float* mat, float thr,
+                                             float keep_thr, int* src, int* counters) {
+  int mx, rc;
+  if (!ctx || !conf || !mat || !src || !counters || lg_dbg_sizes(n, np, &mx)) return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  LgDbg d{ctx, ctx->stream};
+  JobList<PruneJob> pj{};
+  int* dc;  // entries 2p and 2p + 1 are the two sides of pair p: [unconf0, unconf1, kept0, kept1]
+  if ((rc = d.put(counters, 4 * (size_t)((np + 1) / 2), true, &dc))) return rc;
+  for (int i = 0, o = 0; i < np; o += n[i++]) {
+    PruneJob& j = pj.j[i];
+    float *dcf, *dm;
+    if ((rc = d.put(conf + o, (size_t)n[i], false, &dcf)) || (rc = d.put(mat + o, (size_t)n[i], false, &dm)) ||
+        (rc = d.put(src + o, (size_t)n[i], true, &j.src)))
+      return rc;
+    j.conf = dcf, j.mat = dm, j.n = n[i], j.counters = dc + 4 * (i >> 1), j.side = i & 1;
+  }
+  B2_LAUNCH(ctx, k_lg_prune_plan, dim3(1, np), 1024, 0, d.st, pj, thr, keep_thr);
+  B2_CHECK_LAUNCH(ctx);
+  return d.finish("b2_debug_lightglue_prune_host");
+}
+
+extern "C" int b2_debug_lightglue_gather_host(b2_context* ctx, int np, const int* n, const int* cnt, const int* src, const float* x,
+                                              const float* cs, const float* sn, const int* ind, const uint16_t* planes, float* x2,
+                                              float* cs2, float* sn2, int* ind2, uint16_t* planes2) {
+  int mx, rc;
+  if (!ctx || !cnt || !src || !x || !cs || !sn || !ind || !x2 || !cs2 || !sn2 || !ind2 || !planes != !planes2 || lg_dbg_sizes(n, np, &mx))
+    return B2_ERR_ARG;
+  for (int i = 0, o = 0; i < np; o += n[i++]) {  // the kernel trusts the plan: cnt <= n rows, each src entry a row
+    if (cnt[i] < 0 || cnt[i] > n[i]) return B2_ERR_ARG;
+    for (int r = 0; r < cnt[i]; ++r)
+      if (src[o + r] < 0 || src[o + r] >= n[i]) return B2_ERR_ARG;
+  }
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  LgDbg d{ctx, ctx->stream};
+  JobList<GatherJob> gj{};
+  int* dcnt;
+  if ((rc = d.put(cnt, (size_t)np, false, &dcnt))) return rc;
+  for (int i = 0, o = 0; i < np; o += n[i++]) {
+    GatherJob& j = gj.j[i];
+    const size_t m = (size_t)n[i];
+    int *ds, *di;
+    float *dx, *dcs, *dsn;
+    uint16_t *dp = nullptr, *dp2 = nullptr;  // per entry: hi [n][256] then lo [n][256]
+    if ((rc = d.put(src + o, m, false, &ds)) || (rc = d.put(x + 256 * (size_t)o, 256 * m, false, &dx)) ||
+        (rc = d.put(cs + 32 * (size_t)o, 32 * m, false, &dcs)) || (rc = d.put(sn + 32 * (size_t)o, 32 * m, false, &dsn)) ||
+        (rc = d.put(ind + o, m, false, &di)) || (rc = d.put(x2 + 256 * (size_t)o, 256 * m, true, &j.x2)) ||
+        (rc = d.put(cs2 + 32 * (size_t)o, 32 * m, true, &j.cs2)) || (rc = d.put(sn2 + 32 * (size_t)o, 32 * m, true, &j.sn2)) ||
+        (rc = d.put(ind2 + o, m, true, &j.ind2)) ||
+        (planes && ((rc = d.put(planes + 512 * (size_t)o, 512 * m, false, &dp)) || (rc = d.put(planes2 + 512 * (size_t)o, 512 * m, true, &dp2)))))
+      return rc;
+    j.src = ds, j.cnt = dcnt + i, j.n = n[i], j.x = dx, j.cs = dcs, j.sn = dsn, j.ind = di;
+    j.ph = reinterpret_cast<const __half*>(dp), j.pstride = 256 * m, j.ph2 = reinterpret_cast<__half*>(dp2), j.pstride2 = 256 * m;
+  }
+  if (mx > 0) {
+    B2_LAUNCH(ctx, k_lg_gather, dim3(cdiv(mx, 8), np), 256, 0, d.st, gj);
+    B2_CHECK_LAUNCH(ctx);
+  }
+  return d.finish("b2_debug_lightglue_gather_host");
+}
+
+extern "C" int b2_debug_lightglue_filter_host(b2_context* ctx, int m, int n, const float* best0, const int* a0, const int* a1, float th,
+                                              const int* ind0, const int* ind1, int64_t* out_matches, float* out_scores, int* out_k) {
+  if (!ctx || m <= 0 || n <= 0 || !best0 || !a0 || !a1 || !ind0 || !ind1 || !out_matches || !out_scores || !out_k) return B2_ERR_ARG;
+  for (int i = 0; i < m; ++i)  // the kernel reads a1[a0[i]]: the arg-max kernels never hand it anything else
+    if (a0[i] < 0 || a0[i] >= n) return b2_fail(ctx, B2_ERR_ARG, "b2_debug_lightglue_filter_host: a0 entry out of range");
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  LgDbg d{ctx, ctx->stream};
+  float *db, *dos;
+  int *da0, *da1, *di0, *di1, *dk;
+  int64_t* dom;
+  int rc;
+  if ((rc = d.put(best0, (size_t)m, false, &db)) || (rc = d.put(a0, (size_t)m, false, &da0)) || (rc = d.put(a1, (size_t)n, false, &da1)) ||
+      (rc = d.put(ind0, (size_t)m, false, &di0)) || (rc = d.put(ind1, (size_t)n, false, &di1)) ||
+      (rc = d.put(out_matches, 2 * (size_t)m, true, &dom)) || (rc = d.put(out_scores, (size_t)m, true, &dos)) ||
+      (rc = d.put(out_k, 1, true, &dk)))
+    return rc;
+  B2_LAUNCH(ctx, k_lg_filter, 1, 1024, 0, d.st, db, da0, da1, m, th, di0, di1, reinterpret_cast<long long*>(dom), dos, dk);
+  B2_CHECK_LAUNCH(ctx);
+  return d.finish("b2_debug_lightglue_filter_host");
+}
+
+extern "C" int b2_debug_lightglue_argmax_host(b2_context* ctx, int path, const float* sim, int M, int N, const float* z0, const float* z1,
+                                              float* best0, int* arg0, int* arg1, int* out_path) {
+  if (!ctx || !sim || !z0 || !z1 || !best0 || !arg0 || !arg1 || !out_path || M <= 0 || N <= 0 || path < 0 || path > 2) return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  cudaSetDevice(ctx->device);
+  LgDbg d{ctx, ctx->stream};
+  DevBuf stats, part, bar, err;
+  float *dsim, *dz0, *dz1, *db;
+  int *da0, *da1;
+  int rc;
+  if ((rc = d.put(sim, (size_t)M * N, false, &dsim)) || (rc = d.put(z0, (size_t)M, false, &dz0)) || (rc = d.put(z1, (size_t)N, false, &dz1)) ||
+      (rc = d.put(best0, (size_t)M, true, &db)) || (rc = d.put(arg0, (size_t)M, true, &da0)) || (rc = d.put(arg1, (size_t)N, true, &da1)))
+    return rc;
+  B2_CUDA(ctx, stats.ensure((size_t)3 * (M + N) * 4));
+  B2_CUDA(ctx, err.ensure(16));
+  B2_CUDA(ctx, cudaMemsetAsync(err.p, 0, 16, d.st));
+  float *r = stats.as<float>(), *c = r + 3 * M;
+  const LgAssign p{dsim, M, N, dz0, dz1, nullptr, nullptr, 0.f, {r, r + M, r + 2 * M}, {c, c + N, c + 2 * N}, db, da0, da1, &part, &bar,
+                   err.as<int>(), nullptr, nullptr, nullptr};
+  const int G = ctx->sm_count - ctx->reserve_sms > 0 ? ctx->sm_count - ctx->reserve_sms : 1;
+  if ((rc = lg_assign_argmax(ctx, d.st, p, path, G, out_path))) return rc;
+  if ((rc = d.finish("b2_debug_lightglue_argmax_host"))) return rc;
+  int e = 0;
+  B2_CUDA(ctx, cudaMemcpy(&e, err.p, 4, cudaMemcpyDeviceToHost));
   if (e) return b2_fail(ctx, B2_ERR_STATE, "the persistent assignment kernel timed out in its grid barrier (kernel bug)");
   return B2_OK;
 }

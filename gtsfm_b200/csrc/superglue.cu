@@ -186,7 +186,7 @@ __global__ void __launch_bounds__(256) k_sg_row_argmax(const float* __restrict__
     int oi = __shfl_xor_sync(0xffffffffu, bi, o);
     if (ov > bv || (ov == bv && oi < bi)) bv = ov, bi = oi;
   }
-  if (lane == 0) best[i] = bv, arg[i] = bi;
+  if (lane == 0) best[i] = bv, arg[i] = bi == 0x7fffffff ? 0 : bi;  // no score beat -inf (a NaN row): k_sg_filter reads a1[arg]
 }
 __global__ void __launch_bounds__(256) k_sg_col_argmax(const float* __restrict__ Z, int M, int N, const float* __restrict__ u,
                                                         const float* __restrict__ v, float norm, int* __restrict__ arg) {

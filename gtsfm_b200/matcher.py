@@ -55,6 +55,24 @@ class LightGlueEngine:
             return out[: k.value].copy(), sc[: k.value].copy()
         return out[: k.value].copy()
 
+    def layer_trace(self):
+        """The per-layer state the last match call recorded under set_option("lightglue_trace", 1): one dict per active side
+        and layer, in the order recorded (include/gtsfm_b200.h, b2_lightglue_trace_get)."""
+        lib, h = self.ctx.lib, self.ctx.handle
+        recs = []
+        for i in range(lib.b2_lightglue_trace_count(h)):
+            meta = np.zeros(8, np.int32)
+            self.ctx.check(lib.b2_lightglue_trace_get(h, i, _lib.ptr(meta), None, None, None, None, None), "lightglue_trace_get")
+            pair, side, layer, n, heads, unconf, kept, stop = (int(v) for v in meta)
+            x, ind = np.empty((n, DESC_DIM), np.float32), np.empty(n, np.int32)
+            conf, mat = np.empty(n if heads else 0, np.float32), np.empty(n if heads else 0, np.float32)
+            keep = np.empty(kept if heads else 0, np.int32)
+            self.ctx.check(lib.b2_lightglue_trace_get(h, i, _lib.ptr(meta), _lib.ptr(x), _lib.ptr(ind), _lib.ptr(conf), _lib.ptr(mat),
+                                                      _lib.ptr(keep)), "lightglue_trace_get")
+            recs.append(dict(pair=pair, side=side, layer=layer, n=n, heads=bool(heads), unconf=unconf, kept=kept, stop=bool(stop), x=x,
+                             ind=ind, conf=conf, mat=mat, keep=keep))
+        return recs
+
 
 class B200LightGlueMatcher(MatcherBase):
     """LightGlue on hand-written sm_90a kernels behind GTSfM's MatcherBase.

@@ -50,6 +50,7 @@ uint64_t b2_h2d_bytes(const b2_context* ctx);
  * "lightglue_batch" = 0..8: pairs per lock-step batch of b2_lightglue_match_batched_dev (0 = 8, the maximum).
  * "force_simt" = 0 | 1: models whose weights are set afterwards run the exact-fp32 SIMT kernels instead of the wgmma
  * split-fp16 ones (the on-device cross-check of the tensor-core path; tests only).
+ * "lightglue_trace" = 0 | 1: (1) record LightGlue's per-layer state in host memory (b2_lightglue_trace_get; tests only).
  * "ransac_workspace_mb" = 1..: device workspace one sub-batch of b2_ransac_verify_batched_dev may use (default 1024); a call with
  * more problems than fit is cut into consecutive sub-batches, which changes no result.
  * "viewgraph_workspace_mb" = 1..: the segment window of one chunk of b2_viewgraph_cycle_filter_host's MEDIAN (default 1024);
@@ -146,6 +147,38 @@ int b2_debug_lightglue_assign_host(b2_context* ctx, int path, int ctas, const fl
                                    const float* z1, const int* ind0, const int* ind1, float threshold, float* row_stats,
                                    float* col_stats, float* best0, int* arg0, int* arg1, int64_t* out_matches, float* out_scores,
                                    int* out_k, int* out_path);
+/* Test-only: the LightGlue assignment's statistics and mutual arg-max alone (b2_debug_lightglue_assign_host without the
+ * filter): best0 [M], arg0 [M], arg1 [N].  A row or column none of whose scores beats -inf (NaN scores) gets index 0 and,
+ * for rows, best0 = -inf. */
+int b2_debug_lightglue_argmax_host(b2_context* ctx, int path, const float* sim, int M, int N, const float* z0, const float* z1,
+                                   float* best0, int* arg0, int* arg1, int* out_path);
+/* Test-only: one LightGlue kernel on HOST arrays, as one batched launch of the matcher.  Entry i (0 <= i < np <= 16) has n[i]
+ * rows (0 allowed); per-row arrays are concatenated over the entries.  Every output is copied in first (what the kernel does
+ * not write comes back unchanged) and followed on the device by a guard that the kernel must not touch (B2_ERR_STATE).
+ *  posenc:   kp [n][2], wr [32][2] -> cs, sn [n][32] (rotary table of the bounding-box-normalised keypoints), ind [n] = 0..n-1.
+ *  ln_gelu:  LayerNorm(512, eps 1e-5; g, b) + exact GELU of h [n][512]: in place, or (hi, lo given) as split planes
+ *            [n][512] (hi + lo * 2^-11) with h left alone.
+ *  rowheads: x [n][256] -> o1 = sigmoid(w1.x + b1) (w1 NULL: head off) and head 2 = w2.x + b2 where mode[i] & 1, written as
+ *            its sigmoid to o2 where mode[i] & 2 and raw to zraw where mode[i] & 4.
+ *  prune:    entries 2p, 2p + 1 are the sides of pair p: counters [p][4] = (#conf < thr side 0, side 1, #kept side 0,
+ *            side 1), kept = mat > keep_thr or conf <= thr; src [n] receives the kept rows in order.
+ *  gather:   rows src[0 .. cnt[i]) of x [n][256], cs / sn [n][32], ind [n] (and planes [2][n][256], hi then lo) -> x2, cs2,
+ *            sn2, ind2 (planes2) rows 0 .. cnt[i).  cnt[i] <= n[i] and src entries < n[i] are checked.
+ *  filter:   (m rows, n columns) mutual check a1[a0[i]] == i, score exp(best0[i]) > th -> int64 rows (ind0[i], ind1[a0[i]]) in
+ *            ascending i, their scores, *out_k.  a0 entries must lie in [0, n). */
+int b2_debug_lightglue_posenc_host(b2_context* ctx, int np, const int* n, const float* kp, const float* wr, float* cs, float* sn,
+                                   int* ind);
+int b2_debug_lightglue_ln_gelu_host(b2_context* ctx, int np, const int* n, const float* g, const float* b, float* h, uint16_t* hi,
+                                    uint16_t* lo);
+int b2_debug_lightglue_rowheads_host(b2_context* ctx, int np, const int* n, const int* mode, const float* x, const float* w1,
+                                     const float* b1, const float* w2, const float* b2, float* o1, float* o2, float* zraw);
+int b2_debug_lightglue_prune_host(b2_context* ctx, int np, const int* n, const float* conf, const float* mat, float thr,
+                                  float keep_thr, int* src, int* counters);
+int b2_debug_lightglue_gather_host(b2_context* ctx, int np, const int* n, const int* cnt, const int* src, const float* x,
+                                   const float* cs, const float* sn, const int* ind, const uint16_t* planes, float* x2, float* cs2,
+                                   float* sn2, int* ind2, uint16_t* planes2);
+int b2_debug_lightglue_filter_host(b2_context* ctx, int m, int n, const float* best0, const int* a0, const int* a1, float th,
+                                   const int* ind0, const int* ind1, int64_t* out_matches, float* out_scores, int* out_k);
 
 /* ---- SuperPoint -------------------------------------------------------------------------------------------------- */
 /* `blob`: the 24 state-dict tensors in reference order (conv1a.weight, conv1a.bias, conv1b.weight, ... convDb.bias;
@@ -268,6 +301,14 @@ typedef struct b2_lightglue_image {
   int n;
   void* out;
 } b2_lightglue_image;
+/* The per-layer trace, recorded by every b2_lightglue_match_* call (and cleared at its start) while
+ * b2_set_option("lightglue_trace", 1) is set; off by default (it synchronises after every layer).  One record per active
+ * side and layer: meta [8] = (pair index in the call, side, layer, n rows, heads, #unconfident, #kept, early exit fired
+ * after this layer); x [n][256] after the layer, ind [n] original row indices; with heads = 1 also conf [n], mat [n] (the
+ * confidence and matchability the pruning decision read) and keep [#kept] (the rows kept, ascending).  NULL arrays are
+ * skipped: call once with meta only to size them. */
+int b2_lightglue_trace_count(b2_context* ctx);
+int b2_lightglue_trace_get(b2_context* ctx, int i, int* meta, float* x, int* ind, float* conf, float* mat, int* keep);
 size_t b2_lightglue_encoded_bytes(int n);
 int b2_lightglue_encode_batched_dev(b2_context* ctx, const b2_lightglue_image* imgs, int n_imgs, const b2_lightglue_params* params,
                                     void* stream);

@@ -65,9 +65,10 @@ def _ffn(sd, p, x, msg):
 def _half_sdpa(q, k, v):
     """What the reference's CUDA branch computes (lightglue.py:116-121): q, k, v cast to half, flash SDPA (fp32 accumulation
     of half operands), half result cast back.  Emulated on the CPU: operands and result rounded to fp16, arithmetic in fp32."""
-    q, k, v = (t.half().float() for t in (q, k, v))
+    dt = q.dtype
+    q, k, v = (t.half().to(dt) for t in (q, k, v))
     att = F.softmax(q @ k.transpose(-1, -2) * (q.shape[-1] ** -0.5), -1)
-    return (att @ v).half().float()
+    return (att @ v).half().to(dt)
 
 
 def self_block(sd, i, x, cs, fp16_attention=False):
@@ -121,18 +122,25 @@ def log_assignment(sd, i, d0, d1):
 
 def lightglue_match(
     kp0: np.ndarray, desc0: np.ndarray, kp1: np.ndarray, desc1: np.ndarray, sd: Dict[str, np.ndarray],
-    trace: Optional[dict] = None, fp16_attention: bool = False,
+    trace: Optional[dict] = None, fp16_attention: bool = False, dtype=np.float32, prune_min_kpts: int = -1,
 ) -> np.ndarray:
-    """-> (K, 2) int64 rows (index into set 0, index into set 1), ascending in column 0 (lightglue.py:594-602)."""
+    """-> (K, 2) int64 rows (index into set 0, index into set 1), ascending in column 0 (lightglue.py:594-602).
+
+    ``dtype``: weights, inputs and every operation in it (np.float64: the replay the device's per-layer state is held
+    against).  ``prune_min_kpts``: a side with at most this many keypoints is not pruned (the device's parameter of that
+    name; -1, the CPU semantics, prunes always).  ``trace`` receives per layer i: ``desc{0,1}_l{i}`` after the layer,
+    ``ind{0,1}_l{i}`` the original index of each row, and where the heads ran ``t{0,1}_l{i}`` (token confidence),
+    ``unconf_l{i}``, and for each pruned side ``ma{0,1}_l{i}`` (matchability) and ``keep{0,1}_l{i}`` (rows kept)."""
     m, n = len(kp0), len(kp1)
     if m == 0 or n == 0:
         return np.zeros((0, 2), np.int64)
     thr = torch.from_numpy(confidence_thresholds())
+    sd = {k: np.asarray(v, dtype) for k, v in sd.items()}
     with torch.no_grad():
-        k0 = normalize_keypoints_bbox(torch.from_numpy(np.asarray(kp0, np.float32)))
-        k1 = normalize_keypoints_bbox(torch.from_numpy(np.asarray(kp1, np.float32)))
-        d0 = torch.from_numpy(np.ascontiguousarray(desc0, dtype=np.float32))
-        d1 = torch.from_numpy(np.ascontiguousarray(desc1, dtype=np.float32))
+        k0 = normalize_keypoints_bbox(torch.from_numpy(np.asarray(kp0, np.float32).astype(dtype)))
+        k1 = normalize_keypoints_bbox(torch.from_numpy(np.asarray(kp1, np.float32).astype(dtype)))
+        d0 = torch.from_numpy(np.ascontiguousarray(desc0, dtype=np.float32).astype(dtype))
+        d1 = torch.from_numpy(np.ascontiguousarray(desc1, dtype=np.float32).astype(dtype))
         cs0, cs1 = rotary_table(sd, k0), rotary_table(sd, k1)
         ind0, ind1 = torch.arange(m), torch.arange(n)
         sizes = []
@@ -147,6 +155,8 @@ def lightglue_match(
             if trace is not None:
                 trace[f"desc0_l{i}"] = d0.numpy().copy()
                 trace[f"desc1_l{i}"] = d1.numpy().copy()
+                trace[f"ind0_l{i}"] = ind0.numpy().copy()
+                trace[f"ind1_l{i}"] = ind1.numpy().copy()
             if i == N_LAYERS - 1:
                 continue
             # lightglue.py:84-94,645-656
@@ -154,13 +164,20 @@ def lightglue_match(
             t0 = torch.sigmoid(_lin(sd, p, d0))[:, 0]
             t1 = torch.sigmoid(_lin(sd, p, d1))[:, 0]
             unconf = (torch.cat([t0, t1]) < thr[i]).float().sum()
+            if trace is not None:
+                trace[f"t0_l{i}"], trace[f"t1_l{i}"] = t0.numpy().copy(), t1.numpy().copy()
+                trace[f"unconf_l{i}"] = int(unconf)
             if 1.0 - unconf / (m + n) > DEPTH_CONF:
                 break
             # lightglue.py:551-566,636-643 (pruning threshold -1 on CPU: always attempted)
             for side in (0, 1):
                 d, t = (d0, t0) if side == 0 else (d1, t1)
+                if len(d) <= prune_min_kpts:
+                    continue
                 ma = torch.sigmoid(_lin(sd, f"log_assignment.{i}.matchability", d))[:, 0]
                 keep = torch.where((ma > (1 - WIDTH_CONF)) | (t <= thr[i]))[0]
+                if trace is not None:
+                    trace[f"ma{side}_l{i}"], trace[f"keep{side}_l{i}"] = ma.numpy().copy(), keep.numpy().copy()
                 if side == 0:
                     ind0, d0, cs0 = ind0[keep], d0[keep], (cs0[0][keep], cs0[1][keep])
                 else:
