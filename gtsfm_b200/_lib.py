@@ -215,6 +215,8 @@ SIGNATURES = {
     "b2_superglue_set_weights": (_i, [_vp, _vp, _sz]),
     "b2_superglue_match_dev": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _vp, _ip, _vp]),
     "b2_superglue_match_host": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _vp, _ip]),
+    "b2_superglue_trace_count": (_i, [_vp]),
+    "b2_superglue_trace_get": (_i, [_vp, _i, _vp, _vp]),
     "b2_netvlad_blob_floats": (_sz, []),
     "b2_netvlad_set_weights": (_i, [_vp, _vp, _sz]),
     "b2_netvlad_describe_dev": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp]),

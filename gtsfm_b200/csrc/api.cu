@@ -85,6 +85,11 @@ extern "C" int b2_set_option(b2_context* ctx, const char* name, int64_t value) {
     ctx->lg_trace = (int)value;
     return B2_OK;
   }
+  if (!strcmp(name, "superglue_trace")) {  // 1: per-layer SuperGlue state copied to host memory (a test aid: it synchronises)
+    if (value != 0 && value != 1) return b2_fail(ctx, B2_ERR_ARG, "superglue_trace takes 0 or 1");
+    ctx->sg_trace = (int)value;
+    return B2_OK;
+  }
   if (!strcmp(name, "feature_cache")) {  // 0 (default): forget every cached upload and copy on every call; 1: cache
     if (value != 0 && value != 1) return b2_fail(ctx, B2_ERR_ARG, "feature_cache takes 0 or 1");
     ctx->fcache_on = (int)value;

@@ -131,6 +131,7 @@ struct b2_context {
   int vg_workspace_mb = 1024;  // view-graph filter: segment window of one chunk; b2_set_option "viewgraph_workspace_mb"
   int force_simt = -1;  // 1: models loaded afterwards run the exact-fp32 SIMT kernels (no tensor cores); -1 = B2_FORCE_SIMT env
   int lg_trace = 0;     // 1: b2_lightglue_match_* record each side's state after every layer (b2_lightglue_trace_get)
+  int sg_trace = 0;     // 1: b2_superglue_match_* record each side's state after every layer (b2_superglue_trace_get)
   std::string err;
   std::mutex mu;
   uint64_t launches = 0;

@@ -30,6 +30,12 @@ struct SgSide {
   int n = 0;
 };
 
+// One array of the match, recorded when b2_set_option("superglue_trace", 1) is set (b2_superglue_trace_get).
+struct SgTraceRec {
+  int layer = 0, side = 0, n = 0, kind = 0, cols = 0;  // kind 0: x [n][256] after `layer`; 1: md [n][256]; 2: Z [n][cols]
+  std::vector<float> v;
+};
+
 struct SuperGlueState {
   bool loaded = false, use_tc = true;
   DevBuf wblob, wblob_h, wblob_l, errflag;
@@ -39,6 +45,7 @@ struct SuperGlueState {
   float bin_score = 0.f;
   SgSide side[2];
   DevBuf sim, counters, attn_part, attn_ml, attn_cnt, sk_part, sk_bar;
+  std::vector<SgTraceRec> trace;
 };
 
 void sg_destroy(b2_context* ctx) {
@@ -395,11 +402,41 @@ static int sg_assign(b2_context* ctx, cudaStream_t st, const SgAssign& p, int pa
   return B2_OK;
 }
 
+// Appends the n x cols fp32 array in `d` to the trace (synchronises the stream).  With `planes`, `d` holds split-fp16
+// planes instead (hi [n * cols], then lo [n * cols] scaled by 2^11, as the wgmma path writes a linear's plane output): the
+// record is hi + lo * 2^-11, the value the next GEMM reads.
+static int sg_trace_push(b2_context* ctx, cudaStream_t st, SuperGlueState* s, int layer, int side, int kind, int n, int cols,
+                         const DevBuf& d, bool planes) {
+  B2_CUDA(ctx, cudaStreamSynchronize(st));
+  SgTraceRec r;
+  r.layer = layer, r.side = side, r.n = n, r.kind = kind, r.cols = cols;
+  const size_t e = (size_t)n * cols;
+  r.v.resize(e);
+  if (planes) {
+    std::vector<__half> h(2 * e);
+    B2_CUDA(ctx, cudaMemcpy(h.data(), d.p, h.size() * sizeof(__half), cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < e; ++i) r.v[i] = (float)((double)__half2float(h[i]) + (double)__half2float(h[e + i]) / (double)tc::LO_SCALE);
+  } else {
+    B2_CUDA(ctx, cudaMemcpy(r.v.data(), d.p, e * sizeof(float), cudaMemcpyDeviceToHost));
+  }
+  s->trace.push_back(std::move(r));
+  return B2_OK;
+}
+
+static int sg_trace_x(b2_context* ctx, cudaStream_t st, SuperGlueState* s, int layer) {
+  for (int i = 0; i < 2; ++i) {
+    int rc = sg_trace_push(ctx, st, s, layer, i, 0, s->side[i].n, 256, s->side[i].x, false);
+    if (rc) return rc;
+  }
+  return B2_OK;
+}
+
 static int sg_match_impl(b2_context* ctx,const float* kp0, const float* sc0, const float* desc0, int n0, int h0, int w0,
                          const float* kp1, const float* sc1, const float* desc1, int n1, int h1, int w1, int iters, float thr,
                          unsigned* out_matches, float* out_scores, int* out_k, cudaStream_t st) {
   SuperGlueState* s = ctx->sg;
   if (!s || !s->loaded) return b2_fail(ctx, B2_ERR_STATE, "superglue weights not set");
+  s->trace.clear();
   *out_k = 0;
   if (n0 <= 0 || n1 <= 0) return B2_OK;  // superglue.py:233-240
   TcWeights tw{s->wblob.as<float>(), s->wblob_h.as<__half>(), s->wblob_l.as<__half>(), s->errflag.as<int>(), s->use_tc};
@@ -428,6 +465,7 @@ static int sg_match_impl(b2_context* ctx,const float* kp0, const float* sc0, con
               fmaxf(fw, fh) * 0.7f, kw, sd.x.as<float>(), s->use_tc ? xp.hi : (__half*)nullptr, s->use_tc ? xp.lo : (__half*)nullptr);
     B2_CHECK_LAUNCH(ctx);
   }
+  if (ctx->sg_trace && (rc = sg_trace_x(ctx, st, s, -1))) return rc;
   SgSide &a = s->side[0], &b = s->side[1];
   auto PL = [](DevBuf& buf, int n, int width) { return planes_of(buf, (size_t)n * width); };
   for (int l = 0; l < SG_LAYERS; ++l) {
@@ -470,6 +508,7 @@ static int sg_match_impl(b2_context* ctx,const float* kp0, const float* sc0, con
     if ((rc = run_linear(ctx, st, tw, mg, 2))) return rc;
     if ((rc = run_linear(ctx, st, tw, f0, 2))) return rc;
     if ((rc = run_linear(ctx, st, tw, f3, 2))) return rc;
+    if (ctx->sg_trace && (rc = sg_trace_x(ctx, st, s, l))) return rc;
   }
   // final projection + score matrix / sqrt(256) (superglue.py:251-258)
   {
@@ -481,6 +520,8 @@ static int sg_match_impl(b2_context* ctx,const float* kp0, const float* sc0, con
       g.cf = sd.md.as<float>(), g.ldc = 256, g.cp = PL(sd.md, sd.n, 256), g.ldch = 256, g.M = sd.n, g.N = 256;
     }
     if ((rc = run_linear(ctx, st, tw, p, 2))) return rc;
+    for (int i = 0; ctx->sg_trace && i < 2; ++i)
+      if ((rc = sg_trace_push(ctx, st, s, SG_LAYERS, i, 1, s->side[i].n, 256, s->side[i].md, s->use_tc))) return rc;
   }
   const int M = a.n, N = b.n;
   B2_CUDA(ctx, s->sim.ensure((size_t)M * N * 4));
@@ -489,6 +530,7 @@ static int sg_match_impl(b2_context* ctx,const float* kp0, const float* sc0, con
   gs.bf = b.md.as<float>(), gs.bp = PL(b.md, b.n, 256), gs.ldb = 256, gs.scale = 1.0f / 16.0f;
   gs.cf = s->sim.as<float>(), gs.ldc = N, gs.tc_want_f32 = true, gs.M = M, gs.N = N;
   if ((rc = run_linear(ctx, st, tw, &gs, 1))) return rc;
+  if (ctx->sg_trace && (rc = sg_trace_push(ctx, st, s, SG_LAYERS, -1, 2, M, N, s->sim, false))) return rc;
   // log-space Sinkhorn (superglue.py:141-170); u lives in a.u [M+1], v in b.vv [N+1]
   int* counters = s->counters.as<int>();
   const SgAssign sg{s->sim.as<float>(), M, N, s->bin_score, iters, thr, a.u.as<float>(), b.vv.as<float>(), a.best.as<float>(),
@@ -545,6 +587,25 @@ extern "C" int b2_superglue_match_host(b2_context* ctx, const float* kp0, const 
     if (out_scores) B2_CUDA(ctx, cudaMemcpyAsync(out_scores, ctx->stage_d[7].p, (size_t)*out_k * 4, cudaMemcpyDeviceToHost, st));
     B2_CUDA(ctx, cudaStreamSynchronize(st));
   }
+  return B2_OK;
+}
+
+// ---- the per-layer trace (b2_set_option "superglue_trace") ------------------------------------------------------------------
+
+extern "C" int b2_superglue_trace_count(b2_context* ctx) {
+  if (!ctx) return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  return ctx->sg ? (int)ctx->sg->trace.size() : 0;
+}
+
+extern "C" int b2_superglue_trace_get(b2_context* ctx, int i, int* meta, float* out) {
+  if (!ctx || !meta) return B2_ERR_ARG;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (!ctx->sg || i < 0 || i >= (int)ctx->sg->trace.size()) return b2_fail(ctx, B2_ERR_ARG, "no such superglue trace record");
+  const SgTraceRec& r = ctx->sg->trace[i];
+  const int m[5] = {r.layer, r.side, r.n, r.kind, r.cols};
+  memcpy(meta, m, sizeof(m));
+  if (out) memcpy(out, r.v.data(), r.v.size() * sizeof(float));
   return B2_OK;
 }
 

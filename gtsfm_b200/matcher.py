@@ -160,6 +160,20 @@ class SuperGlueEngine:
             return out[: k.value].copy(), sc[: k.value].copy()
         return out[: k.value].copy()
 
+    def layer_trace(self):
+        """The arrays the last match call recorded under set_option("superglue_trace", 1), in the order recorded
+        (include/gtsfm_b200.h, b2_superglue_trace_get): one dict per record with `kind` "x" (layer -1 .. 17), "md" or "Z"."""
+        lib, h = self.ctx.lib, self.ctx.handle
+        recs = []
+        for i in range(lib.b2_superglue_trace_count(h)):
+            meta = np.zeros(5, np.int32)
+            self.ctx.check(lib.b2_superglue_trace_get(h, i, _lib.ptr(meta), None), "superglue_trace_get")
+            layer, side, n, kind, cols = (int(v) for v in meta)
+            v = np.empty((n, cols), np.float32)
+            self.ctx.check(lib.b2_superglue_trace_get(h, i, _lib.ptr(meta), _lib.ptr(v)), "superglue_trace_get")
+            recs.append(dict(layer=layer, side=side, n=n, kind=("x", "md", "Z")[kind], v=v))
+        return recs
+
 
 class B200SuperGlueMatcher(MatcherBase):
     """SuperGlue on hand-written sm_90a kernels behind GTSfM's MatcherBase (gtsfm/frontend/matcher/superglue_matcher.py:30-115)."""

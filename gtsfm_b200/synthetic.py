@@ -122,7 +122,9 @@ def superglue_state_dict(seed: int = 1, profile: str = "full") -> Dict[str, np.n
 
     ``profile="sharp"`` scales the identity part of ``final_proj`` (12 -> 32) so that true correspondences still win the
     optimal transport against thousands of distractors (the 2048- and 5000-keypoint fixtures and the bench workload); every
-    other tensor is identical to the default profile (the RNG stream is consumed in the same order)."""
+    other tensor is identical to the default profile (the RNG stream is consumed in the same order).  ``profile="attn"``
+    scales the q and k projections by 8, so that attention logits are O(1) and each softmax is far from uniform (with the
+    default weights they are O(0.03), and the attention scale barely reaches the output)."""
     rng = np.random.default_rng(seed)
     sd: Dict[str, np.ndarray] = {}
     d = 256
@@ -154,6 +156,10 @@ def superglue_state_dict(seed: int = 1, profile: str = "full") -> Dict[str, np.n
         conv1d(p + "mlp.0", 2 * d, 2 * d, gain=1.0)
         bn(p + "mlp.1", 2 * d)
         conv1d(p + "mlp.3", d, 2 * d, gain=0.03, bias_std=0.0)
+    if profile == "attn":
+        for i in range(18):
+            for j in range(2):
+                sd[f"gnn.layers.{i}.attn.proj.{j}.weight"] *= np.float32(8.0)
     w, b = _lin(rng, d, d, gain=0.15, bias_std=0.0)
     fgain = 32.0 if profile == "sharp" else 12.0
     sd["final_proj.weight"] = (w + fgain * np.eye(d, dtype=np.float32))[:, :, None].astype(np.float32)

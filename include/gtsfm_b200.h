@@ -51,6 +51,7 @@ uint64_t b2_h2d_bytes(const b2_context* ctx);
  * "force_simt" = 0 | 1: models whose weights are set afterwards run the exact-fp32 SIMT kernels instead of the wgmma
  * split-fp16 ones (the on-device cross-check of the tensor-core path; tests only).
  * "lightglue_trace" = 0 | 1: (1) record LightGlue's per-layer state in host memory (b2_lightglue_trace_get; tests only).
+ * "superglue_trace" = 0 | 1: (1) record SuperGlue's per-layer state in host memory (b2_superglue_trace_get; tests only).
  * "ransac_workspace_mb" = 1..: device workspace one sub-batch of b2_ransac_verify_batched_dev may use (default 1024); a call with
  * more problems than fit is cut into consecutive sub-batches, which changes no result.
  * "viewgraph_workspace_mb" = 1..: the segment window of one chunk of b2_viewgraph_cycle_filter_host's MEDIAN (default 1024);
@@ -327,6 +328,14 @@ int b2_superglue_match_host(b2_context* ctx, const float* kp0, const float* scor
                             int w0, const float* kp1, const float* score1, const float* desc1, int n1, int h1, int w1,
                             int sinkhorn_iters, float match_threshold, uint32_t* out_matches, float* out_scores,
                             int* out_k);
+/* The per-layer trace, recorded by every b2_superglue_match_* call (and cleared at its start) while
+ * b2_set_option("superglue_trace", 1) is set; off by default (it synchronises after every layer).  meta [5] = (layer, side,
+ * n rows, kind, columns); out receives n x columns floats, row-major.  Records, in order: kind 0, x [n][256] of side 0 and 1
+ * after the keypoint encoder (layer -1) and after each GNN layer 0..17; kind 1, final_proj's md [n][256] of side 0 and 1
+ * (layer 18); kind 2, the score matrix Z = md0 md1^T / 16 [M][N] (layer 18, side -1).  A NULL `out` is skipped: call once
+ * with meta only to size it. */
+int b2_superglue_trace_count(b2_context* ctx);
+int b2_superglue_trace_get(b2_context* ctx, int i, int* meta, float* out);
 
 /* ---- RANSAC verifier --------------------------------------------------------------------------------------------- */
 typedef struct b2_ransac_params {
