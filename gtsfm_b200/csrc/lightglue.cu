@@ -19,11 +19,12 @@ constexpr int LG_LAYERS = 9;
 constexpr size_t LG_NFLOATS = 11851601;
 constexpr int D = 256;
 
+// w0 / b0: ffn.0 with the attention output projection folded in (weights.pack_lightglue), so it reads cat[x, ctx]
 struct SelfW {
-  float *wqkv, *bqkv, *wout, *bout, *w0, *b0, *lng, *lnb, *w3, *b3;  // wqkv / bqkv rows in b2_lightglue_qkv_rows order
+  float *wqkv, *bqkv, *w0, *b0, *lng, *lnb, *w3, *b3;  // wqkv / bqkv rows in b2_lightglue_qkv_rows order
 };
 struct CrossW {
-  float *wqv, *bqv, *wout, *bout, *w0, *b0, *lng, *lnb, *w3, *b3;  // wqv [512][256] = [to_qk; to_v], bqv [512] likewise
+  float *wqv, *bqv, *w0, *b0, *lng, *lnb, *w3, *b3;  // wqv [512][256] = [to_qk; to_v], bqv [512] likewise
 };
 struct AssignW {
   float *wm, *bm, *wf, *bf;
@@ -38,7 +39,7 @@ constexpr int LG_MAX_SIDES = 2 * LG_MAX_PAIRS;  // = GW_MAXP = AP_MAXP problems 
 static_assert(LG_MAX_SIDES <= GW_MAXP && LG_MAX_SIDES <= AP_MAXP, "batch does not fit one launch");
 
 struct LgSide {  // per-image workspace
-  DevBuf x[2], xs[2], qkv, q, k, v, ctx, msg, h, hs, cs[2], sn[2], ind[2], conf, mat, src, md, rmax, rlog, ls, lsg, amax, aidx;
+  DevBuf x[2], xs[2], qkv, q, k, v, ctx, h, hs, cs[2], sn[2], ind[2], conf, mat, src, md, rmax, rlog, ls, lsg, amax, aidx;
   int cur = 0;  // which of x / xs / cs / sn / ind is live
   int n = 0;
   int cap = 0;  // rows allocated; split-plane buffers keep their lo plane at +cap * width halves whatever n shrinks to
@@ -700,6 +701,11 @@ extern "C" int b2_lightglue_set_weights(b2_context* ctx, const float* blob, size
   }
   for (size_t i = 0; i < sizes.size(); ++i) soff[i] = src_total, src_total += sizes[i];
   if (src_total != LG_NFLOATS) return b2_fail(ctx, B2_ERR_STATE, "internal lightglue layout mismatch");
+  for (int i = 0; i < LG_LAYERS; ++i)  // out_proj, to_out
+    for (size_t t : {1 + LAYER_T * i + 2, 1 + LAYER_T * i + SELF_T + 4})
+      if (!folded_projection(blob + soff[t], blob + soff[t + 1], D))
+        return b2_fail(ctx, B2_ERR_ARG, "lightglue blob: layer " + std::to_string(i) + "'s attention output projections are not folded "
+                                        "into ffn.0 (pack the checkpoint with weights.pack_lightglue)");
   std::vector<float> host(total, 0.f);
   for (size_t i = 0; i < sizes.size(); ++i) memcpy(host.data() + doff[i], blob + soff[i], sizes[i] * sizeof(float));
   int qkv_rows[3 * D];
@@ -719,11 +725,12 @@ extern "C" int b2_lightglue_set_weights(b2_context* ctx, const float* blob, size
   s->wr = next();
   for (int i = 0; i < LG_LAYERS; ++i) {
     SelfW& a = s->sw[i];
-    a.wqkv = next(), a.bqkv = next(), a.wout = next(), a.bout = next(), a.w0 = next(), a.b0 = next(), a.lng = next(),
-    a.lnb = next(), a.w3 = next(), a.b3 = next();
+    a.wqkv = next(), a.bqkv = next(), next(), next();  // out_proj: the identity (folded)
+    a.w0 = next(), a.b0 = next(), a.lng = next(), a.lnb = next(), a.w3 = next(), a.b3 = next();
     CrossW& c = s->cw[i];
     c.wqv = next(), c.bqv = next(), next(), next();  // to_v's weight and bias sit right behind to_qk's
-    c.wout = next(), c.bout = next(), c.w0 = next(), c.b0 = next(), c.lng = next(), c.lnb = next(), c.w3 = next(), c.b3 = next();
+    next(), next();                                  // to_out: the identity (folded)
+    c.w0 = next(), c.b0 = next(), c.lng = next(), c.lnb = next(), c.w3 = next(), c.b3 = next();
   }
   for (int i = 0; i < LG_LAYERS; ++i) {
     AssignW& a = s->aw[i];
@@ -776,7 +783,6 @@ static int lg_side_alloc(b2_context* ctx, LgSide& sd, int n, bool use_tc) {
   B2_CUDA(ctx, sd.k.ensure(N * 256 * 4));
   B2_CUDA(ctx, sd.v.ensure(N * 256 * 4));
   B2_CUDA(ctx, sd.ctx.ensure(N * 256 * 4));
-  B2_CUDA(ctx, sd.msg.ensure(N * 256 * 4));
   B2_CUDA(ctx, sd.h.ensure(N * 512 * 4));
   B2_CUDA(ctx, sd.hs.ensure(N * 512 * 4));
   B2_CUDA(ctx, sd.md.ensure(N * 256 * 4));
@@ -805,25 +811,23 @@ static int lg_max_n(const LightGlueState* s, const LgActive& act) {
   return mx;
 }
 
-// x + ffn(cat[x, msg])  (lightglue.py:152-157,172,228-229): Linear(512,512) -> LN -> GELU -> Linear(512,256) + x, preceded
-// by the attention output projection (out_proj / to_out); every image of the batch goes through each GEMM together.
-// `blk` ("lg_self" / "lg_cross") prefixes the profiler labels of the three GEMM call sites.
-static int lg_out_and_ffn(b2_context* ctx, cudaStream_t st, LightGlueState* s, const LgActive& act, const char* blk, const float* wout,
-                          const float* bout, const float* w0, const float* b0, const float* lng, const float* lnb, const float* w3,
-                          const float* b3) {
+// x + ffn(cat[x, msg]) with msg = out(ctx)  (lightglue.py:152-157,172,228-229): Linear(512,512) -> LN -> GELU ->
+// Linear(512,256) + x.  The message projection (out_proj / to_out) is folded into the first linear on the host
+// (weights.fold_message_projection), so that linear reads cat[x, ctx] straight from the attention output; every image of
+// the batch goes through each GEMM together.  `blk` ("lg_self" / "lg_cross") prefixes the profiler labels of the two GEMM
+// call sites.
+static int lg_ffn(b2_context* ctx, cudaStream_t st, LightGlueState* s, const LgActive& act, const char* blk, const float* w0,
+                  const float* b0, const float* lng, const float* lnb, const float* w3, const float* b3) {
   int rc;
   const TcWeights tw = lg_tw(s);
-  LinArgs o[LG_MAX_SIDES], f0[LG_MAX_SIDES], f3[LG_MAX_SIDES];
+  LinArgs f0[LG_MAX_SIDES], f3[LG_MAX_SIDES];
   for (int i = 0; i < act.n; ++i) {
     LgSide& sd = s->side[act.side[i]];
     const size_t e = (size_t)sd.cap * 256;
     float* x = sd.x[sd.cur].as<float>();
-    LinArgs& a = o[i];
-    a.a1f = sd.ctx.as<float>(), a.a1p = planes_of(sd.ctx, e), a.lda1 = 256, a.K1 = 256, a.w = wout, a.ldb = 256, a.bias = bout;
-    a.cf = sd.msg.as<float>(), a.ldc = 256, a.cp = planes_of(sd.msg, e), a.ldch = 256, a.M = sd.n, a.N = 256;
     LinArgs& f = f0[i];
     f.a1f = x, f.a1p = planes_of(sd.xs[sd.cur], e), f.lda1 = 256, f.K1 = 256;
-    f.a2f = sd.msg.as<float>(), f.a2p = planes_of(sd.msg, e), f.lda2 = 256, f.K2 = 256;
+    f.a2f = sd.ctx.as<float>(), f.a2p = planes_of(sd.ctx, e), f.lda2 = 256, f.K2 = 256;
     f.w = w0, f.ldb = 512, f.bias = b0, f.cf = sd.h.as<float>(), f.ldc = 512, f.tc_want_f32 = true, f.M = sd.n, f.N = 512;
     LinArgs& c = f3[i];
     c.a1f = sd.h.as<float>(), c.a1p = planes_of(sd.hs, (size_t)sd.cap * 512), c.lda1 = 512, c.K1 = 512, c.w = w3, c.ldb = 512, c.bias = b3;
@@ -831,7 +835,6 @@ static int lg_out_and_ffn(b2_context* ctx, cudaStream_t st, LightGlueState* s, c
     c.cf = x, c.ldc = 256, c.tc_want_f32 = true, c.cp = planes_of(sd.xs[sd.cur], e), c.ldch = 256, c.M = sd.n, c.N = 256;
   }
   const std::string site(blk);
-  if ((rc = run_linear(ctx, st, tw, o, act.n, (site + "_out").c_str()))) return rc;
   if ((rc = run_linear(ctx, st, tw, f0, act.n, (site + "_ffn0").c_str()))) return rc;
   {
     JobList<LnJob> lj{};
@@ -887,7 +890,7 @@ static int lg_self_layer(b2_context* ctx, cudaStream_t st, LightGlueState* s, co
     fj[i] = {&a.q, &a.k, &a.v, &a.ctx, a.n, a.n, a.cap, a.cap};
   }
   if ((rc = run_flash(ctx, st, tw, fj, act.n, 0.125f, fp16_attn))) return rc;
-  return lg_out_and_ffn(ctx, st, s, act, "lg_self", w.wout, w.bout, w.w0, w.b0, w.lng, w.lnb, w.w3, w.b3);
+  return lg_ffn(ctx, st, s, act, "lg_self", w.w0, w.b0, w.lng, w.lnb, w.w3, w.b3);
 }
 
 static int lg_cross_block(b2_context* ctx, cudaStream_t st, LightGlueState* s, const LgActive& act, int layer, bool fp16_attn) {
@@ -913,7 +916,7 @@ static int lg_cross_block(b2_context* ctx, cudaStream_t st, LightGlueState* s, c
     fj[i] = {&a.q, &b.q, &b.v, &a.ctx, a.n, b.n, a.cap, b.cap};
   }
   if ((rc = run_flash(ctx, st, tw, fj, act.n, 0.125f, fp16_attn))) return rc;
-  return lg_out_and_ffn(ctx, st, s, act, "lg_cross", w.wout, w.bout, w.w0, w.b0, w.lng, w.lnb, w.w3, w.b3);
+  return lg_ffn(ctx, st, s, act, "lg_cross", w.w0, w.b0, w.lng, w.lnb, w.w3, w.b3);
 }
 
 // Network input of the sides in `act` (kp[i], desc[i] belong to act.side[i]): x = desc and its split planes, the rotary

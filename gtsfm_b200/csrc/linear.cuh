@@ -25,6 +25,18 @@ struct Pl {  // split-fp16 planes of an activation
 };
 static inline Pl planes_of(const DevBuf& b, size_t elems) { return {b.as<__half>(), b.as<__half>() + elems}; }
 
+// The packers (weights.fold_message_projection) fold each attention output projection into the feed-forward linear that
+// reads the message and leave the identity in its place; a blob whose projection is anything else was not folded, and
+// running it without that projection would compute another network.
+static inline bool folded_projection(const float* w /*[d][d]*/, const float* b /*[d]*/, int d) {
+  for (int r = 0; r < d; ++r) {
+    if (b[r] != 0.f) return false;
+    for (int c = 0; c < d; ++c)
+      if (w[(size_t)r * d + c] != (r == c ? 1.f : 0.f)) return false;
+  }
+  return true;
+}
+
 // One linear / GEMM call site of ONE problem, expressed for both execution paths: fp32 views feed the exact-fp32 SIMT
 // kernel, split-fp16 plane views feed the wgmma kernel.
 struct LinArgs {

@@ -10,6 +10,8 @@
 // as an nn.Linear and shares the wgmma split-fp16 kernels with LightGlue.  The host loader has already folded the
 // eval-mode BatchNorms and permuted the q/k/v projection rows (and the merge columns) from the reference's
 // channel = dim * 4 + head interleave (superglue.py:104) to head-major, so attention runs on plain [4][N][64] operands.
+// It has also folded each layer's merge into its mlp.0 (weights.fold_message_projection): mlp.0 reads cat[x, ctx]
+// straight from the attention output, and the message itself is never formed.
 // The (M+1) x (N+1) coupling matrix is never materialised: the dustbin row / column are handled analytically.
 #include <stdlib.h>
 
@@ -21,12 +23,12 @@ namespace {
 constexpr int SG_LAYERS = 18;
 constexpr size_t SG_NFLOATS = 12003905;
 struct SgLayerW {
-  float *wq, *bq, *wk, *bk, *wv, *bv, *wm, *bm, *w0, *b0, *w3, *b3;
+  float *wq, *bq, *wk, *bk, *wv, *bv, *w0, *b0, *w3, *b3;  // w0 / b0: mlp.0 with merge folded in
 };
 }  // namespace
 
 struct SgSide {
-  DevBuf x, xs, q, k, v, ctx, msg, h, hs, md, u, vv, best, arg;
+  DevBuf x, xs, q, k, v, ctx, h, hs, md, u, vv, best, arg;
   int n = 0;
 };
 
@@ -305,6 +307,9 @@ extern "C" int b2_superglue_set_weights(b2_context* ctx, const float* blob, size
   std::vector<float> host(total, 0.f);
   size_t so = 0;
   for (size_t i = 0; i < sizes.size(); ++i) {
+    if (i >= 10 && (i - 10) % 12 == 6 && !folded_projection(blob + so, blob + so + sizes[i], 256))  // attn.merge of a GNN layer
+      return b2_fail(ctx, B2_ERR_ARG, "superglue blob: layer " + std::to_string((i - 10) / 12) + "'s attn.merge is not folded into "
+                                      "mlp.0 (pack the checkpoint with weights.pack_superglue)");
     memcpy(host.data() + doff[i], blob + so, sizes[i] * sizeof(float));
     so += sizes[i];
   }
@@ -326,7 +331,7 @@ extern "C" int b2_superglue_set_weights(b2_context* ctx, const float* blob, size
   for (int l = 0; l < 5; ++l) s->kw[l] = next(), s->kb[l] = next();
   for (int l = 0; l < SG_LAYERS; ++l) {
     SgLayerW& w = s->lw[l];
-    w.wq = next(), w.bq = next(), w.wk = next(), w.bk = next(), w.wv = next(), w.bv = next(), w.wm = next(), w.bm = next();
+    w.wq = next(), w.bq = next(), w.wk = next(), w.bk = next(), w.wv = next(), w.bv = next(), next(), next();  // merge: the identity
     w.w0 = next(), w.b0 = next(), w.w3 = next(), w.b3 = next();
   }
   s->wf = next(), s->bf = next();
@@ -453,7 +458,7 @@ static int sg_match_impl(b2_context* ctx,const float* kp0, const float* sc0, con
     SgSide& sd = s->side[i];
     const size_t N = (size_t)ns[i];
     sd.n = ns[i];
-    DevBuf* b256[] = {&sd.x, &sd.xs, &sd.q, &sd.k, &sd.v, &sd.ctx, &sd.msg, &sd.md};
+    DevBuf* b256[] = {&sd.x, &sd.xs, &sd.q, &sd.k, &sd.v, &sd.ctx, &sd.md};
     for (DevBuf* b : b256) B2_CUDA(ctx, b->ensure(N * 256 * 4));
     B2_CUDA(ctx, sd.h.ensure(N * 512 * 4));
     B2_CUDA(ctx, sd.hs.ensure(N * 512 * 4));
@@ -489,15 +494,12 @@ static int sg_match_impl(b2_context* ctx,const float* kp0, const float* sc0, con
     SgSide &sa = cross ? b : a, &sb = cross ? a : b;  // sources of image 0 / image 1
     const FlashJob fj[2] = {{&a.q, &sa.k, &sa.v, &a.ctx, a.n, sa.n, a.n, sa.n}, {&b.q, &sb.k, &sb.v, &b.ctx, b.n, sb.n, b.n, sb.n}};
     if ((rc = run_flash(ctx, st, tw, fj, 2, 0.125f))) return rc;
-    LinArgs mg[2], f0[2], f3[2];
+    LinArgs f0[2], f3[2];
     for (int i = 0; i < 2; ++i) {
       SgSide& sd = s->side[i];
-      LinArgs& m = mg[i];
-      m.a1f = sd.ctx.as<float>(), m.a1p = PL(sd.ctx, sd.n, 256), m.lda1 = 256, m.K1 = 256, m.w = w.wm, m.ldb = 256, m.bias = w.bm;
-      m.cf = sd.msg.as<float>(), m.ldc = 256, m.cp = PL(sd.msg, sd.n, 256), m.ldch = 256, m.M = sd.n, m.N = 256;
-      LinArgs& f = f0[i];  // mlp.0 (BatchNorm folded) + ReLU on cat([x, message])
+      LinArgs& f = f0[i];  // mlp.0 (BatchNorm and merge folded) + ReLU on cat([x, ctx]) = mlp.0 on cat([x, message])
       f.a1f = sd.x.as<float>(), f.a1p = PL(sd.xs, sd.n, 256), f.lda1 = 256, f.K1 = 256;
-      f.a2f = sd.msg.as<float>(), f.a2p = PL(sd.msg, sd.n, 256), f.lda2 = 256, f.K2 = 256;
+      f.a2f = sd.ctx.as<float>(), f.a2p = PL(sd.ctx, sd.n, 256), f.lda2 = 256, f.K2 = 256;
       f.w = w.w0, f.ldb = 512, f.bias = w.b0, f.relu = 1, f.cf = sd.h.as<float>(), f.ldc = 512, f.cp = PL(sd.hs, sd.n, 512), f.ldch = 512;
       f.M = sd.n, f.N = 512;
       LinArgs& c = f3[i];  // desc + mlp.3(...)  (superglue.py:136-137)
@@ -505,7 +507,6 @@ static int sg_match_impl(b2_context* ctx,const float* kp0, const float* sc0, con
       c.resid = sd.x.as<float>(), c.ldr = 256, c.cf = sd.x.as<float>(), c.ldc = 256, c.tc_want_f32 = true;
       c.cp = PL(sd.xs, sd.n, 256), c.ldch = 256, c.M = sd.n, c.N = 256;
     }
-    if ((rc = run_linear(ctx, st, tw, mg, 2))) return rc;
     if ((rc = run_linear(ctx, st, tw, f0, 2))) return rc;
     if ((rc = run_linear(ctx, st, tw, f3, 2))) return rc;
     if (ctx->sg_trace && (rc = sg_trace_x(ctx, st, s, l))) return rc;

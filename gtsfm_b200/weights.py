@@ -84,11 +84,30 @@ def pack_lightglue(sd: StateDict) -> np.ndarray:
             for k in list(sd):
                 if k.startswith(old + "."):
                     sd[k.replace(old, new, 1)] = sd.pop(k)
+    for i in range(LIGHTGLUE_LAYERS):
+        for blk, out in (("self_attn", "out_proj"), ("cross_attn", "to_out")):
+            p = f"transformers.{i}.{blk}."
+            fold_message_projection(sd, p + out, p + "ffn.0")
     return _pack(sd, LIGHTGLUE_ORDER)
 
 
-def fold_superglue_batchnorm(sd: StateDict, eps: float = 1e-5) -> StateDict:
-    """eval-mode BatchNorm1d folded into the preceding k=1 Conv1d: w' = w * g / sqrt(var + eps), b' = (b - mu) * g / sqrt(var + eps) + beta."""
+def fold_message_projection(sd: StateDict, out: str, ffn0: str) -> None:
+    """In place: the attention output projection `out` folded into the linear `ffn0` that reads cat[x, out(ctx)], in fp64:
+    W0 [x; Wo ctx + bo] + b0 = [W0a | W0b Wo] [x; ctx] + (b0 + W0b bo).  `out` becomes the identity with a zero bias, so the
+    blob keeps its layout and still describes the same network; the device skips it and feeds ctx to `ffn0` directly.  The
+    folded tensors stay fp64 here and are rounded to fp32 once, by _pack."""
+    wo, bo = np.asarray(sd[out + ".weight"], np.float64), np.asarray(sd[out + ".bias"], np.float64)
+    w0, b0 = np.asarray(sd[ffn0 + ".weight"], np.float64), np.asarray(sd[ffn0 + ".bias"], np.float64)
+    m = wo.shape[0]  # the message fills the last m inputs of ffn0
+    sd[ffn0 + ".weight"] = np.concatenate([w0[:, :-m], w0[:, -m:] @ wo], 1)
+    sd[ffn0 + ".bias"] = b0 + w0[:, -m:] @ bo
+    sd[out + ".weight"] = np.eye(m, wo.shape[1], dtype=np.float32)
+    sd[out + ".bias"] = np.zeros(m, np.float32)
+
+
+def fold_superglue_batchnorm(sd: StateDict, eps: float = 1e-5, dtype=np.float32) -> StateDict:
+    """eval-mode BatchNorm1d folded into the preceding k=1 Conv1d: w' = w * g / sqrt(var + eps), b' = (b - mu) * g / sqrt(var + eps) + beta.
+    The folded tensors and the squeezed k=1 weights come out as `dtype` (np.float64 leaves them for a further fold)."""
     out: StateDict = {}
     pairs = [(f"kenc.encoder.{i}", f"kenc.encoder.{i + 1}") for i in (0, 3, 6, 9)]
     pairs += [(f"gnn.layers.{l}.mlp.0", f"gnn.layers.{l}.mlp.1") for l in range(SUPERGLUE_GNN_LAYERS)]
@@ -101,15 +120,15 @@ def fold_superglue_batchnorm(sd: StateDict, eps: float = 1e-5) -> StateDict:
         mu = np.asarray(sd[bn + ".running_mean"], np.float64)
         var = np.asarray(sd[bn + ".running_var"], np.float64)
         scale = g / np.sqrt(var + eps)
-        out[conv + ".weight"] = (w * scale[:, None]).astype(np.float32)
-        out[conv + ".bias"] = ((b - mu) * scale + beta).astype(np.float32)
+        out[conv + ".weight"] = (w * scale[:, None]).astype(dtype)
+        out[conv + ".bias"] = ((b - mu) * scale + beta).astype(dtype)
         folded.add(conv)
     for k, v in sd.items():
         base = k.rsplit(".", 1)[0]
         if base in folded or k in out:
             continue
         a = np.asarray(v)
-        out[k] = a[:, :, 0].astype(np.float32) if (a.ndim == 3 and a.shape[2] == 1) else a
+        out[k] = a[:, :, 0].astype(dtype) if (a.ndim == 3 and a.shape[2] == 1) else a
     return out
 
 
@@ -130,7 +149,12 @@ def superglue_head_major(sd: StateDict) -> StateDict:
 
 
 def pack_superglue(sd: StateDict) -> np.ndarray:
-    return _pack(superglue_head_major(fold_superglue_batchnorm(sd)), SUPERGLUE_ORDER)
+    """BatchNorm folded, attention channels head-major, then each layer's merge folded into its mlp.0 (after the
+    permutation, so the folded columns are head-major too); every folded tensor is rounded to fp32 once."""
+    fsd = superglue_head_major(fold_superglue_batchnorm(sd, dtype=np.float64))
+    for l in range(SUPERGLUE_GNN_LAYERS):
+        fold_message_projection(fsd, f"gnn.layers.{l}.attn.merge", f"gnn.layers.{l}.mlp.0")
+    return _pack(fsd, SUPERGLUE_ORDER)
 
 
 # ---- NetVLAD (thirdparty/hloc/netvlad.py) ---------------------------------------------------------------------------------------

@@ -232,7 +232,8 @@ int b2_image_resize_dev(b2_context* ctx, const uint8_t* src, int height, int wid
 /* ---- LightGlue --------------------------------------------------------------------------------------------------- */
 /* `blob`: packed fp32 tensors in the order documented in gtsfm_b200/weights.py::LIGHTGLUE_ORDER (nn.Linear layout
  * (out,in) row-major as in the checkpoint).  n_floats must equal 11851601 (the 251 parameter tensors; the
- * confidence_thresholds buffer is recomputed). */
+ * confidence_thresholds buffer is recomputed).  As weights.pack_lightglue writes it, each block's out_proj / to_out is
+ * folded into its ffn.0 and its own slot holds the identity with a zero bias; any other projection there is refused. */
 int b2_lightglue_set_weights(b2_context* ctx, const float* host_blob, size_t n_floats);
 /* Host-only, needs no device: out[r] (768 ints) = the checkpoint row of each self block's QKV projection that the device
  * copy holds at row r.  The device copy is [q | k | v], 256 rows each in head-major order h * 64 + j; the checkpoint
@@ -316,7 +317,8 @@ int b2_lightglue_encode_batched_dev(b2_context* ctx, const b2_lightglue_image* i
 
 /* ---- SuperGlue --------------------------------------------------------------------------------------------------- */
 /* `blob`: packed fp32 tensors in gtsfm_b200/weights.py::SUPERGLUE_ORDER with eval-mode BatchNorm already folded
- * into the preceding Conv1d by the host loader. */
+ * into the preceding Conv1d by the host loader, and each GNN layer's attn.merge folded into its mlp.0 (the merge slot
+ * holds the identity with a zero bias; any other merge is refused), as weights.pack_superglue writes it. */
 int b2_superglue_set_weights(b2_context* ctx, const float* host_blob, size_t n_floats);
 /* score: [n] keypoint responses; (h, w): image sizes used for keypoint normalisation (superglue.py:63-70).
  * out_matches: [min(n0,n1)][2] uint32 rows (i, matches0[i]) ascending in i. */
