@@ -165,6 +165,14 @@ class ViewGraphParams(C.Structure):  # b2_viewgraph_params
 
 VG_MEDIAN, VG_MIN = 0, 1  # B2_VG_MEDIAN, B2_VG_MIN
 
+
+class TriangulationParams(C.Structure):  # b2_triangulation_params
+    _fields_ = [("mode", C.c_int), ("num_hypotheses", C.c_int), ("reproj_error_threshold", C.c_double),
+                ("min_triangulation_angle", C.c_double), ("seed", C.c_uint64)]
+
+
+TRI_NO_RANSAC, TRI_SAMPLE_UNIFORM = 0, 1  # B2_TRI_NO_RANSAC, B2_TRI_SAMPLE_UNIFORM
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 
@@ -241,6 +249,8 @@ SIGNATURES = {
     "b2_twoview_eval_batched_dev": (_i, [_vp, C.POINTER(TwoViewEvalProblem), _i, C.POINTER(TwoViewEvalParams),
                                         C.POINTER(TwoViewEvalResult), _vp]),
     "b2_viewgraph_cycle_filter_host": (_i, [_vp, _vp, _vp, _i, C.POINTER(ViewGraphParams), _vp, _vp, _vp, _vp]),
+    "b2_triangulate_tracks_host": (_i, [_vp, _vp, C.c_int64, _vp, _vp, _vp, _vp, _i, C.POINTER(TriangulationParams), _vp, _vp, _vp,
+                                        _vp, _vp]),
     "b2_debug_viewgraph_triplets_host": (_i, [_vp, _vp, _vp, _i, C.c_int64, _vp, _vp, C.POINTER(C.c_int64), _vp]),
     "b2_twoview_ba_batched_dev": (_i, [_vp, C.POINTER(TwoViewProblem), _i, C.POINTER(TwoViewParams), C.POINTER(TwoViewResult), _vp]),
     "b2_twoview_ba_workspace_bytes": (_sz, [C.POINTER(TwoViewProblem), C.POINTER(TwoViewParams)]),

@@ -37,6 +37,7 @@ extern "C" void b2_destroy(b2_context* ctx) {
   tv_destroy(ctx);
   te_destroy(ctx);
   vg_destroy(ctx);
+  da_destroy(ctx);
   rt_destroy(ctx);
   nv_destroy(ctx);
   mn_destroy(ctx);
@@ -74,6 +75,11 @@ extern "C" int b2_set_option(b2_context* ctx, const char* name, int64_t value) {
   if (!strcmp(name, "viewgraph_workspace_mb")) {  // segment window of one chunk of b2_viewgraph_cycle_filter_host
     if (value < 1 || value > (1 << 20)) return b2_fail(ctx, B2_ERR_ARG, "viewgraph_workspace_mb takes 1..1048576");
     ctx->vg_workspace_mb = (int)value;
+    return B2_OK;
+  }
+  if (!strcmp(name, "data_assoc_workspace_mb")) {  // device workspace of one chunk of b2_triangulate_tracks_host
+    if (value < 1 || value > (1 << 20)) return b2_fail(ctx, B2_ERR_ARG, "data_assoc_workspace_mb takes 1..1048576");
+    ctx->da_workspace_mb = (int)value;
     return B2_OK;
   }
   if (!strcmp(name, "force_simt")) {  // takes effect for models whose weights are set AFTER this call

@@ -107,6 +107,7 @@ struct OrbState;
 struct TwoViewState;
 struct TwoViewEvalState;
 struct ViewGraphState;
+struct DataAssocState;
 
 // Device copies of host feature arrays handed to the *_host matcher entry points.  GTSfM matches one image's (keypoints,
 // descriptors) against ~20-40 partners, always passing the same host arrays, so re-uploading 5 MB per image per pair is
@@ -129,6 +130,7 @@ struct b2_context {
   int lg_batch = 0;     // pairs per LightGlue batch (0 = the library maximum, 8); b2_set_option "lightglue_batch"
   int rs_workspace_mb = 1024;  // RANSAC workspace budget per sub-batch of a batched call; b2_set_option "ransac_workspace_mb"
   int vg_workspace_mb = 1024;  // view-graph filter: segment window of one chunk; b2_set_option "viewgraph_workspace_mb"
+  int da_workspace_mb = 256;   // data association: device workspace of one chunk of tracks; "data_assoc_workspace_mb"
   int force_simt = -1;  // 1: models loaded afterwards run the exact-fp32 SIMT kernels (no tensor cores); -1 = B2_FORCE_SIMT env
   int lg_trace = 0;     // 1: b2_lightglue_match_* record each side's state after every layer (b2_lightglue_trace_get)
   int sg_trace = 0;     // 1: b2_superglue_match_* record each side's state after every layer (b2_superglue_trace_get)
@@ -155,6 +157,7 @@ struct b2_context {
   TwoViewState* tv = nullptr;
   TwoViewEvalState* te = nullptr;
   ViewGraphState* vg = nullptr;
+  DataAssocState* da = nullptr;
   // staging shared by the *_host entry points
   DevBuf stage_d[8];
   HostBuf stage_h[4];
@@ -250,6 +253,7 @@ void ob_destroy(b2_context* ctx);
 void tv_destroy(b2_context* ctx);
 void te_destroy(b2_context* ctx);
 void vg_destroy(b2_context* ctx);
+void da_destroy(b2_context* ctx);
 
 // shared device helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

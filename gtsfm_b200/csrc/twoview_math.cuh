@@ -230,15 +230,23 @@ TV_HD void projection_matrix(const double* R, const double* t, const double* cal
   }
 }
 
-// triangulateDLT on two views -> false when the rank (singular values above 1e-9) is below 3 or the point is at infinity
-TV_HD bool dlt(const double* P0, const double* P1, const double* uv0, const double* uv1, double* X) {
-  double A[16], s[4], V[16];
+// A camera of the two-view problem: Pose3(R, t) (world from camera) and {f, k1, k2, u0, v0}
+struct Cam {
+  double R[9], t[3], cal[5];
+};
+
+// The two rows of the DLT system one view contributes: u P[2] - P[0], v P[2] - P[1]
+TV_HD void dlt_rows(const double* P, const double* uv, double* a) {
   for (int j = 0; j < 4; ++j) {
-    A[j] = uv0[0] * P0[8 + j] - P0[j];
-    A[4 + j] = uv0[1] * P0[8 + j] - P0[4 + j];
-    A[8 + j] = uv1[0] * P1[8 + j] - P1[j];
-    A[12 + j] = uv1[1] * P1[8 + j] - P1[4 + j];
+    a[j] = uv[0] * P[8 + j] - P[j];
+    a[4 + j] = uv[1] * P[8 + j] - P[4 + j];
   }
+}
+
+// The null vector of a 4-column system reduced to 4 x 4 (A, destroyed) -> false when the rank (singular values above
+// 1e-9) is below 3 or the point is at infinity
+TV_HD bool dlt_solve(double* A, double* X) {
+  double s[4], V[16];
   svd4(A, s, V);
   int rank = 0, jmin = 0;
   for (int j = 0; j < 4; ++j) {
@@ -251,24 +259,72 @@ TV_HD bool dlt(const double* P0, const double* P1, const double* uv0, const doub
   return isfinite(X[0]) && isfinite(X[1]) && isfinite(X[2]);
 }
 
-// A camera of the two-view problem: Pose3(R, t) (world from camera) and {f, k1, k2, u0, v0}
-struct Cam {
-  double R[9], t[3], cal[5];
-};
+// triangulateDLT on two views
+TV_HD bool dlt(const double* P0, const double* P1, const double* uv0, const double* uv1, double* X) {
+  double A[16];
+  dlt_rows(P0, uv0, A);
+  dlt_rows(P1, uv1, A + 8);
+  return dlt_solve(A, X);
+}
 
-// TriangulationFactor residuals of a point in both cameras (a point behind a camera: residual (2f, 2f), zero Jacobian)
-TV_HD void tri_resid(const Cam* cams, const double* uv, const double* X, double* r, double* J) {
-  for (int c = 0; c < 2; ++c) {
-    double pr[2];
-    const double z = project(cams[c].R, cams[c].t, cams[c].cal, X, pr, nullptr, J ? J + 6 * c : nullptr);
-    if (!(z > 0.0)) {
-      r[2 * c] = r[2 * c + 1] = 2.0 * cams[c].cal[0];
-      if (J)
-        for (int i = 0; i < 6; ++i) J[6 * c + i] = 0.0;
-    } else {
-      r[2 * c] = pr[0] - uv[2 * c], r[2 * c + 1] = pr[1] - uv[2 * c + 1];
+// Folds one row a[4] (destroyed) into the upper-triangular R (row-major 4 x 4) by Givens rotations, so that R^T R gains
+// a a^T: R then has the singular values and right singular vectors of every row folded in so far.
+TV_HD void qr_fold_row(double* R, double* a) {
+  for (int j = 0; j < 4; ++j) {
+    if (a[j] == 0.0) continue;
+    const double r = hypot(R[j * 4 + j], a[j]), c = R[j * 4 + j] / r, s = a[j] / r;
+    R[j * 4 + j] = r;
+    a[j] = 0.0;
+    for (int k = j + 1; k < 4; ++k) {
+      const double x = R[j * 4 + k], y = a[k];
+      R[j * 4 + k] = c * x + s * y, a[k] = c * y - s * x;
     }
   }
+}
+
+// triangulateDLT on n >= 2 views given by `views` (see refine_point_views).  Two views go through dlt's 4 x 4 system as
+// it is; more are reduced to 4 x 4 by a streamed QR of the 2n x 4 system first (same singular values, same null vector).
+template <class Views>
+TV_HD bool dlt_views(const Views& views, double* X) {
+  const int n = views.size();
+  double A[16], P[12];
+  if (n == 2) {
+    for (int k = 0; k < 2; ++k) {
+      const Cam& c = views.cam(k);
+      projection_matrix(c.R, c.t, c.cal, P);
+      dlt_rows(P, views.uv(k), A + 8 * k);
+    }
+    return dlt_solve(A, X);
+  }
+  for (int i = 0; i < 16; ++i) A[i] = 0.0;
+  for (int k = 0; k < n; ++k) {
+    const Cam& c = views.cam(k);
+    double a[8];
+    projection_matrix(c.R, c.t, c.cal, P);
+    dlt_rows(P, views.uv(k), a);
+    qr_fold_row(A, a);
+    qr_fold_row(A, a + 4);
+  }
+  return dlt_solve(A, X);
+}
+
+// TriangulationFactor residual of a point in one camera, Jacobian J [2][3] (may be NULL); a point behind the camera:
+// residual (2f, 2f), zero Jacobian
+TV_HD void tri_resid1(const Cam& c, const double* uv, const double* X, double* r, double* J) {
+  double pr[2];
+  const double z = project(c.R, c.t, c.cal, X, pr, nullptr, J);
+  if (!(z > 0.0)) {
+    r[0] = r[1] = 2.0 * c.cal[0];
+    if (J)
+      for (int i = 0; i < 6; ++i) J[i] = 0.0;
+  } else {
+    r[0] = pr[0] - uv[0], r[1] = pr[1] - uv[1];
+  }
+}
+
+// TriangulationFactor residuals of a point in both cameras
+TV_HD void tri_resid(const Cam* cams, const double* uv, const double* X, double* r, double* J) {
+  for (int c = 0; c < 2; ++c) tri_resid1(cams[c], uv + 2 * c, X, r + 2 * c, J ? J + 6 * c : nullptr);
 }
 TV_HD double tri_cost(const Cam* cams, const double* uv, const double* X) {
   double r[4];
@@ -276,38 +332,60 @@ TV_HD double tri_cost(const Cam* cams, const double* uv, const double* X) {
   return 0.5 * (r[0] * r[0] + r[1] * r[1] + r[2] * r[2] + r[3] * r[3]);
 }
 
-// triangulateNonlinear: gtsam's LM (lambda0 1, absolute tolerance 1, 100 iterations) on the point alone
-TV_HD void refine_point(const Cam* cams, const double* uv, double* X) {
-  double err = tri_cost(cams, uv, X);
+// The two views of the two-view problem, as refine_point_views and dlt_views take views: size(), cam(k), uv(k) and
+// cost(X), the triangulation cost 0.5 sum |r|^2
+struct TwoViews {
+  const Cam* cams;
+  const double* uvs;  // {u0, v0, u1, v1}
+  TV_HD int size() const { return 2; }
+  TV_HD const Cam& cam(int k) const { return cams[k]; }
+  TV_HD const double* uv(int k) const { return uvs + 2 * k; }
+  TV_HD double cost(const double* X) const { return tri_cost(cams, uvs, X); }
+};
+
+// triangulateNonlinear: gtsam's LM (lambda0 1, absolute tolerance 1, 100 iterations) on the point alone, over any number
+// of views.  The normal equations and the linearised decrease are accumulated view by view, row by row, in view order
+// (nothing is stored per view), so two views sum in the order of the 4-row two-view system.
+template <class Views>
+TV_HD void refine_point_views(const Views& views, double* X) {
+  const int n = views.size();
+  double err = views.cost(X);
   if (err <= 0.0) return;
   double lam = TRI_LAMBDA0, nw = err;
   int its = 0;
   for (;;) {
     const double cur = nw;
-    double r[4], J[12];
-    tri_resid(cams, uv, X, r, J);
     for (;;) {
       double H[9] = {0}, g[3] = {0};
-      for (int i = 0; i < 3; ++i) {
-        for (int j = 0; j < 3; ++j)
-          for (int m = 0; m < 4; ++m) H[i * 3 + j] += J[m * 3 + i] * J[m * 3 + j];
-        for (int m = 0; m < 4; ++m) g[i] += J[m * 3 + i] * r[m];
-        H[i * 4] += lam;
+      for (int k = 0; k < n; ++k) {
+        double r[2], J[6];
+        tri_resid1(views.cam(k), views.uv(k), X, r, J);
+        for (int m = 0; m < 2; ++m) {
+          for (int i = 0; i < 3; ++i) {
+            for (int j = 0; j < 3; ++j) H[i * 3 + j] += J[m * 3 + i] * J[m * 3 + j];
+            g[i] += J[m * 3 + i] * r[m];
+          }
+        }
       }
+      for (int i = 0; i < 3; ++i) H[i * 4] += lam;
       bool success = false, stop = false;
       double Xn[3];
       if (chol(H, 3, 3)) {
         double d[3] = {-g[0], -g[1], -g[2]};
         chol_solve(H, 3, 3, d);
         double lin = 0.0, old = 0.0;
-        for (int m = 0; m < 4; ++m) {
-          const double jd = J[m * 3] * d[0] + J[m * 3 + 1] * d[1] + J[m * 3 + 2] * d[2];
-          lin -= r[m] * jd + 0.5 * jd * jd;
-          old += 0.5 * r[m] * r[m];
+        for (int k = 0; k < n; ++k) {
+          double r[2], J[6];
+          tri_resid1(views.cam(k), views.uv(k), X, r, J);
+          for (int m = 0; m < 2; ++m) {
+            const double jd = J[m * 3] * d[0] + J[m * 3 + 1] * d[1] + J[m * 3 + 2] * d[2];
+            lin -= r[m] * jd + 0.5 * jd * jd;
+            old += 0.5 * r[m] * r[m];
+          }
         }
         if (lin >= 0.0) {
           for (int i = 0; i < 3; ++i) Xn[i] = X[i] + d[i];
-          const double dc = cur - tri_cost(cams, uv, Xn);
+          const double dc = cur - views.cost(Xn);
           success = lin > DBL_EPSILON * old ? dc / lin > LM_MIN_FIDELITY : true;
           stop = fabs(dc) < LM_REL_TOL * cur;
         }
@@ -321,12 +399,14 @@ TV_HD void refine_point(const Cam* cams, const double* uv, double* X) {
       lam *= LM_FACTOR;
       if (lam >= LM_LAMBDA_MAX) break;
     }
-    nw = tri_cost(cams, uv, X);
+    nw = views.cost(X);
     const double dec = cur - nw;
     const bool conv = dec / cur <= LM_REL_TOL || dec <= TRI_ABS_TOL || nw <= 0.0;
     if (!(its < TRI_MAX_ITERS && !conv && isfinite(cur))) return;
   }
 }
+
+TV_HD void refine_point(const Cam* cams, const double* uv, double* X) { refine_point_views(TwoViews{cams, uv}, X); }
 
 // Point3dInitializer.triangulate (NO_RANSAC) for one correspondence uv = {u0, v0, u1, v1} -> false when dropped
 TV_HD bool triangulate(const Cam* cams, const double* uv, double reproj_thr, double min_angle_deg, double* X) {

@@ -262,3 +262,89 @@ except Exception:  # noqa: BLE001
         @abc.abstractmethod
         def run(self, i2Ri1_dict, i2Ui1_dict, calibrations, corr_idxs_i1i2, keypoints, two_view_reports, output_dir=None):
             ...
+
+
+try:  # pragma: no cover - exercised only inside a full GTSfM environment
+    from gtsam import SfmTrack
+    from gtsfm.common.sfm_track import SfmMeasurement, SfmTrack2d
+    from gtsfm.data_association.data_assoc import DataAssociation
+    from gtsfm.data_association.point3d_initializer import TriangulationExitCode, TriangulationOptions, TriangulationSamplingMode
+    HAVE_GTSFM_DATA_ASSOCIATION = True  # the reference's DataAssociation is the base: its run_triangulation is the fallback
+except Exception:  # noqa: BLE001
+    HAVE_GTSFM_DATA_ASSOCIATION = False
+    import sys
+    from dataclasses import dataclass
+    from enum import Enum
+    from typing import List, NamedTuple
+
+    class TriangulationExitCode(Enum):  # mirrors point3d_initializer.py:34-43
+        SUCCESS = 0
+        CHEIRALITY_FAILURE = 1
+        INLIERS_UNDERCONSTRAINED = 2
+        POSES_UNDERCONSTRAINED = 3
+        EXCEEDS_REPROJ_THRESH = 4
+        LOW_TRIANGULATION_ANGLE = 5
+
+    class TriangulationSamplingMode(str, Enum):  # mirrors point3d_initializer.py:46-58
+        NO_RANSAC = "NO_RANSAC"
+        RANSAC_SAMPLE_UNIFORM = "RANSAC_SAMPLE_UNIFORM"
+        RANSAC_SAMPLE_BIASED_BASELINE = "RANSAC_SAMPLE_BIASED_BASELINE"
+        RANSAC_TOPK_BASELINES = "RANSAC_TOPK_BASELINES"
+
+    class TriangulationOptions(NamedTuple):  # mirrors point3d_initializer.py:61-112
+        mode: TriangulationSamplingMode
+        reproj_error_threshold: float = np.inf
+        min_triangulation_angle: float = 0.0
+        min_inlier_ratio: float = 0.1
+        confidence: float = 0.9999
+        dyn_num_hypotheses_multiplier: float = 3.0
+        min_num_hypotheses: int = 0
+        max_num_hypotheses: int = sys.maxsize
+
+        def num_ransac_hypotheses(self) -> int:
+            assert self.reproj_error_threshold > 0
+            assert 0 < self.min_inlier_ratio < 1
+            assert 0 < self.confidence < 1
+            assert self.dyn_num_hypotheses_multiplier > 0
+            assert 0 <= self.min_num_hypotheses < self.max_num_hypotheses
+            dyn = int((np.log(1 - self.confidence) / np.log(1 - self.min_inlier_ratio ** 2)) * self.dyn_num_hypotheses_multiplier)
+            return max(min(self.max_num_hypotheses, dyn), self.min_num_hypotheses)
+
+    class SfmMeasurement(NamedTuple):  # mirrors gtsfm/common/sfm_track.py:18-35
+        i: int
+        uv: np.ndarray
+
+    class SfmTrack2d(NamedTuple):  # mirrors gtsfm/common/sfm_track.py:38-78 (what triangulation reads)
+        measurements: List[SfmMeasurement]
+
+        def number_measurements(self) -> int:
+            return len(self.measurements)
+
+        def measurement(self, idx: int) -> SfmMeasurement:
+            return self.measurements[idx]
+
+    class SfmTrack:  # the part of gtsam.SfmTrack a triangulated track exposes
+        def __init__(self, pt):
+            self._pt = np.asarray(pt, np.float64).reshape(3)
+            self._meas: list = []
+
+        def addMeasurement(self, i, uv) -> None:  # noqa: N802 - gtsam's name
+            self._meas.append((int(i), np.asarray(uv, np.float64).reshape(2)))
+
+        def numberMeasurements(self) -> int:  # noqa: N802
+            return len(self._meas)
+
+        def measurement(self, k):
+            return self._meas[k]
+
+        def point3(self) -> np.ndarray:
+            return self._pt
+
+    @dataclass(frozen=True)
+    class DataAssociation:  # the fields of data_assoc.py:45-58 and the method a subclass overrides
+        min_track_len: int
+        triangulation_options: TriangulationOptions
+        save_track_patches_viz: Optional[bool] = False
+
+        def run_triangulation(self, cameras, tracks_2d):
+            raise NotImplementedError("the reference's run_triangulation needs GTSfM")

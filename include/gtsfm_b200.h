@@ -56,6 +56,8 @@ uint64_t b2_h2d_bytes(const b2_context* ctx);
  * more problems than fit is cut into consecutive sub-batches, which changes no result.
  * "viewgraph_workspace_mb" = 1..: the segment window of one chunk of b2_viewgraph_cycle_filter_host's MEDIAN (default 1024);
  * a graph with more segment entries than fit is processed in several chunks, which changes no result.
+ * "data_assoc_workspace_mb" = 1..: device workspace one chunk of b2_triangulate_tracks_host may use (default 256); a call
+ * with more tracks than fit is cut into consecutive chunks of whole tracks, which changes no result.
  * "feature_cache" = 0 | 1: drop every cached device copy of host feature arrays and (0, default) copy on every call like the
  * reference / (1) keep device copies keyed by (host pointer, size) and validated by a hash of the FULL contents, so arrays
  * edited in place are re-sent.  Only pays off for callers that pass the same numpy buffers repeatedly (it does nothing for
@@ -581,6 +583,37 @@ int b2_viewgraph_cycle_filter_host(b2_context* ctx, const int32_t* edges, const 
  * particular order; *out_count = the number of triplets (entries past `capacity` are not written). */
 int b2_debug_viewgraph_triplets_host(b2_context* ctx, const int32_t* edges, const double* R, int n, int64_t capacity,
                                      int32_t* out_nodes, double* out_error, int64_t* out_count, void* stream);
+
+/* ---- Data association: triangulation of 2-D tracks (gtsfm/data_association/data_assoc.py:205-273,
+ * point3d_initializer.py:139-295) -----------------------------------------------------------------------------------------
+ * Track t is measurements [track_off[t], track_off[t+1]) of meas_cam (image index, 0 <= i < num_images) and meas_uv
+ * (pixels).  Camera i is cams[i] = R_wTi (9, row-major), t_wTi (3), f, u0, v0 (Cal3Bundler without distortion), used only
+ * where cam_valid[i] != 0.  RANSAC_SAMPLE_UNIFORM: min(num_hypotheses, C(n, 2)) two-view hypotheses per track of n
+ * measurements (every pair when C(n, 2) <= num_hypotheses, else a keyed permutation of the pairs, seed and track position:
+ * csrc/data_assoc_math.cuh), each triangulated with triangulatePoint3(rank_tol 1e-9, optimize) and scored by its inliers
+ * (projectSafe error < reproj_error_threshold); most inliers wins, then the lower average inlier error, then the earlier
+ * hypothesis.  NO_RANSAC: every measurement is an inlier.  Then, in this order: < 2 inliers -> INLIERS_UNDERCONSTRAINED,
+ * < 2 inliers with a camera -> POSES_UNDERCONSTRAINED, n-view triangulatePoint3 of those failing -> CHEIRALITY_FAILURE, an
+ * inlier's error (NaN without a camera) not below the threshold -> EXCEEDS_REPROJ_THRESH, every pairwise triangulation
+ * angle below min_triangulation_angle -> LOW_TRIANGULATION_ANGLE, else SUCCESS.  fp64; oracle/data_assoc_ref.py is the
+ * NumPy statement.  Tracks are processed in chunks under "data_assoc_workspace_mb" (b2_set_option); a chunked run returns
+ * what one chunk returns, bit for bit. */
+#define B2_TRI_NO_RANSAC 0      /* TriangulationSamplingMode.NO_RANSAC */
+#define B2_TRI_SAMPLE_UNIFORM 1 /* TriangulationSamplingMode.RANSAC_SAMPLE_UNIFORM */
+typedef struct b2_triangulation_params {
+  int mode;                       /* B2_TRI_NO_RANSAC or B2_TRI_SAMPLE_UNIFORM */
+  int num_hypotheses;             /* TriangulationOptions.num_ransac_hypotheses() (>= 1; unused by NO_RANSAC) */
+  double reproj_error_threshold;  /* px, > 0, may be inf */
+  double min_triangulation_angle; /* degrees */
+  uint64_t seed;                  /* keys the permutation of tracks with more pairs than hypotheses */
+} b2_triangulation_params;
+/* HOST inputs and outputs.  Per track: exit_code [T] (TriangulationExitCode), point [T][3] (NaN unless the n-view
+ * triangulation ran: exit codes 0, 4, 5), avg_err [T] (nanmean of the inliers' errors; NaN for exit codes 1-3, the
+ * reference's None); per measurement: inlier [M] (the RANSAC inlier set, or all for NO_RANSAC).  Bad arguments return
+ * B2_ERR_ARG before any launch.  One synchronisation per chunk. */
+int b2_triangulate_tracks_host(b2_context* ctx, const int64_t* track_off, int64_t T, const int32_t* meas_cam, const double* meas_uv,
+                               const double* cams, const uint8_t* cam_valid, int num_images, const b2_triangulation_params* params,
+                               int8_t* exit_code, double* point, double* avg_err, uint8_t* inlier, void* stream);
 
 /* ---- LMedS verifier (gtsfm/frontend/verifier/lmeds.py: cv2.findEssentialMat / findFundamentalMat with LMEDS) ----------
  * A batched device restatement of cv2's LMeDS estimator: cv::RNG subsets (seed 2^64 - 1, F subsets with collinear points
