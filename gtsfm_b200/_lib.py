@@ -251,6 +251,7 @@ SIGNATURES = {
     "b2_viewgraph_cycle_filter_host": (_i, [_vp, _vp, _vp, _i, C.POINTER(ViewGraphParams), _vp, _vp, _vp, _vp]),
     "b2_triangulate_tracks_host": (_i, [_vp, _vp, C.c_int64, _vp, _vp, _vp, _vp, _i, C.POINTER(TriangulationParams), _vp, _vp, _vp,
                                         _vp, _vp]),
+    "b2_mfas_outlier_weights_host": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "b2_debug_viewgraph_triplets_host": (_i, [_vp, _vp, _vp, _i, C.c_int64, _vp, _vp, C.POINTER(C.c_int64), _vp]),
     "b2_twoview_ba_batched_dev": (_i, [_vp, C.POINTER(TwoViewProblem), _i, C.POINTER(TwoViewParams), C.POINTER(TwoViewResult), _vp]),
     "b2_twoview_ba_workspace_bytes": (_sz, [C.POINTER(TwoViewProblem), C.POINTER(TwoViewParams)]),

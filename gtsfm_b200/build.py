@@ -25,8 +25,9 @@ NVCC_FLAGS = [
 ]
 # per-source additions: the LMedS verifier replays cv2's double arithmetic, so its products and sums are not contracted
 # into FMAs (its solvers then round as the host build in tests/cpp/lmeds_shim.cpp does); the ORB detector likewise replays
-# cv2's float arithmetic (Harris, angles, pattern rotation, resize coordinates) and writes its one FMA chain out explicitly
-NVCC_FLAGS_FOR = {"lmeds.cu": ["-fmad=false"], "orb.cu": ["-fmad=false"]}
+# cv2's float arithmetic (Harris, angles, pattern rotation, resize coordinates) and writes its one FMA chain out explicitly;
+# 1DSfM's MFAS forms each edge weight m . d as gtsam's Eigen dot does, without FMAs, so the orderings are gtsam's
+NVCC_FLAGS_FOR = {"lmeds.cu": ["-fmad=false"], "orb.cu": ["-fmad=false"], "mfas.cu": ["-fmad=false"]}
 
 
 def nvcc() -> str:

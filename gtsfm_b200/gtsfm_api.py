@@ -348,3 +348,47 @@ except Exception:  # noqa: BLE001
 
         def run_triangulation(self, cameras, tracks_2d):
             raise NotImplementedError("the reference's run_triangulation needs GTSfM")
+
+
+try:  # pragma: no cover - exercised only inside a full GTSfM environment
+    from gtsfm.averaging.translation.averaging_1dsfm import TranslationAveraging1DSFM
+    HAVE_GTSFM_1DSFM = True  # the reference's class is the base: its sampler and run_translation_averaging are used
+except Exception:  # noqa: BLE001
+    HAVE_GTSFM_1DSFM = False
+    from enum import Enum
+
+    class TranslationAveraging1DSFM:  # mirrors averaging_1dsfm.py:79-155 (constructor, sampler; no averaging)
+        class ProjectionSamplingMethod(str, Enum):
+            SAMPLE_INPUT_MEASUREMENTS = "SAMPLE_INPUT_MEASUREMENTS"
+            SAMPLE_WITH_INPUT_DENSITY = "SAMPLE_WITH_INPUT_DENSITY"
+            SAMPLE_WITH_UNIFORM_DENSITY = "SAMPLE_WITH_UNIFORM_DENSITY"
+
+        def __init__(self, robust_measurement_noise: bool = True, use_tracks_for_averaging: bool = True,
+                     reject_outliers: bool = True, projection_sampling_method=ProjectionSamplingMethod.SAMPLE_WITH_UNIFORM_DENSITY,
+                     max_delayed_calls: int = 16, use_all_tracks_for_averaging: bool = False,
+                     use_relative_camera_poses: bool = True) -> None:
+            self._robust_measurement_noise = robust_measurement_noise
+            self._max_1dsfm_projection_directions = 2000
+            self._outlier_weight_threshold = 0.125
+            self._reject_outliers = reject_outliers
+            self._projection_sampling_method = projection_sampling_method
+            self._use_tracks_for_averaging = use_tracks_for_averaging
+            self._max_delayed_calls = max_delayed_calls
+            self._use_relative_camera_poses = use_relative_camera_poses
+            self._use_all_tracks_for_averaging = use_all_tracks_for_averaging
+            np.random.seed(0)
+
+        def __sample_projection_directions(self, w_i2Ui1_list):
+            """The reference's sampler on NumPy's global RNG, as (K, 3) rows normalised as gtsam's Unit3 (Eigen) does."""
+            method = self.ProjectionSamplingMethod(self._projection_sampling_method)
+            num = self._max_1dsfm_projection_directions
+            if method == self.ProjectionSamplingMethod.SAMPLE_INPUT_MEASUREMENTS:
+                n = len(w_i2Ui1_list)
+                return [w_i2Ui1_list[i] for i in np.random.choice(n, min(n, num), replace=False)]
+            if method == self.ProjectionSamplingMethod.SAMPLE_WITH_UNIFORM_DENSITY:
+                v = np.random.normal(size=(num, 3))
+                return v / np.sqrt((v[:, 0] * v[:, 0] + v[:, 1] * v[:, 1]) + v[:, 2] * v[:, 2])[:, None]
+            raise ValueError("SAMPLE_WITH_INPUT_DENSITY samples a scipy KDE through GTSfM, which is not installed")
+
+        def run_translation_averaging(self, *args, **kwargs):
+            raise NotImplementedError("run_translation_averaging (track selection, TranslationRecovery) needs GTSfM")

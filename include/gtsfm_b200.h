@@ -58,6 +58,8 @@ uint64_t b2_h2d_bytes(const b2_context* ctx);
  * a graph with more segment entries than fit is processed in several chunks, which changes no result.
  * "data_assoc_workspace_mb" = 1..: device workspace one chunk of b2_triangulate_tracks_host may use (default 256); a call
  * with more tracks than fit is cut into consecutive chunks of whole tracks, which changes no result.
+ * "mfas_workspace_mb" = 1..: device workspace one chunk of directions of b2_mfas_outlier_weights_host may use (default 1024);
+ * a call with more directions than fit is cut into consecutive chunks, which changes no result.
  * "feature_cache" = 0 | 1: drop every cached device copy of host feature arrays and (0, default) copy on every call like the
  * reference / (1) keep device copies keyed by (host pointer, size) and validated by a hash of the FULL contents, so arrays
  * edited in place are re-sent.  Only pays off for callers that pass the same numpy buffers repeatedly (it does nothing for
@@ -614,6 +616,23 @@ typedef struct b2_triangulation_params {
 int b2_triangulate_tracks_host(b2_context* ctx, const int64_t* track_off, int64_t T, const int32_t* meas_cam, const double* meas_uv,
                                const double* cams, const uint8_t* cam_valid, int num_images, const b2_triangulation_params* params,
                                int8_t* exit_code, double* point, double* avg_err, uint8_t* inlier, void* stream);
+
+/* ---- 1DSfM outlier rejection: MFAS over projection directions (gtsfm/averaging/translation/averaging_1dsfm.py:216-296,
+ * gtsam MFAS::computeOutlierWeights) -----------------------------------------------------------------------------------------
+ * Nodes are dense ids 0..V-1 in gtsam key order; edge e = (edge_a[e], edge_b[e]) with unit measurement meas[e] (3 doubles),
+ * edges strictly increasing in (a, b) (std::map<KeyPair> order), no node pair twice in either orientation, no self edge.
+ * For each direction d_k (dirs[k], 3 doubles): w_e = (mx*dx + my*dy) + mz*dz, the edge points a -> b when w_e >= 0, and the
+ * greedy removes, at every step, the live node with in-weight < 1e-8 of lowest id, else the one with the largest
+ * (out + 1) / (in + 1) (ties: lowest id), subtracting its edges from its live neighbours.  Edge s -> t is violated when t is
+ * removed before s.  weight_sum[e] = the sum over k = 0..K-1 in order of |w_e(d_k)| where e is violated (the reference's
+ * Python-float accumulation of the outlier weights).  fp64; oracle/mfas_ref.py is the NumPy statement.  Directions are
+ * processed in chunks under "mfas_workspace_mb" (b2_set_option); a chunked run returns what one chunk returns, bit for bit.
+ * HOST inputs and outputs: weight_sum [E]; order_out [K][V] (the node removed at each step) and violated_out
+ * [K][ceil(E/32)] (bit e % 32 of word e / 32) are optional test hooks (NULL: not written).  Bad arguments (ids outside
+ * [0, V), a self edge, edges out of order, a repeated node pair, non-finite values) return B2_ERR_ARG before any launch. */
+int b2_mfas_outlier_weights_host(b2_context* ctx, int V, int E, const int32_t* edge_a, const int32_t* edge_b, const double* meas,
+                                 int K, const double* dirs, double* weight_sum, int32_t* order_out, uint32_t* violated_out,
+                                 void* stream);
 
 /* ---- LMedS verifier (gtsfm/frontend/verifier/lmeds.py: cv2.findEssentialMat / findFundamentalMat with LMEDS) ----------
  * A batched device restatement of cv2's LMeDS estimator: cv::RNG subsets (seed 2^64 - 1, F subsets with collinear points
