@@ -173,6 +173,19 @@ class TriangulationParams(C.Structure):  # b2_triangulation_params
 
 TRI_NO_RANSAC, TRI_SAMPLE_UNIFORM = 0, 1  # B2_TRI_NO_RANSAC, B2_TRI_SAMPLE_UNIFORM
 
+
+class BaParams(C.Structure):  # b2_ba_params
+    _fields_ = [("noise_sigma", C.c_double), ("huber_k", C.c_double), ("gauge", C.c_int), ("max_iters", C.c_int),
+                ("karcher_beta", C.c_double), ("pose_prior_sigma", C.c_double), ("cal_prior_sigma", C.c_double * 3)]
+
+
+class BaResult(C.Structure):  # b2_ba_result
+    _fields_ = [("iterations", C.c_int), ("trace_len", C.c_int), ("trials", C.c_int), ("pad_", C.c_int),
+                ("final_error", C.c_double)]
+
+
+BA_KARCHER, BA_FIRST_POSE_PRIOR = 0, 1  # B2_BA_KARCHER, B2_BA_FIRST_POSE_PRIOR
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 
@@ -251,6 +264,9 @@ SIGNATURES = {
     "b2_viewgraph_cycle_filter_host": (_i, [_vp, _vp, _vp, _i, C.POINTER(ViewGraphParams), _vp, _vp, _vp, _vp]),
     "b2_triangulate_tracks_host": (_i, [_vp, _vp, C.c_int64, _vp, _vp, _vp, _vp, _i, C.POINTER(TriangulationParams), _vp, _vp, _vp,
                                         _vp, _vp]),
+    "b2_bundle_adjust_workspace_bytes": (_sz, [_i, C.c_int64, _vp]),
+    "b2_bundle_adjust_host": (_i, [_vp, _i, _vp, C.c_int64, _vp, _vp, _vp, _vp, C.POINTER(BaParams), _vp, _vp, _vp, C.POINTER(BaResult),
+                                   _vp, _vp, _i, _vp]),
     "b2_mfas_outlier_weights_host": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "b2_debug_viewgraph_triplets_host": (_i, [_vp, _vp, _vp, _i, C.c_int64, _vp, _vp, C.POINTER(C.c_int64), _vp]),
     "b2_twoview_ba_batched_dev": (_i, [_vp, C.POINTER(TwoViewProblem), _i, C.POINTER(TwoViewParams), C.POINTER(TwoViewResult), _vp]),

@@ -39,6 +39,7 @@ extern "C" void b2_destroy(b2_context* ctx) {
   vg_destroy(ctx);
   da_destroy(ctx);
   mf_destroy(ctx);
+  gb_destroy(ctx);
   rt_destroy(ctx);
   nv_destroy(ctx);
   mn_destroy(ctx);
@@ -86,6 +87,11 @@ extern "C" int b2_set_option(b2_context* ctx, const char* name, int64_t value) {
   if (!strcmp(name, "mfas_workspace_mb")) {  // device workspace of one chunk of directions of b2_mfas_outlier_weights_host
     if (value < 1 || value > (1 << 20)) return b2_fail(ctx, B2_ERR_ARG, "mfas_workspace_mb takes 1..1048576");
     ctx->mf_workspace_mb = (int)value;
+    return B2_OK;
+  }
+  if (!strcmp(name, "ba_workspace_mb")) {  // bound on the device workspace of one b2_bundle_adjust_host call
+    if (value < 1 || value > (1 << 20)) return b2_fail(ctx, B2_ERR_ARG, "ba_workspace_mb takes 1..1048576");
+    ctx->ba_workspace_mb = (int)value;
     return B2_OK;
   }
   if (!strcmp(name, "force_simt")) {  // takes effect for models whose weights are set AFTER this call

@@ -421,12 +421,8 @@ __global__ void __launch_bounds__(TV_THREADS) k_tv_ba(const TvProb* __restrict__
               }
             cn += prior_cost(sh, sh.cand);
           }
-          if (lin >= 0.0) {
-            e_new = cn;
-            const double dcst = cur - e_new;
-            success = lin > DBL_EPSILON * old ? dcst / lin > LM_MIN_FIDELITY : true;
-            stop = fabs(dcst) < LM_REL_TOL * cur;
-          }
+          e_new = cn;
+          lm_trial(lin, old, cur, e_new, success, stop);
         }
         __syncthreads();
         if (success) {
@@ -441,9 +437,7 @@ __global__ void __launch_bounds__(TV_THREADS) k_tv_ba(const TvProb* __restrict__
       }
       if (tid == 0) p.trace[ntrace] = nw;
       ++ntrace;
-      const double dec = cur - nw;
-      const bool conv = dec / cur <= LM_REL_TOL || dec <= LM_ABS_TOL || nw <= 0.0;
-      if (!(its < prm.max_iters && !conv && isfinite(cur))) break;
+      if (!lm_continue(its, prm.max_iters, cur, nw, LM_ABS_TOL)) break;
     }
   }
   if (tid == 0) {

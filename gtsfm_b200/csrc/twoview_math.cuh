@@ -6,7 +6,8 @@
 // PinholeCamera<Cal3Bundler>, the projection and Jacobians of GeneralSFMFactor2<Cal3Bundler>, Pose3's retraction (gtsam's
 // default build sets GTSAM_POSE3_EXPMAP, so retract is the full SE(3) exponential, compose(Expmap(xi)) with xi = [w, v]),
 // the Block Huber reweighting of noiseModel::Robust, and the Levenberg-Marquardt step policy of gtsam's
-// LevenbergMarquardtOptimizer (tryLambda with the fixed lambda factor).
+// LevenbergMarquardtOptimizer (tryLambda with the fixed lambda factor).  The global bundle adjustment (global_ba.cu) uses
+// the same projection, retraction, Huber and LM decision over N cameras.
 #pragma once
 #include <float.h>
 #include <math.h>
@@ -33,8 +34,29 @@ constexpr int TRI_MAX_ITERS = 100;
 // indeterminate system: a Cholesky pivot of the undamped Hessian at or below this fraction of the unknown's diagonal
 constexpr double INDETERMINATE_PIVOT = 1e-10;
 
-TV_HD double huber_weight(double e) { return e <= HUBER_K ? 1.0 : HUBER_K / e; }
-TV_HD double huber_loss(double e) { return e <= HUBER_K ? 0.5 * e * e : HUBER_K * (e - 0.5 * HUBER_K); }
+// noiseModel::mEstimator::Huber(k) on a whitened error norm e: the IRLS weight and the loss (0.5 e^2 inside the basin)
+TV_HD double huber_weight(double e, double k) { return e <= k ? 1.0 : k / e; }
+TV_HD double huber_loss(double e, double k) { return e <= k ? 0.5 * e * e : k * (e - 0.5 * k); }
+TV_HD double huber_weight(double e) { return huber_weight(e, HUBER_K); }
+TV_HD double huber_loss(double e) { return huber_loss(e, HUBER_K); }
+
+// One tryLambda decision of gtsam's LevenbergMarquardtOptimizer: `lin` the linearised cost decrease of the step, `old` the
+// undamped linearised cost at dx = 0, `cur` the cost before and `e_new` the cost after the step (read only when lin >= 0).
+// success: accept the step (lambda /= 10); otherwise stop: leave the lambda loop without a step, else lambda *= 10.
+TV_HD void lm_trial(double lin, double old, double cur, double e_new, bool& success, bool& stop) {
+  success = stop = false;
+  if (!(lin >= 0.0)) return;
+  const double dc = cur - e_new;
+  success = lin > DBL_EPSILON * old ? dc / lin > LM_MIN_FIDELITY : true;
+  stop = fabs(dc) < LM_REL_TOL * cur;
+}
+// After an outer iteration (cost cur before, nw after, its successful iterations so far): whether LM goes on
+// (checkConvergence with the relative and the given absolute tolerance, maxIterations, a finite error)
+TV_HD bool lm_continue(int its, int max_iters, double cur, double nw, double abs_tol) {
+  const double dec = cur - nw;
+  const bool conv = dec / cur <= LM_REL_TOL || dec <= abs_tol || nw <= 0.0;
+  return its < max_iters && !conv && isfinite(cur);
+}
 
 TV_HD void mat3_mul(const double* A, const double* B, double* C) {
   for (int i = 0; i < 3; ++i)
@@ -385,9 +407,7 @@ TV_HD void refine_point_views(const Views& views, double* X) {
         }
         if (lin >= 0.0) {
           for (int i = 0; i < 3; ++i) Xn[i] = X[i] + d[i];
-          const double dc = cur - views.cost(Xn);
-          success = lin > DBL_EPSILON * old ? dc / lin > LM_MIN_FIDELITY : true;
-          stop = fabs(dc) < LM_REL_TOL * cur;
+          lm_trial(lin, old, cur, views.cost(Xn), success, stop);
         }
       }
       if (success) {
@@ -400,9 +420,7 @@ TV_HD void refine_point_views(const Views& views, double* X) {
       if (lam >= LM_LAMBDA_MAX) break;
     }
     nw = views.cost(X);
-    const double dec = cur - nw;
-    const bool conv = dec / cur <= LM_REL_TOL || dec <= TRI_ABS_TOL || nw <= 0.0;
-    if (!(its < TRI_MAX_ITERS && !conv && isfinite(cur))) return;
+    if (!lm_continue(its, TRI_MAX_ITERS, cur, nw, TRI_ABS_TOL)) return;
   }
 }
 

@@ -392,3 +392,51 @@ except Exception:  # noqa: BLE001
 
         def run_translation_averaging(self, *args, **kwargs):
             raise NotImplementedError("run_translation_averaging (track selection, TranslationRecovery) needs GTSfM")
+
+
+try:  # pragma: no cover - exercised only inside a full GTSfM environment
+    from gtsfm.bundle.bundle_adjustment import BundleAdjustmentOptimizer, RobustBAMode
+    HAVE_GTSFM_BA = True  # the reference's class is the base: its stage loop, evaluate and fallback are used
+except Exception:  # noqa: BLE001
+    HAVE_GTSFM_BA = False
+    from enum import Enum
+
+    class RobustBAMode(Enum):  # mirrors bundle_adjustment.py:44-51
+        NONE = "NONE"
+        HUBER = "HUBER"
+        GMC = "GMC"
+        TLS = "TLS"
+
+    class BundleAdjustmentOptimizer:  # mirrors bundle_adjustment.py:64-143 (the constructor's fields; no graph, no metrics)
+        def __init__(self, reproj_error_thresholds=(None,), robust_ba_mode=RobustBAMode.NONE, shared_calib: bool = False,
+                     max_iterations: Optional[int] = None, cam_pose3_prior_noise_sigma: float = 0.1,
+                     calibration_prior_focal_sigma: float = 20.0, calibration_prior_dist_sigma: float = 0.1,
+                     measurement_noise_sigma: float = 2.0, allow_indeterminate_linear_system: bool = True,
+                     print_summary: bool = False, ordering_type: str = "METIS", save_iteration_visualization: bool = False,
+                     robust_noise_basin: float = 1.345, use_karcher_mean_factor: bool = True, use_pose_prior: bool = False,
+                     use_calibration_prior: bool = True, use_first_point_prior: bool = False, use_gnc: bool = False,
+                     gnc_loss=RobustBAMode.GMC, factor_weight_outlier_threshold: float = 0.0, min_track_length: int = 2) -> None:
+            self._reproj_error_thresholds = reproj_error_thresholds
+            self._robust_ba_mode = RobustBAMode[robust_ba_mode] if isinstance(robust_ba_mode, str) else robust_ba_mode
+            self._shared_calib = shared_calib
+            self._max_iterations = max_iterations
+            self._cam_pose3_prior_noise_sigma = cam_pose3_prior_noise_sigma
+            self._use_calibration_prior = use_calibration_prior
+            self._calibration_prior_focal_sigma = calibration_prior_focal_sigma
+            self._calibration_prior_dist_sigma = calibration_prior_dist_sigma
+            self._measurement_noise_sigma = measurement_noise_sigma
+            self._allow_indeterminate_linear_system = allow_indeterminate_linear_system
+            self._ordering_type = ordering_type
+            self._print_summary = print_summary
+            self._save_iteration_visualization = save_iteration_visualization
+            self._robust_noise_basin = robust_noise_basin
+            self._use_karcher_mean_factor = use_karcher_mean_factor
+            self._use_pose_prior = use_pose_prior
+            self._use_first_point_prior = use_first_point_prior
+            self._use_gnc = use_gnc
+            self._gnc_loss = RobustBAMode[gnc_loss] if isinstance(gnc_loss, str) else gnc_loss
+            self._factor_weight_outlier_threshold = factor_weight_outlier_threshold
+            self._min_track_length = min_track_length
+
+        def run_ba_stage_with_filtering(self, *args, **kwargs):
+            raise NotImplementedError("the reference's run_ba_stage_with_filtering needs GTSfM")

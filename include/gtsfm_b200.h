@@ -60,6 +60,8 @@ uint64_t b2_h2d_bytes(const b2_context* ctx);
  * with more tracks than fit is cut into consecutive chunks of whole tracks, which changes no result.
  * "mfas_workspace_mb" = 1..: device workspace one chunk of directions of b2_mfas_outlier_weights_host may use (default 1024);
  * a call with more directions than fit is cut into consecutive chunks, which changes no result.
+ * "ba_workspace_mb" = 1..: bound on the device workspace of one b2_bundle_adjust_host call (default 4096); a problem whose
+ * workspace (b2_bundle_adjust_workspace_bytes) is larger returns B2_ERR_ARG.
  * "feature_cache" = 0 | 1: drop every cached device copy of host feature arrays and (0, default) copy on every call like the
  * reference / (1) keep device copies keyed by (host pointer, size) and validated by a hash of the FULL contents, so arrays
  * edited in place are re-sent.  Only pays off for callers that pass the same numpy buffers repeatedly (it does nothing for
@@ -633,6 +635,51 @@ int b2_triangulate_tracks_host(b2_context* ctx, const int64_t* track_off, int64_
 int b2_mfas_outlier_weights_host(b2_context* ctx, int V, int E, const int32_t* edge_a, const int32_t* edge_b, const double* meas,
                                  int K, const double* dirs, double* weight_sum, int32_t* order_out, uint32_t* violated_out,
                                  void* stream);
+
+/* ---- Global bundle adjustment (gtsfm/bundle/bundle_adjustment.py: BundleAdjustmentOptimizer.run_ba_stage_with_filtering's
+ * optimisation) ------------------------------------------------------------------------------------------------------------
+ * gtsam's LevenbergMarquardtOptimizer with LevenbergMarquardtParams() defaults on the graph the reference builds with
+ * shared_calib False: one GeneralSFMFactor2<Cal3Bundler>(uv, Isotropic(2, noise_sigma) [Robust Huber(huber_k)], X(i), P(j),
+ * K(i)) per measurement, the gauge (KarcherMeanFactorPose3 over every pose with beta, or a PriorFactorPose3 on camera 0's
+ * input pose), and one PriorFactor<Cal3Bundler> per camera on its input (f, k1, k2).  fp64 throughout.
+ * Cameras are HOST [C][17]: R (9, row-major wRc), t (3, wtc), f, k1, k2, u0, v0; every camera is a variable (the caller
+ * passes the valid cameras in sorted order).  Points HOST [N][3]; measurements grouped by track: track_off [N + 1]
+ * (track j owns measurements track_off[j] .. track_off[j + 1] - 1), meas_cam [M] camera index, meas_uv [M][2].
+ * One LM trial: linearise (one thread per measurement), eliminate each point's damped 3 x 3 block, assemble the dense
+ * reduced camera system (9 unknowns per camera, the Karcher term), factor it by a blocked fp64 Cholesky, back-substitute the
+ * points, and evaluate the candidate's cost and the linearised decrease; the host reads those scalars once per trial and
+ * applies twoview_math.cuh's lm_trial / lm_continue.  A damped system whose Cholesky fails is a rejected trial.  Every sum
+ * has a fixed order and there are no floating-point atomics: repeated calls return identical bits.
+ * Outputs (HOST): cams_out [C][17], points_out [N][3], reproj_err [M] (|project - uv| at the result, NaN when the point is
+ * not in front of the camera), result (iterations, final_error = the graph's error at the result), and optionally trace
+ * [max_iters + 2] (the cost before the first and after every outer iteration; result->trace_len entries) and trial_out
+ * [trial_cap] (per trial: 1 accepted, 0 rejected, 2 rejected and the lambda search stopped, -1 the damped system was not
+ * positive definite; result->trials counts every trial, also those past trial_cap).
+ * B2_ERR_ARG before any launch: C < 1, N < 1, a camera or point index out of range, a track without a measurement or with
+ * two measurements in one camera, a non-finite input, f <= 0, bad params, or a workspace above "ba_workspace_mb". */
+enum { B2_BA_KARCHER = 0, B2_BA_FIRST_POSE_PRIOR = 1 };
+typedef struct b2_ba_params {
+  double noise_sigma;        /* measurement_noise_sigma (> 0) */
+  double huber_k;            /* robust_noise_basin of the Huber model; 0: no robust model (robust_ba_mode NONE) */
+  int gauge;                 /* B2_BA_KARCHER or B2_BA_FIRST_POSE_PRIOR */
+  int max_iters;             /* maxIterations: 0..100000 */
+  double karcher_beta;       /* KarcherMeanFactorPose3's beta (1000 in the reference) */
+  double pose_prior_sigma;   /* cam_pose3_prior_noise_sigma of the first-pose prior */
+  double cal_prior_sigma[3]; /* calibration prior sigmas of f, k1, k2 (calibration_prior_focal_sigma, _dist_sigma twice) */
+} b2_ba_params;
+typedef struct b2_ba_result {
+  int iterations; /* successful LM iterations */
+  int trace_len;  /* entries written to trace */
+  int trials;     /* tryLambda trials */
+  int pad_;
+  double final_error;
+} b2_ba_result;
+/* Device workspace of a call (what "ba_workspace_mb" bounds); 0 for invalid sizes. */
+size_t b2_bundle_adjust_workspace_bytes(int C, int64_t N, const int64_t* track_off);
+int b2_bundle_adjust_host(b2_context* ctx, int C, const double* cams, int64_t N, const double* points, const int64_t* track_off,
+                          const int32_t* meas_cam, const double* meas_uv, const b2_ba_params* params, double* cams_out,
+                          double* points_out, double* reproj_err, b2_ba_result* result, double* trace, int32_t* trial_out,
+                          int trial_cap, void* stream);
 
 /* ---- LMedS verifier (gtsfm/frontend/verifier/lmeds.py: cv2.findEssentialMat / findFundamentalMat with LMEDS) ----------
  * A batched device restatement of cv2's LMeDS estimator: cv::RNG subsets (seed 2^64 - 1, F subsets with collinear points
