@@ -186,6 +186,11 @@ class BaResult(C.Structure):  # b2_ba_result
 
 BA_KARCHER, BA_FIRST_POSE_PRIOR = 0, 1  # B2_BA_KARCHER, B2_BA_FIRST_POSE_PRIOR
 
+
+class TrParams(C.Structure):  # b2_tr_params
+    _fields_ = [("sigma", C.c_double), ("huber_k", C.c_double), ("prior_sigma", C.c_double), ("scale", C.c_double),
+                ("max_iters", C.c_int), ("pad_", C.c_int)]
+
 _vp, _i, _f, _sz = C.c_void_p, C.c_int, C.c_float, C.c_size_t
 _ip = C.POINTER(C.c_int)
 
@@ -267,6 +272,9 @@ SIGNATURES = {
     "b2_bundle_adjust_workspace_bytes": (_sz, [_i, C.c_int64, _vp]),
     "b2_bundle_adjust_host": (_i, [_vp, _i, _vp, C.c_int64, _vp, _vp, _vp, _vp, C.POINTER(BaParams), _vp, _vp, _vp, C.POINTER(BaResult),
                                    _vp, _vp, _i, _vp]),
+    "b2_translation_recovery_workspace_bytes": (_sz, [_i, _i, _i, _vp, _vp]),
+    "b2_translation_recovery_host": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp, _vp, C.POINTER(TrParams), _vp, C.POINTER(BaResult), _vp, _vp,
+                                          _i, _vp]),
     "b2_mfas_outlier_weights_host": (_i, [_vp, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp]),
     "b2_debug_viewgraph_triplets_host": (_i, [_vp, _vp, _vp, _i, C.c_int64, _vp, _vp, C.POINTER(C.c_int64), _vp]),
     "b2_twoview_ba_batched_dev": (_i, [_vp, C.POINTER(TwoViewProblem), _i, C.POINTER(TwoViewParams), C.POINTER(TwoViewResult), _vp]),

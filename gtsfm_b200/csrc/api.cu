@@ -40,6 +40,7 @@ extern "C" void b2_destroy(b2_context* ctx) {
   da_destroy(ctx);
   mf_destroy(ctx);
   gb_destroy(ctx);
+  tr_destroy(ctx);
   rt_destroy(ctx);
   nv_destroy(ctx);
   mn_destroy(ctx);
@@ -89,7 +90,7 @@ extern "C" int b2_set_option(b2_context* ctx, const char* name, int64_t value) {
     ctx->mf_workspace_mb = (int)value;
     return B2_OK;
   }
-  if (!strcmp(name, "ba_workspace_mb")) {  // bound on the device workspace of one b2_bundle_adjust_host call
+  if (!strcmp(name, "ba_workspace_mb")) {  // bound on the device workspace of one b2_bundle_adjust_host or b2_translation_recovery_host call
     if (value < 1 || value > (1 << 20)) return b2_fail(ctx, B2_ERR_ARG, "ba_workspace_mb takes 1..1048576");
     ctx->ba_workspace_mb = (int)value;
     return B2_OK;

@@ -110,6 +110,7 @@ struct ViewGraphState;
 struct DataAssocState;
 struct MfasState;
 struct GlobalBaState;
+struct TranslationRecoveryState;
 
 // Device copies of host feature arrays handed to the *_host matcher entry points.  GTSfM matches one image's (keypoints,
 // descriptors) against ~20-40 partners, always passing the same host arrays, so re-uploading 5 MB per image per pair is
@@ -134,7 +135,7 @@ struct b2_context {
   int vg_workspace_mb = 1024;  // view-graph filter: segment window of one chunk; b2_set_option "viewgraph_workspace_mb"
   int da_workspace_mb = 256;   // data association: device workspace of one chunk of tracks; "data_assoc_workspace_mb"
   int mf_workspace_mb = 1024;  // 1DSfM's MFAS: device workspace of one chunk of projection directions; "mfas_workspace_mb"
-  int ba_workspace_mb = 4096;  // global bundle adjustment: bound on one call's device workspace; "ba_workspace_mb"
+  int ba_workspace_mb = 4096;  // global BA and translation recovery: bound on one call's device workspace; "ba_workspace_mb"
   int force_simt = -1;  // 1: models loaded afterwards run the exact-fp32 SIMT kernels (no tensor cores); -1 = B2_FORCE_SIMT env
   int lg_trace = 0;     // 1: b2_lightglue_match_* record each side's state after every layer (b2_lightglue_trace_get)
   int sg_trace = 0;     // 1: b2_superglue_match_* record each side's state after every layer (b2_superglue_trace_get)
@@ -164,6 +165,7 @@ struct b2_context {
   DataAssocState* da = nullptr;
   MfasState* mf = nullptr;
   GlobalBaState* gb = nullptr;
+  TranslationRecoveryState* tr = nullptr;
   // staging shared by the *_host entry points
   DevBuf stage_d[8];
   HostBuf stage_h[4];
@@ -262,6 +264,7 @@ void vg_destroy(b2_context* ctx);
 void da_destroy(b2_context* ctx);
 void mf_destroy(b2_context* ctx);
 void gb_destroy(b2_context* ctx);
+void tr_destroy(b2_context* ctx);
 
 // shared device helpers -------------------------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

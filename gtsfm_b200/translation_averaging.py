@@ -1,26 +1,79 @@
-"""1DSfM's outlier rejection on the device.
+"""1DSfM's outlier rejection and translation recovery on the device.
 
 Drop-in for gtsfm/averaging/translation/averaging_1dsfm.py (`TranslationAveraging1DSFM`): the reference's constructor
 arguments plus `device` and `ctx`.  With GTSfM installed the class subclasses the reference's and overrides
-`compute_inliers` only, so `run_translation_averaging` (track selection, landmark directions, TranslationRecovery,
-metrics) stays the reference's own.  The projection directions come from the reference's own sampler on NumPy's global
-RNG, as in a reference run; the MFAS ordering of every direction and the per-edge sum of the outlier weights come from
-one fp64 call into libgtsfm_b200.so (`b2_mfas_outlier_weights_host`, csrc/mfas.cu).  Where gtsam breaks a tie in the
-hash order of an unordered_map, the device takes the lowest key (DESIGN.md).
+`compute_inliers` and `__run_averaging` only, so `run_translation_averaging` (track selection, landmark directions,
+metrics) stays the reference's own.
+- Outlier rejection: the projection directions come from the reference's own sampler on NumPy's global RNG, as in a
+  reference run; the MFAS ordering of every direction and the per-edge sum of the outlier weights come from one fp64 call
+  into libgtsfm_b200.so (`b2_mfas_outlier_weights_host`, csrc/mfas.cu).  Where gtsam breaks a tie in the hash order of an
+  unordered_map, the device takes the lowest key (DESIGN.md).
+- Translation recovery: gtsam's TranslationRecovery (Huber LM over one Point3 per camera and landmark) runs as one fp64
+  call (`b2_translation_recovery_host`, csrc/translation_recovery.cu).  gtsam draws the initial values from its
+  process-wide std::mt19937(42), never reseeded; this module keeps one mirror of that stream per process
+  (`reseed_translation_rng` resets it), so consecutive calls in one process continue it as gtsam's do.  Nodes joined by
+  zero translations share one value, as TranslationRecovery merges them (`merge_same_translation`).  Relative pose
+  priors (i2Ti1_priors) and problems over the "ba_workspace_mb" budget run the reference's method, logged once; such a
+  call starts gtsam's own generator where it stands, which after a device call is not where a reference run's would be
+  (DESIGN.md §3).
 
 Without GTSfM the mirror in gtsfm_api.py restates the SAMPLE_INPUT_MEASUREMENTS and SAMPLE_WITH_UNIFORM_DENSITY samplers;
-SAMPLE_WITH_INPUT_DENSITY raises ValueError and `run_translation_averaging` is unavailable.
+SAMPLE_WITH_INPUT_DENSITY raises ValueError and `run_translation_averaging` is unavailable.  `recover_translations` is the
+recovery's dict entry point, which needs no GTSfM.
 """
 from __future__ import annotations
 
-from typing import Any, Dict, Set, Tuple
+import logging
+from typing import Any, Dict, List, Optional, Set, Tuple
 
 import numpy as np
 
 from . import _lib
-from .gtsfm_api import TranslationAveraging1DSFM
+from .gtsfm_api import HAVE_GTSFM_1DSFM, TranslationAveraging1DSFM
+
+logger = logging.getLogger(__name__)
 
 OUTLIER_WEIGHT_THRESHOLD = 0.125  # averaging_1dsfm.py:52
+NOISE_MODEL_SIGMA = 0.01          # averaging_1dsfm.py:55, Isotropic.Sigma(2, 0.01) on the 3-vector error
+HUBER_LOSS_K = 1.3                # averaging_1dsfm.py:56
+PRIOR_SIGMA = 0.01                # TranslationRecovery::addPrior's priorNoiseModel, Isotropic::Sigma(3, 0.01)
+LM_MAX_ITERS = 100                # LevenbergMarquardtParams().maxIterations
+DEFAULT_WORKSPACE_MB = 4096       # b2_context's "ba_workspace_mb" default
+
+_logged_fallback = False
+
+
+class _Mt19937Uniform:
+    """std::uniform_real_distribution<double>(-1, 1) on std::mt19937, as libstdc++ draws it: two 32-bit words per value,
+    (w0 + w1 2^32) / 2^64 in double (just below 1 if it rounds to 1), mapped to 2 c - 1.  NumPy's legacy-seeded MT19937
+    emits std::mt19937's words."""
+
+    def __init__(self, seed: int):
+        self._bg = np.random.MT19937()
+        self._bg._legacy_seeding(seed)
+
+    def draws(self, n: int) -> np.ndarray:
+        w = self._bg.random_raw(2 * n).astype(np.float64).reshape(-1, 2)
+        c = (w[:, 0] + w[:, 1] * 4294967296.0) / 18446744073709551616.0
+        c = np.where(c >= 1.0, np.nextafter(1.0, 0.0), c)
+        return 2.0 * c + -1.0
+
+
+_rng: Optional[_Mt19937Uniform] = None
+
+
+def reseed_translation_rng(seed: int = 42) -> None:
+    """Restart this process's mirror of gtsam's kRandomNumberGenerator, as a fresh process would have it (tests)."""
+    global _rng
+    _rng = _Mt19937Uniform(seed)
+
+
+def random_points(n: int) -> np.ndarray:
+    """n Point3(u(), u(), u()) from the process-wide stream, (n, 3).  g++ evaluates the constructor's arguments right to
+    left, so z takes the first draw of each point."""
+    if _rng is None:
+        reseed_translation_rng()
+    return _rng.draws(3 * n).reshape(-1, 3)[:, ::-1].copy()
 
 
 def _vectors(values) -> np.ndarray:
@@ -105,6 +158,32 @@ class B200TranslationAveraging1DSFM(TranslationAveraging1DSFM):
             self._ctx = _lib.Context(self._device)
         return self._ctx
 
+    def _TranslationAveraging1DSFM__run_averaging(self, num_images: int, w_i2Ui1_dict: Dict, w_i2Ui1_dict_tracks: Dict, wRi_list: List,
+                                                  i2Ti1_priors: Dict, absolute_pose_priors: List, scale_factor: float) -> List[Optional[np.ndarray]]:
+        """The reference's __run_averaging with TranslationRecovery on the device: the translation of every camera with a
+        rotation that appears in an edge, None for the others."""
+        why = None
+        if len(i2Ti1_priors) > 0:
+            why = "relative pose priors (i2Ti1_priors)"
+        else:
+            _, _, nodes, C, L, ea, eb, _ = reduced_problem(w_i2Ui1_dict, w_i2Ui1_dict_tracks)
+            if len(ea) and not 0 < recovery_workspace_bytes(C, L, ea, eb) <= _budget_mb(self._ctx) << 20:
+                why = "a problem over the ba_workspace_mb budget"
+        if why is not None:
+            if not HAVE_GTSFM_1DSFM:
+                raise ValueError(f"{why} needs the reference's TranslationRecovery, and GTSfM is not installed")
+            global _logged_fallback
+            if not _logged_fallback:
+                logger.info("B200TranslationAveraging1DSFM: %s is not served on the device; running the reference's method", why)
+                _logged_fallback = True
+            out = super()._TranslationAveraging1DSFM__run_averaging(num_images, w_i2Ui1_dict, w_i2Ui1_dict_tracks, wRi_list,
+                                                                    i2Ti1_priors, absolute_pose_priors, scale_factor)
+            if len(i2Ti1_priors) == 0:  # gtsam drew one Point3 per solved node from its stream: keep the mirror in step
+                random_points(len(nodes))
+            return out
+        wti = recover_translations(self._context(), w_i2Ui1_dict, w_i2Ui1_dict_tracks, self._robust_measurement_noise, scale_factor)
+        return [wti[i] if wRi_list[i] is not None and i in wti else None for i in range(num_images)]
+
     def projection_directions(self, w_i2Ui1_dict: Dict, w_iUj_dict_tracks: Dict) -> np.ndarray:
         """The reference's __sample_projection_directions on its combined measurement list (consumes NumPy's global RNG
         as a reference run does): (K, 3)."""
@@ -134,3 +213,136 @@ class B200TranslationAveraging1DSFM(TranslationAveraging1DSFM):
             if f and i in inlier_cameras:  # a track measurement is kept only when its camera has an inlier camera pair
                 tracks[(j, i)] = v
         return cams, tracks, inlier_cameras
+
+
+def translation_graph(w_i2Ui1_dict: Dict, w_iUj_dict_tracks: Dict):
+    """TranslationRecovery's graph on dense node ids: camera pair (i1, i2) -> edge (C(i2), C(i1), w_i2Ui1) first, then track
+    measurement (j, i) -> (C(i), L(j), w_iUj), in the dicts' order.  -> (cameras (C,) sorted camera indices, tracks (L,)
+    sorted track ids, edge_a, edge_b (E,) int32 with cameras 0..C-1 then landmarks, meas (E, 3))."""
+    cam = np.array([(i2, i1) for (i1, i2) in w_i2Ui1_dict], np.int64).reshape(-1, 2)
+    trk = np.array([(i, j) for (j, i) in w_iUj_dict_tracks], np.int64).reshape(-1, 2)
+    cams = np.unique(np.concatenate([cam.ravel(), trk[:, 0]]))
+    tracks = np.unique(trk[:, 1])
+    if len(cams) + len(tracks) >= 2 ** 30:
+        raise ValueError("more than 2^30 nodes")
+    a = np.concatenate([np.searchsorted(cams, cam[:, 0]), np.searchsorted(cams, trk[:, 0])]).astype(np.int32)
+    b = np.concatenate([np.searchsorted(cams, cam[:, 1]), len(cams) + np.searchsorted(tracks, trk[:, 1])]).astype(np.int32)
+    meas = _vectors(list(w_i2Ui1_dict.values()) + list(w_iUj_dict_tracks.values()))
+    return cams, tracks, a, b, meas
+
+
+def initial_values(edge_a, edge_b, num_nodes: int) -> np.ndarray:
+    """initializeRandomly: a, then b, of every edge in order; each node's first appearance draws its Point3 from the
+    process-wide stream.  -> (num_nodes, 3)."""
+    order = np.stack([np.asarray(edge_a), np.asarray(edge_b)], 1).ravel()
+    first, idx = np.unique(order, return_index=True)
+    if len(first) != num_nodes:
+        raise ValueError("a node without an edge")
+    x = np.empty((num_nodes, 3))
+    x[order[np.sort(idx)]] = random_points(num_nodes)
+    return x
+
+
+def recovery_workspace_bytes(num_cameras: int, num_landmarks: int, edge_a, edge_b) -> int:
+    """b2_translation_recovery_workspace_bytes: the call's device workspace (0 for invalid input)."""
+    ea = np.ascontiguousarray(edge_a, np.int32)
+    eb = np.ascontiguousarray(edge_b, np.int32)
+    return int(_lib.load().b2_translation_recovery_workspace_bytes(int(num_cameras), int(num_landmarks), len(ea), _lib.ptr(ea), _lib.ptr(eb)))
+
+
+def recover_arrays(ctx: "_lib.Context", num_cameras: int, num_landmarks: int, edge_a, edge_b, meas, init, huber_k: float = HUBER_LOSS_K,
+                   scale: float = 1.0, sigma: float = NOISE_MODEL_SIGMA, prior_sigma: float = PRIOR_SIGMA, max_iters: int = LM_MAX_ITERS,
+                   trace: bool = False) -> dict:
+    """The device call on arrays: nodes 0..C-1 cameras, C..C+L-1 landmarks; edges (edge_a, edge_b, meas (E, 3)) in the
+    reference's order; init (C + L, 3).  huber_k 0: no robust model.  -> dict of x (C + L, 3), final_error, iterations
+    and, with `trace`, trace and trials."""
+    ea = np.ascontiguousarray(edge_a, np.int32).reshape(-1)
+    eb = np.ascontiguousarray(edge_b, np.int32).reshape(-1)
+    m = np.ascontiguousarray(meas, np.float64).reshape(-1, 3)
+    x0 = np.ascontiguousarray(init, np.float64).reshape(-1, 3)
+    C, L, E = int(num_cameras), int(num_landmarks), len(ea)
+    if len(eb) != E or len(m) != E or len(x0) != C + L:
+        raise ValueError("edge_a, edge_b, meas and init do not agree in size")
+    prm = _lib.TrParams(sigma=float(sigma), huber_k=float(huber_k), prior_sigma=float(prior_sigma), scale=float(scale),
+                        max_iters=int(max_iters))
+    out = np.empty_like(x0)
+    res = _lib.BaResult()
+    tr = np.zeros(prm.max_iters + 2) if trace else None
+    cap = 64 * (prm.max_iters + 2) if trace else 0
+    trials = np.zeros(cap, np.int32) if trace else None
+    rc = ctx.lib.b2_translation_recovery_host(ctx.handle, C, L, E, _lib.ptr(ea), _lib.ptr(eb), _lib.ptr(m), _lib.ptr(x0), _lib.C.byref(prm),
+                                              _lib.ptr(out), _lib.C.byref(res), _lib.ptr(tr), _lib.ptr(trials), cap, None)
+    ctx.check(rc, "translation_recovery")
+    d = dict(x=out, final_error=float(res.final_error), iterations=int(res.iterations))
+    if trace:
+        d["trace"] = tr[:res.trace_len].copy()
+        d["trials"] = trials[:min(res.trials, cap)].copy()
+    return d
+
+
+def _budget_mb(ctx) -> int:
+    return ctx.options.get("ba_workspace_mb", DEFAULT_WORKSPACE_MB) if ctx is not None else DEFAULT_WORKSPACE_MB
+
+
+ZERO_TRANSLATION_TOL = 1e-9  # Unit3::equals' default tolerance, against Unit3(0, 0, 0)
+
+
+def merge_same_translation(num_nodes: int, edge_a, edge_b, meas):
+    """TranslationRecovery::run's zero-translation sets: nodes joined by a measurement equal to Unit3(0, 0, 0) (every
+    component within 1e-9) share one translation; edges inside a set leave the graph, the others join the sets'
+    representatives.  -> (root (num_nodes,) each node's representative, its lowest id; keep (E,) the edges that stay)."""
+    ea, eb = np.asarray(edge_a, np.int64), np.asarray(edge_b, np.int64)
+    parent = np.arange(num_nodes)
+
+    def find(x):
+        while parent[x] != x:
+            parent[x] = parent[parent[x]]
+            x = parent[x]
+        return x
+
+    for e in np.nonzero(np.all(np.abs(np.asarray(meas).reshape(-1, 3)) <= ZERO_TRANSLATION_TOL, axis=1))[0]:
+        ra, rb = find(ea[e]), find(eb[e])
+        if ra != rb:
+            parent[max(ra, rb)] = min(ra, rb)
+    root = np.array([find(x) for x in range(num_nodes)], np.int64)
+    return root, root[ea] != root[eb]
+
+
+def reduced_problem(w_i2Ui1_dict: Dict, w_iUj_dict_tracks: Dict):
+    """The problem TranslationRecovery solves: translation_graph without the zero-translation sets' inner edges, on the
+    sets' representatives.  -> (cameras (C,), root (V,), nodes (the solved nodes, ascending, cameras first), C', L',
+    edge_a, edge_b (E',) on nodes' compact ids, meas (E', 3))."""
+    cams, tracks, ea, eb, meas = translation_graph(w_i2Ui1_dict, w_iUj_dict_tracks)
+    root, keep = merge_same_translation(len(cams) + len(tracks), ea, eb, meas)
+    a, b = root[ea[keep]], root[eb[keep]]
+    nodes = np.unique(np.concatenate([a, b]))
+    nc = int(np.sum(nodes < len(cams)))
+    return (cams, root, nodes, nc, len(nodes) - nc, np.searchsorted(nodes, a).astype(np.int32), np.searchsorted(nodes, b).astype(np.int32),
+            meas[keep])
+
+
+def recover_translations(ctx: "_lib.Context", w_i2Ui1_dict: Dict, w_iUj_dict_tracks: Dict, robust_measurement_noise: bool = True,
+                         scale_factor: float = 1.0) -> Dict[int, np.ndarray]:
+    """TranslationRecovery().run(measurements, scale_factor) on the reference's direction dicts ((i1, i2) -> w_i2Ui1 and
+    (j, i) -> w_iUj, Unit3 or 3-vectors): {camera index: its translation} for every camera of an edge.  Nodes joined by
+    zero translations share one value; with no other edge, every set sits at the origin.  Draws the initial values of
+    the solved nodes from the process-wide stream.  ValueError for a problem over the "ba_workspace_mb" budget (checked
+    before any draw) or that the device refuses."""
+    cams, root, nodes, C, L, ea, eb, meas = reduced_problem(w_i2Ui1_dict, w_iUj_dict_tracks)
+    if len(root) == 0:
+        return {}
+    x = np.full((len(root), 3), np.nan)
+    if len(ea):
+        need = recovery_workspace_bytes(C, L, ea, eb)
+        if not 0 < need <= _budget_mb(ctx) << 20:
+            raise ValueError(f"the translation recovery needs {need} bytes of device workspace, over the ba_workspace_mb budget")
+        x0 = initial_values(ea, eb, C + L)
+        try:
+            out = recover_arrays(ctx, C, L, ea, eb, meas, x0, huber_k=HUBER_LOSS_K if robust_measurement_noise else 0.0, scale=scale_factor)
+        except _lib.B200Error as e:
+            raise ValueError(str(e)) from e
+        x[nodes] = out["x"]
+    else:
+        x[np.unique(root)] = 0.0
+    x = x[root]  # a set without an edge to the solve has no value (gtsam would raise)
+    return {int(i): x[k].copy() for k, i in enumerate(cams) if np.all(np.isfinite(x[k]))}

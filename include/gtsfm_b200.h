@@ -60,8 +60,9 @@ uint64_t b2_h2d_bytes(const b2_context* ctx);
  * with more tracks than fit is cut into consecutive chunks of whole tracks, which changes no result.
  * "mfas_workspace_mb" = 1..: device workspace one chunk of directions of b2_mfas_outlier_weights_host may use (default 1024);
  * a call with more directions than fit is cut into consecutive chunks, which changes no result.
- * "ba_workspace_mb" = 1..: bound on the device workspace of one b2_bundle_adjust_host call (default 4096); a problem whose
- * workspace (b2_bundle_adjust_workspace_bytes) is larger returns B2_ERR_ARG.
+ * "ba_workspace_mb" = 1..: bound on the device workspace of one b2_bundle_adjust_host or b2_translation_recovery_host call
+ * (default 4096); a problem whose workspace (b2_bundle_adjust_workspace_bytes, b2_translation_recovery_workspace_bytes) is
+ * larger returns B2_ERR_ARG.
  * "feature_cache" = 0 | 1: drop every cached device copy of host feature arrays and (0, default) copy on every call like the
  * reference / (1) keep device copies keyed by (host pointer, size) and validated by a hash of the FULL contents, so arrays
  * edited in place are re-sent.  Only pays off for callers that pass the same numpy buffers repeatedly (it does nothing for
@@ -680,6 +681,41 @@ int b2_bundle_adjust_host(b2_context* ctx, int C, const double* cams, int64_t N,
                           const int32_t* meas_cam, const double* meas_uv, const b2_ba_params* params, double* cams_out,
                           double* points_out, double* reproj_err, b2_ba_result* result, double* trace, int32_t* trial_out,
                           int trial_cap, void* stream);
+
+/* ---- 1DSfM translation recovery (gtsfm/averaging/translation/averaging_1dsfm.py: __run_averaging, gtsam
+ * TranslationRecovery::run(measurements, scale)) ------------------------------------------------------------------------------
+ * gtsam's LevenbergMarquardtOptimizer with LevenbergMarquardtParams() defaults on the graph TranslationRecovery builds: one
+ * TranslationFactor(a, b, m) per edge (error normalize(x_b - x_a) - m, Isotropic(sigma) [Robust Huber(huber_k), reweighted on
+ * the norm of the whole whitened 3-vector]), PriorFactor<Point3>(a_0, 0, Isotropic(3, prior_sigma)) and
+ * PriorFactor<Point3>(b_0, scale m_0, the edges' model) on edge 0.  fp64 throughout; oracle/translation_recovery_ref.py is
+ * the NumPy statement.
+ * Nodes: cameras 0..C-1, then landmarks C..C+L-1; every node is an unknown Point3 and has at least one edge.  Edges HOST
+ * edge_a, edge_b [E], meas [E][3], in the reference's measurement order (edge 0 defines the gauge and the scale); an edge
+ * joins two cameras or a camera and a landmark.  init HOST [C + L][3]: the initial values (gtsam draws them from its
+ * process-wide std::mt19937; the caller mirrors that).
+ * One LM trial: linearise (one thread per edge), eliminate each landmark's damped 3 x 3 block, assemble the dense reduced
+ * camera system (3 unknowns per camera) by one CTA per camera pair over a list sorted once per call, factor it by the
+ * blocked fp64 Cholesky global BA uses, back-substitute the landmarks, and evaluate the candidate's cost and the linearised
+ * decrease; the host reads those scalars once per trial.  A damped system whose Cholesky fails is a rejected trial.  Every
+ * sum has a fixed order and there are no floating-point atomics: repeated calls return identical bits.
+ * Outputs (HOST): out [C + L][3] every node at the result, result (b2_ba_result: iterations, trials, final_error), and
+ * optionally trace [max_iters + 2] and trial_out [trial_cap], as b2_bundle_adjust_host writes them.
+ * B2_ERR_ARG before any launch: E = 0, an index outside [0, C + L), a self edge, an edge joining two landmarks, a node
+ * without an edge, a zero or non-finite measurement, a non-finite initial value, bad params, or a workspace above
+ * "ba_workspace_mb". */
+typedef struct b2_tr_params {
+  double sigma;       /* the edges' isotropic sigma (> 0; 0.01 in the reference) */
+  double huber_k;     /* the Huber threshold (1.3 in the reference); 0: no robust model */
+  double prior_sigma; /* the first-node prior's sigma (> 0; 0.01, TranslationRecovery's default) */
+  double scale;       /* scale_factor: the second prior holds b_0 at scale m_0 */
+  int max_iters;      /* maxIterations: 0..100000 (100 by default) */
+  int pad_;
+} b2_tr_params;
+/* Device workspace of a call (what "ba_workspace_mb" bounds); 0 for invalid sizes or indices. */
+size_t b2_translation_recovery_workspace_bytes(int C, int L, int E, const int32_t* edge_a, const int32_t* edge_b);
+int b2_translation_recovery_host(b2_context* ctx, int C, int L, int E, const int32_t* edge_a, const int32_t* edge_b,
+                                 const double* meas, const double* init, const b2_tr_params* params, double* out,
+                                 b2_ba_result* result, double* trace, int32_t* trial_out, int trial_cap, void* stream);
 
 /* ---- LMedS verifier (gtsfm/frontend/verifier/lmeds.py: cv2.findEssentialMat / findFundamentalMat with LMEDS) ----------
  * A batched device restatement of cv2's LMeDS estimator: cv::RNG subsets (seed 2^64 - 1, F subsets with collinear points
